@@ -101,7 +101,7 @@ _libs = {}
 
 
 def build(force: bool = False) -> Path:
-    """Compile libb200t5.so and libb200t5_f16.so for sm_100a with nvcc (cross-compiles without a GPU)."""
+    """Compile libb200t5.so and libb200t5_f16.so for sm_90a with nvcc (cross-compiles without a GPU)."""
     for path in LIB_PATHS.values():
         if force and path.exists():
             path.unlink()
@@ -120,7 +120,7 @@ def load(flavour: str = "bf16") -> C.CDLL:
     if not path.exists():
         raise RuntimeError(
             f"{path} is missing: run `make -C {CSRC}` (or __graft_entry__.build()). "
-            "There is no CPU or PyTorch fallback for the B200 path."
+            "There is no CPU or PyTorch fallback for the CUDA path."
         )
     # RTLD_LOCAL (the ctypes default): both flavours export the same names and must not see each other
     lib = C.CDLL(str(path), mode=getattr(os, "RTLD_NOW", 2))

@@ -3,10 +3,9 @@
 //
 // attention_decode.cuh reads K/V with per-thread 16-byte loads and does the arithmetic on the CUDA cores: ~54 warp
 // instructions per 512 bytes, i.e. ~60 % of an SM's issue slots at the HBM rate, and its bandwidth is proportional to
-// the warps resident per SM (it needs ~28 of them for 42 GB/s per SM). That is fine when it has the GPU to itself
-// (0.96 of the HBM peak), but the decode step overlaps it with the latency-bound split-K GEMMs of the other
-// row-chain, whose CTAs (30 K registers, ~140 KB of shared memory each) cannot co-reside with a full complement of
-// attention CTAs and take their place: in situ a 128-row launch runs at 0.73 (round 2, %globaltimer stamps).
+// the warps resident per SM. That is fine when it has the GPU to itself, but the decode step overlaps it with the
+// latency-bound split-K GEMMs of the other row-chain, whose CTAs (44 K registers, up to ~165 KB of shared memory
+// each) cannot co-reside with a full complement of attention CTAs and take their place.
 //
 // Here neither the bytes in flight nor the arithmetic depend on how many warps are resident:
 //   * one producer lane per CTA streams the K and V slabs of the CTA's (row, head) items through a ring of 8 KB
@@ -17,10 +16,8 @@
 //     as four 16-d tiles (one per warp, accumulated over the whole item in registers), the vectors q and p occupying
 //     column 0 of the B operand. ~25 warp instructions per 8 KB chunk and warp instead of ~220.
 //     The tensor pipe runs at 1/8 utilisation by construction - irrelevant for a kernel that is bound by HBM; what
-//     matters is that the issue slots are free. (First version of this kernel, same ring with the CUDA-core
-//     arithmetic of attention_decode.cuh on 2 x 4 consumer warps per SM: 0.63 of the HBM peak, issue-bound -
-//     39 % of the issue slots with 2.3 warps per scheduler; profiles/decode_r2.md. The tcgen05 formulation of round 1
-//     (0.73, profiles/xattn_tc_r1.md) paid ~80 clocks per tiny UMMA.)
+//     matters is that the issue slots are free (the CUDA-core arithmetic of attention_decode.cuh on the same ring is
+//     issue-bound).
 // Two CTAs per SM x `stages` x 8 KB are in flight whatever else is resident, the CTAs are persistent (grid sized so
 // that every CTA gets the same number of items), and their footprint (2 x ~45 KB, 2 x 160 threads) leaves room for
 // a split-K GEMM CTA of the other chain on the same SM.
@@ -83,7 +80,7 @@ DEVINL void mma_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32
 // has no memory semantics, so without a data dependency ptxas is free to schedule the arrive between the last
 // ldmatrix and the mma that waits for it (it did: LDSM, SYNCS.ARRIVE, HMMA) - the slot is then handed back while the
 // shared-memory read may still sit in the SM's memory queue, and with a GEMM CTA hammering shared memory on the same
-// SM the refill occasionally won (run-to-run different tokens, round 2; profiles/decode_r2.md section 7). The
+// SM the refill occasionally won (run-to-run different tokens). The
 // compare is never false (an mma produces the canonical NaN only), but ptxas cannot know that.
 DEVINL void xs_release_slot(uint64_t* bar, float last_acc) {
   asm volatile(
@@ -98,7 +95,7 @@ DEVINL void xs_release_slot(uint64_t* bar, float last_acc) {
 
 // tmK / tmV: [rows, 64] views (box 64 x 64 rows, 128-byte swizzle) of the K and V planes; item `it` (= (row, head),
 // chain-relative) owns rows k_row0 + it * Tk .. + Tk of tmK and v_row0 + it * Tk .. of tmV.
-// <= 64 registers: two of these CTAs (20 K registers) and one split-K GEMM CTA (192 x 160) share an SM's 64 K
+// <= 64 registers: two of these CTAs (20 K registers) and one split-K GEMM CTA (288 x 152, gemm_splitk.cuh) share an SM's 64 K
 __global__ void __maxnreg__(64)
 attn_cross_stream_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                          int k_row0, int v_row0,

@@ -1,17 +1,20 @@
 // Encoder self-attention with T5 relative-position bias and key-padding mask
 // (modeling_t5.py:253-344; bias buckets :188-251, shared across layers :755-758).
 //
-// Round-1 implementation: warp-level mma.sync (m16n8k16, bf16 -> fp32) flash-style
-// kernel that never materialises the [B,H,S,S] score tensor, but keeps HF's exact
-// (non-online) rounding contract (SURVEY Appendix A.3) by running two passes over the
-// keys: pass 1 computes the row max and sum(exp) over the bf16-rounded biased scores,
-// pass 2 recomputes the identical scores, forms p = bf16(exp(s-max)/sum) and
-// accumulates P.V in fp32. (The tcgen05/TMEM version of this kernel is the next step;
-// attention is ~4 % of the batch time at FLAN-T5-base, see DESIGN.md.)
+// Warp-level mma.sync (m16n8k16, bf16 -> fp32) flash-style kernel that never materialises
+// the [B,H,S,S] score tensor, but keeps HF's exact (non-online) rounding contract (SURVEY
+// Appendix A.3) by running two passes over the keys: pass 1 computes the row max and
+// sum(exp) over the bf16-rounded biased scores, pass 2 recomputes the identical scores,
+// forms p = bf16(exp(s-max)/sum) and accumulates P.V in fp32. Recomputing Q K^T (d = 64)
+// is cheaper than keeping a 64 x S fp32 score tile per CTA in registers or shared memory.
 //
 // qkv: [B*S, 3*I] bf16 from the fused QKV GEMM (q | k | v, head-major inside each).
 // One CTA = 4 warps = 64 query rows of one (b,h); keys are visited in chunks of 64,
-// only up to extent[b] (padded keys contribute exactly 0 after the fp32 softmax).
+// only up to extent[b] (padded keys contribute exactly 0 after the fp32 softmax). Key rows at or beyond the extent
+// are zero-filled, not loaded: in the packed layout they belong to the next prompt or were never written, and
+// p = 0 times a NaN or Inf there would still poison P.V.
+// Packed rows (cu != NULL): prompt b occupies rows cu[b] .. cu[b] + extent[b] - 1 of qkv and ctx, and only
+// those query rows are computed and written.
 #pragma once
 #include "attention_decode.cuh"
 #include "ptx.cuh"
@@ -21,6 +24,9 @@ namespace b200 {
 constexpr int kEncThreads = 128;
 constexpr int kEncQ = 64;
 constexpr int kEncKC = 64;
+// Prompts up to this length run on packed rows (the slot pool admits prompts through the packed path only,
+// modeling._POOL_MAX_S); longer ones run on all B*S rows.
+constexpr int kEncPackMaxS = 512;
 
 DEVINL void cp_async_16(uint32_t smem_dst, const void* gsrc, bool valid) {
   const int sz = valid ? 16 : 0;
@@ -71,6 +77,7 @@ encoder_attn_kernel(const act_t* __restrict__ qkv,     // [B*S, 3I]
                     const float* __restrict__ rel_bias,        // [H][2S-1], index j - i + S - 1
                     const unsigned char* __restrict__ key_ok,  // [B][S]
                     const int* __restrict__ extent,            // [B]
+                    const int* __restrict__ cu,                // packed rows: prompt b starts at row cu[b] (NULL: b * S)
                     int S, int H) {
   extern __shared__ __align__(128) uint8_t enc_smem[];
   const int I = H * 64;
@@ -89,8 +96,11 @@ encoder_attn_kernel(const act_t* __restrict__ qkv,     // [B*S, 3I]
   const uint32_t sQ_u = smem_u32(sQ), sK_u = smem_u32(sK), sV_u = smem_u32(sV);
 
   const int ext = extent[b];
+  const int rows = cu ? ext : S;  // query rows of this prompt that exist in the layout
+  if (i0 >= rows) return;
+  const size_t row0 = cu ? static_cast<size_t>(cu[b]) : static_cast<size_t>(b) * S;
   const int nchunks = (ext + kEncKC - 1) / kEncKC;
-  const act_t* qg = qkv + static_cast<size_t>(b) * S * ld + h * 64;
+  const act_t* qg = qkv + row0 * ld + h * 64;
   const act_t* kg = qg + I;
   const act_t* vg = qg + 2 * I;
 
@@ -103,8 +113,8 @@ encoder_attn_kernel(const act_t* __restrict__ qkv,     // [B*S, 3I]
     }
     for (int x = threadIdx.x; x < S; x += kEncThreads) sOk[x] = key_ok[static_cast<size_t>(b) * S + x];
   }
-  load_tile_async(sQ_u, qg, ld, i0, min(kEncQ, S - i0));
-  load_tile_async(sK_u, kg, ld, 0, min(kEncKC, S));
+  load_tile_async(sQ_u, qg, ld, i0, min(kEncQ, rows - i0));
+  load_tile_async(sK_u, kg, ld, 0, min(kEncKC, ext));
   cp_async_commit();
 
   uint32_t qa[4][4];  // Q fragments for the 4 k-steps (d = 64)
@@ -126,16 +136,16 @@ encoder_attn_kernel(const act_t* __restrict__ qkv,     // [B*S, 3I]
         l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
         l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
       }
-      load_tile_async(sK_u, kg, ld, 0, min(kEncKC, S));
-      load_tile_async(sV_u, vg, ld, 0, min(kEncKC, S));
+      load_tile_async(sK_u, kg, ld, 0, min(kEncKC, ext));
+      load_tile_async(sV_u, vg, ld, 0, min(kEncKC, ext));
       cp_async_commit();
     }
     for (int c = 0; c < nchunks; ++c) {
       const int buf = c & 1;
       if (c + 1 < nchunks) {
         const int r0 = (c + 1) * kEncKC;
-        load_tile_async(sK_u + (buf ^ 1) * 8192, kg, ld, r0, min(kEncKC, S - r0));
-        if (pass == 1) load_tile_async(sV_u + (buf ^ 1) * 8192, vg, ld, r0, min(kEncKC, S - r0));
+        load_tile_async(sK_u + (buf ^ 1) * 8192, kg, ld, r0, min(kEncKC, ext - r0));
+        if (pass == 1) load_tile_async(sV_u + (buf ^ 1) * 8192, vg, ld, r0, min(kEncKC, ext - r0));
         cp_async_commit();
         cp_async_wait<1>();
       } else {
@@ -239,8 +249,8 @@ encoder_attn_kernel(const act_t* __restrict__ qkv,     // [B*S, 3I]
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int i = i0 + row_l0 + r * 8;
-    if (i < S) {
-      act_t* dst = ctx + (static_cast<size_t>(b) * S + i) * I + h * 64 + tq * 2;
+    if (i < rows) {
+      act_t* dst = ctx + (row0 + i) * I + h * 64 + tq * 2;
 #pragma unroll
       for (int nt = 0; nt < 8; ++nt)
         *reinterpret_cast<uint32_t*>(dst + nt * 8) = pack_act2(oacc[nt][2 * r], oacc[nt][2 * r + 1]);

@@ -1,4 +1,4 @@
-// libb200t5.so - C ABI (include/b200t5.h) over the sm_100a kernels in this directory.
+// libb200t5.so - C ABI (include/b200t5.h) over the sm_90a (H100) kernels in this directory.
 // Host side: weight store + repacking, per-shape execution plans (workspace, TMA tensor
 // maps, KV arenas, the CUDA graph of one decode step), the greedy loop.
 //
@@ -23,7 +23,6 @@
 #include "attention_decode.cuh"
 #include "attention_cross_stream.cuh"
 #include "attention_encoder.cuh"
-#include "attention_encoder_tc.cuh"
 #include "elementwise.cuh"
 #include "gemm.cuh"
 #include "gemm_splitk.cuh"
@@ -207,7 +206,6 @@ struct Plan {
   // encoder workspace
   DevBuf x, xn, qkv, ctx, hff;          // [B*S, d], [B*S, d], [B*S, 3I], [B*S, I], [B*S, F]
   DevBuf key_ok, extent, enc_bias;      // uint8 [B,S], int [B], float [H][2S-1]
-  DevBuf enc_bias_packed;               // [H][q tiles][2][table_words_padded(S)] act2 words: the attention kernel's smem tables
   DevBuf cu, row_b, row_s;              // packed encoder rows: int [B+1] offsets, int [B*S] row -> (prompt, position)
   int* h_cu = nullptr;                  // pinned copy of cu[B] (number of packed rows)
   int packed_rows = 0;                  // rows the last encoder pass ran on
@@ -237,7 +235,7 @@ struct Plan {
   int* h_admit = nullptr;  // pinned: [3][B] = row_on flags, slots, rows
   int n_vtiles = 0;
   // tensor maps for activations (A operands)
-  CUtensorMap tm_xn, tm_ctx, tm_hff, tm_qkv_attn;
+  CUtensorMap tm_xn, tm_ctx, tm_hff;
   CUtensorMap tm_cross_kv;  // [Ld*2*B*H*S, 64] view of the cross-KV arena, box 64 x 64 keys (attention_cross_stream.cuh)
   // decode chains: the batch is cut into independent row ranges that run concurrently (one
   // stream each inside the step graph); every chain sees pointer-offset views of the same buffers
@@ -281,7 +279,7 @@ struct Plan {
 struct b200t5_ctx {
   Cfg c;
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   bool finalized = false;
   int ffo_k = 0;  // K extent of the feed-forward output weight as stored (F, or 2 * round_up(F, 32) in the fp16 build)
   char err[512] = "";
@@ -301,7 +299,6 @@ struct b200t5_ctx {
   bool ev_valid = false;
   int pow_mode = 0;
   bool use_pdl = true;
-  bool enc_attn_tc = true;
   GeluLut gelu_lut{nullptr, 0, 0};
   // decode GEMMs: cluster split-K tiles (gemm_splitk.cuh). {BN, wanted split} per product;
   // B200T5_SK=0 selects the persistent kernel instead, B200T5_SK="bn,s,bn,s,bn,s,bn,s" overrides
@@ -310,28 +307,26 @@ struct b200t5_ctx {
     int bn, split;
   };
   bool pack_rows = true;  // encoder on the valid rows only (variable-length packing); B200T5_PACK=0: all B*S rows as the reference does
-  bool use_2cta = true;   // encoder GEMMs on CTA pairs (gemm_2cta.cuh); B200T5_2CTA=0 selects the single-CTA kernel
+  bool use_2cta = true;   // encoder GEMMs on the 128 x 256 tile configuration (gemm_2cta.cuh); B200T5_2CTA=0 selects the G_*256 kernels
   bool self_block = true;  // decoder self-attention with a 4-warp CTA per (row, head): two memory round trips whatever t is
-                           // (measured: decode 201.5 -> 188.3 ms per batch); B200T5_SELF=warp selects one warp per (row, head)
+                           // B200T5_SELF=warp selects one warp per (row, head)
   // Cross-attention of the decode step: the TMA-ring + mma.sync stream kernel (attention_cross_stream.cuh: small
-  // footprint, shares the SMs with the other chain's GEMM CTAs; the faster step when every prompt fills the window:
-  // decode 187.6 vs 191.0 ms at 512 keys per row, the layer's K/V stream at 0.92 vs 0.84 of the HBM peak in situ) or the
-  // per-thread-load kernel (attention_decode.cuh: one short-lived CTA per (row, head), seven per SM; the faster one on
-  // ragged prompts: 148.3 vs 165.7 ms at uniform lengths, 117.8 vs 123.4 at alpaca-like ones). 2 = choose per call from
+  // footprint, shares the SMs with the other chain's GEMM CTAs; meant for batches whose prompts fill the window) or the
+  // per-thread-load kernel (attention_decode.cuh: one short-lived CTA per (row, head), several per SM; meant for
+  // ragged prompts). 2 = choose per call from
   // the batch's fill (valid prompt tokens / B*S >= kXattnStreamFill -> stream); B200T5_XATTN=ldg|stream|auto, option
   // "xattn" 0|1|2. The kernels differ only in the order of their fp32 accumulations (same tokens up to near-ties).
   int xattn_mode = 2;
   int xs_stages = 5;        // 8 KB ring stages per CTA (two CTAs per SM): B200T5_XS_STAGES
   bool xs_late_pdl = true;  // release the dependent GEMM when a CTA starts its last item instead of at once: B200T5_XS_LATE_PDL
-  bool xs_l2_prefetch = false;   // drive HBM -> L2 one item ahead with bulk L2 prefetches (B200T5_XS_L2PF, "xattn_l2pf"): measured SLOWER
-                                 // (alone 0.71 instead of 0.82 of the HBM peak, decode 235 instead of 203 ms: profiles/decode_r2.md)
+  bool xs_l2_prefetch = false;   // drive HBM -> L2 one item ahead with bulk L2 prefetches (B200T5_XS_L2PF, "xattn_l2pf")
   bool xattn_serialize = false;  // one cross-attention kernel at a time across the chains (B200T5_XS_SERIALIZE, "xattn_serialize")
   std::vector<cudaEvent_t> xattn_ev;
   bool profile_xattn = false;  // b200t5_set_option("profile_xattn"): stamp every cross-attention launch inside the step graph
   int small_prio = 0;  // B200T5_PRIO: launch priority of the latency-bound decode kernels (see launch_priority())
   bool sk_on = true;
   int sk_stages64 = 0, sk_stages128 = 0;  // pipeline stages of the split-K tiles (0 = default 4 / 3): B200T5_SK_STAGES="a,b"
-  SkChoice sk_qkv{64, 2}, sk_proj{64, 4}, sk_wi{128, 2}, sk_ffo{64, 4};  // best of the B200 sweep (tools/sweep_decode.sh)
+  SkChoice sk_qkv{64, 2}, sk_proj{64, 4}, sk_wi{128, 2}, sk_ffo{64, 4};  // split-K choices per product (tools/sweep_decode.py)
   int chains_override = 0;
   cudaStream_t chain_streams[kMaxChains] = {};
   cudaEvent_t chain_ev[kMaxChains + 1] = {};
@@ -361,8 +356,8 @@ static int check_device(b200t5_ctx* h, int device) {
   if (device < 0 || device >= n) return fail(h, B200T5_EINVAL, "device %d out of range (%d devices)", device, n);
   cudaDeviceProp p;
   CU_OK(h, cudaGetDeviceProperties(&p, device));
-  if (p.major != 10)
-    return fail(h, B200T5_ENODEV, "device %d is sm_%d%d; libb200t5 is built for sm_100a only", device, p.major, p.minor);
+  if (p.major != 9)
+    return fail(h, B200T5_ENODEV, "device %d is sm_%d%d; libb200t5 is built for sm_90a only", device, p.major, p.minor);
   CU_OK(h, cudaSetDevice(device));
   return p.multiProcessorCount;
 }
@@ -416,7 +411,7 @@ static cudaError_t run_gemm(b200t5_ctx* h, const GemmOp& g, const void* ep, cuda
   return cudaErrorInvalidValue;
 }
 
-// CTA-pair GEMM (encoder, 256 x 256 tiles)
+// encoder GEMM, 128 x 256 tiles (gemm_2cta.cuh)
 template <class Epi>
 static cudaError_t run_gemm_2cta(b200t5_ctx* h, const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K,
                                  const typename Epi::Params& ep, cudaStream_t s) {
@@ -486,9 +481,6 @@ static cudaError_t init_kernel_attrs() {
   if ((e = cudaFuncSetAttribute(self_attn_decode_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 kSelfWarpsPerCta * 4096 * 4)) != cudaSuccess)
     return e;
-  if ((e = cudaFuncSetAttribute(encoder_attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                static_cast<int>(EncTcSmem::bytes(kEncTcMaxS)))) != cudaSuccess)
-    return e;
   if ((e = cudaFuncSetAttribute(attn_cross_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 static_cast<int>(XsSmem::bytes(kXsMaxStages, 4096)))) != cudaSuccess)
     return e;
@@ -545,7 +537,7 @@ static GeluLutOwner g_gelu;  // one process drives one GPU
 
 // ================================================================== lifecycle
 extern "C" const char* b200t5_version(void) {
-  return B200T5_F16 ? "b200t5 0.1 fp16 (sm_100a, tcgen05/TMA)" : "b200t5 0.1 (sm_100a, tcgen05/TMA)";
+  return B200T5_F16 ? "b200t5 0.1 fp16 (sm_90a, wgmma/TMA)" : "b200t5 0.1 (sm_90a, wgmma/TMA)";
 }
 extern "C" const char* b200t5_last_global_error(void) { return g_err; }
 extern "C" const char* b200t5_last_error(b200t5_handle h) { return h ? h->err : g_err; }
@@ -574,8 +566,6 @@ extern "C" int b200t5_create(const b200t5_config* cfg, int device, b200t5_handle
   h->pow_mode = pm ? atoi(pm) : 0;
   const char* pdl_env = getenv("B200T5_PDL");
   h->use_pdl = pdl_env ? atoi(pdl_env) != 0 : true;
-  const char* ea_env = getenv("B200T5_ENC_ATTN");
-  h->enc_attn_tc = !(ea_env && strcmp(ea_env, "mma") == 0);
   if (const char* pr_env = getenv("B200T5_PRIO")) h->small_prio = atoi(pr_env);
   if (const char* pk_env = getenv("B200T5_PACK")) h->pack_rows = atoi(pk_env) != 0;
   if (const char* tc_env = getenv("B200T5_2CTA")) h->use_2cta = atoi(tc_env) != 0;
@@ -612,7 +602,7 @@ extern "C" int b200t5_create(const b200t5_config* cfg, int device, b200t5_handle
 #if B200T5_F16
   // the fp16 build implements the default kernel set only (the measured-slower experiments and the fallbacks
   // they replace assume the bf16 contract: 2-byte residual stream, table-driven gelu)
-  h->use_2cta = h->pack_rows = h->enc_attn_tc = true;
+  h->use_2cta = h->pack_rows = true;
   if (!h->sk_on) {
     delete h;
     return fail(nullptr, B200T5_EINVAL, "B200T5_SK=0 is not available in the fp16 build");
@@ -1000,35 +990,6 @@ static int build_plan(b200t5_ctx* h, int B, int S, int Tmax) {
     }
     CU_OK(h, pl->enc_bias.alloc(eb.size() * 4));
     CU_OK(h, cudaMemcpy(pl->enc_bias.p, eb.data(), eb.size() * 4, cudaMemcpyHostToDevice));
-    if (S <= kEncTcMaxS) {
-      // The attention kernel's two packed tables per (head, 128-query tile): T0[k] = (bias[2k], bias[2k+1]),
-      // T1[k] = (bias[2k+1], bias[2k+2]) with bias[x] = rel_bias[h][S - 1 - i0 - 127 + x] (0 outside), exactly
-      // what the kernel used to build per CTA (attention_encoder_tc.cuh, bias_at).
-      const int tw = EncTcSmem::table_words_padded(S), ntiles = (S + kEncTcQ - 1) / kEncTcQ;
-      std::vector<uint32_t> pk(static_cast<size_t>(H) * ntiles * 2 * tw, 0u);
-      auto bits = [](float v) -> uint32_t {
-        const act_t a = B200T5_F16 ? act_t(__float2half_rn(v)) : act_t(__float2bfloat16_rn(v));
-        uint16_t u;
-        memcpy(&u, &a, 2);
-        return u;
-      };
-      for (int hh = 0; hh < H; ++hh)
-        for (int ti = 0; ti < ntiles; ++ti) {
-          const int lo = S - 1 - ti * kEncTcQ - 127;
-          auto at = [&](int x) -> float {
-            const int idx = lo + x;
-            return (x < S + 127 && idx >= 0 && idx < 2 * S - 1) ? eb[static_cast<size_t>(hh) * (2 * S - 1) + idx] : 0.f;
-          };
-          uint32_t* t0 = pk.data() + (static_cast<size_t>(hh) * ntiles + ti) * 2 * tw;
-          uint32_t* t1 = t0 + tw;
-          for (int k = 0; k < (S + 128) / 2; ++k) {
-            t0[k] = bits(at(2 * k)) | (bits(at(2 * k + 1)) << 16);
-            t1[k] = bits(at(2 * k + 1)) | (bits(at(2 * k + 2)) << 16);
-          }
-        }
-      CU_OK(h, pl->enc_bias_packed.alloc(pk.size() * 4));
-      CU_OK(h, cudaMemcpy(pl->enc_bias_packed.p, pk.data(), pk.size() * 4, cudaMemcpyHostToDevice));
-    }
     std::vector<float> db(static_cast<size_t>(H) * Tmax);
     for (int n = 0; n < Tmax; ++n) {
       const int bk = b200t5_relative_bucket(-n, 0, c.nb, c.maxdist);
@@ -1040,13 +1001,11 @@ static int build_plan(b200t5_ctx* h, int B, int S, int Tmax) {
   TMAP(h, &pl->tm_xn, pl->xn.p, M, d, 128);
   TMAP(h, &pl->tm_ctx, pl->ctx.p, M, I, 128);
   TMAP_FFO(h, &pl->tm_hff, pl->hff.p, M, F, 128);
-  TMAP(h, &pl->tm_qkv_attn, pl->qkv.p, M, 3 * I, 128);
   TMAP(h, &pl->tm_cross_kv, pl->cross_kv.p, static_cast<uint64_t>(c.Ld) * 2 * B * H * S, 64, kXsChunkKeys);
   CU_OK(h, cudaMemset(pl->ctx.p, 0, pl->ctx.bytes));  // padded query tiles are skipped: keep them finite
   {
     // chains of 128 rows (one M-tile per split-K GEMM): two for a 256-row batch, four for the slot pool's 512 rows
-    // (measured, natural EOS, 4096 full-length prompts: 138.8 k tok/s with four chains, 133.4 k with two; three: 123.9 k -
-    // uneven M-tiles; profiles/stream_r2_chains.log); B200T5_CHAINS overrides
+    // (three would give uneven M-tiles); B200T5_CHAINS overrides
     int nc = B >= 512 ? 4 : (B >= 128 ? 2 : 1);
     if (h->chains_override > 0) nc = h->chains_override;
     if (nc > kMaxChains) nc = kMaxChains;
@@ -1094,9 +1053,9 @@ static int run_encoder(b200t5_ctx* h, const long long* ids, const long long* mas
   h->launches++;
   // Variable-length packing: only rows below extent[b] are ever read downstream, so the encoder runs on those
   // (elementwise.cuh). The number of packed rows sizes the GEMM grids, hence one 4-byte read-back per call.
-  p.packed = h->pack_rows && h->enc_attn_tc && S <= kEncTcMaxS;
+  p.packed = h->pack_rows && S <= kEncPackMaxS;
   if (row_on && !p.packed)
-    return fail(h, B200T5_EINVAL, "slot-pool admission needs the packed encoder path (S <= %d, B200T5_PACK/B200T5_ENC_ATTN at their defaults)", kEncTcMaxS);
+    return fail(h, B200T5_EINVAL, "slot-pool admission needs the packed encoder path (S <= %d, B200T5_PACK at its default)", kEncPackMaxS);
   const int* cu = nullptr;
   p.rows_valid = M;
   if (p.packed) {
@@ -1118,13 +1077,6 @@ static int run_encoder(b200t5_ctx* h, const long long* ids, const long long* mas
   const size_t attn_smem = encoder_attn_smem_bytes(S);
   if (attn_smem > 96 * 1024) return fail(h, B200T5_EINVAL, "encoder length S=%d too long for the attention kernel", S);
   const int wi_tiles = (F + 127) / 128;
-  // diagnostic (B200T5_ENC_PROF=1): phase timeline of the first CTA of layer 0's attention kernel
-  std::unique_ptr<DevBuf> enc_prof;
-  if (getenv("B200T5_ENC_PROF")) {
-    enc_prof.reset(new DevBuf());
-    CU_OK(h, enc_prof->alloc(64));
-    CU_OK(h, cudaMemsetAsync(enc_prof->p, 0, 64, s));
-  }
   for (int l = 0; l < c.Le; ++l) {
     EncLayerW& w = h->enc[l];
     CU_OK(h, run_rmsnorm(h, p.x.as<res_t>(), w.ln0.as<act_t>(), p.xn.as<act_t>(), M, d, c.eps, s));
@@ -1133,14 +1085,8 @@ static int run_encoder(b200t5_ctx* h, const long long* ids, const long long* mas
       if (h->use_2cta) CU_OK(h, run_gemm_2cta<EpiStore>(h, p.tm_xn, w.tm2_qkv, M, 3 * I, d, ep, s));
       else CU_OK(h, run_gemm(h, mk(p.tm_xn, w.tm_qkv, M, 3 * I, d, G_STORE256, 0), &ep, s));
     }
-    if (h->enc_attn_tc && S <= kEncTcMaxS) {
-      encoder_attn_tc_kernel<<<dim3(B * H), kEncTcThreads, EncTcSmem::bytes(S), s>>>(
-          p.tm_qkv_attn, p.ctx.as<act_t>(), p.enc_bias.as<float>(), p.key_ok.as<unsigned char>(), p.extent.as<int>(), cu, S, H,
-          enc_prof && l == 0 ? enc_prof->as<long long>() : nullptr, p.enc_bias_packed.as<uint32_t>());
-    } else {
-      encoder_attn_kernel<<<dim3((S + kEncQ - 1) / kEncQ, B * H), kEncThreads, attn_smem, s>>>(
-          p.qkv.as<act_t>(), p.ctx.as<act_t>(), p.enc_bias.as<float>(), p.key_ok.as<unsigned char>(), p.extent.as<int>(), S, H);
-    }
+    encoder_attn_kernel<<<dim3((S + kEncQ - 1) / kEncQ, B * H), kEncThreads, attn_smem, s>>>(
+        p.qkv.as<act_t>(), p.ctx.as<act_t>(), p.enc_bias.as<float>(), p.key_ok.as<unsigned char>(), p.extent.as<int>(), cu, S, H);
     h->launches++;
     CU_OK(h, cudaGetLastError());
     {
@@ -1164,14 +1110,6 @@ static int run_encoder(b200t5_ctx* h, const long long* ids, const long long* mas
     }
   }
   CU_OK(h, run_rmsnorm(h, p.x.as<res_t>(), h->enc_final_ln.as<act_t>(), p.xn.as<act_t>(), M, d, c.eps, s));
-  if (enc_prof) {
-    long long st[8];
-    CU_OK(h, cudaStreamSynchronize(s));
-    CU_OK(h, cudaMemcpy(st, enc_prof->p, 64, cudaMemcpyDeviceToHost));
-    fprintf(stderr, "ENC_PROF (SM clocks, CTA 0 of layer 0's attention; prologue, loads+QK^T, pass A, pass B, pass C, P.V tail, store):");
-    for (int i = 1; i < 8; ++i) fprintf(stderr, " %lld", st[i] - st[i - 1]);
-    fprintf(stderr, " | total %lld\n", st[7] - st[0]);
-  }
   return B200T5_OK;
 }
 
@@ -1983,7 +1921,7 @@ extern "C" int b200t5_test_gemm(int device, const void* A, const void* W, void* 
   dummy.num_sms = sms;
   cudaError_t e = cudaErrorInvalidValue;
   act_t* Cb = static_cast<act_t*>(C);
-  if (bn == 512) {  // CTA-pair kernel, 256 x 256 tiles (gemm_2cta.cuh)
+  if (bn == 512) {  // the encoder configuration: 128 x 256 tiles, weight loaded in 128-row boxes (gemm_2cta.cuh)
     if (mode == 0) {
       EpiStore::Params ep{Cb, N};
       e = run_gemm_2cta<EpiStore>(&dummy, ta, tb, M, N, K, ep, s);
@@ -2107,7 +2045,7 @@ extern "C" int b200t5_test_gemm_splitk(int device, const void* A, const void* W,
 }
 
 // fp16 build only: the fp32-weight feed-forward output projection, R += A . W^T, through the tf32 two-pass product
-// (A [M,F] fp32 holding fp16 values, W [N,F] fp32, R [M,N] fp32 in/out). kernel 0: CTA-pair encoder kernel,
+// (A [M,F] fp32 holding fp16 values, W [N,F] fp32, R [M,N] fp32 in/out). kernel 0: the encoder GEMM (gemm_2cta.cuh),
 // 1: cluster split-K decode kernel (bn in {64,128}, split in {1,2,4,8}).
 extern "C" int b200t5_test_ffo(int device, const void* A, const void* W, void* R, int M, int N, int F, int kernel, int bn,
                                int split, void* stream) {
@@ -2203,21 +2141,19 @@ extern "C" int b200t5_test_encoder_attn(int device, const void* qkv, void* ctx, 
 #else
   const int sms = hook_device(device);
   if (sms < 0) return sms;
+  // impl 1: the packed-row addressing the encoder uses (prompt b at rows cu[b] = b * S, only its extent computed)
+  DevBuf cu;
   if (impl == 1) {
-    if (S > kEncTcMaxS) return fail(nullptr, B200T5_EINVAL, "tcgen05 encoder attention supports S <= %d", kEncTcMaxS);
-    CUtensorMap tm;
-    if (!make_tmap(&tm, qkv, static_cast<uint64_t>(B) * S, static_cast<uint64_t>(3) * H * 64, 128)) return fail(nullptr, B200T5_ECUDA, "%s", g_err);
-    encoder_attn_tc_kernel<<<dim3(B * H), kEncTcThreads, EncTcSmem::bytes(S), static_cast<cudaStream_t>(stream)>>>(
-        tm, static_cast<act_t*>(ctx), rel_bias, key_ok, extent, nullptr, S, H);
-    cudaError_t e2 = cudaGetLastError();
-    if (e2 != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "encoder_attn_tc: %s", cudaGetErrorString(e2));
-    return B200T5_OK;
+    std::vector<int> hcu(B);
+    for (int b = 0; b < B; ++b) hcu[b] = b * S;
+    if (cu.alloc(B * sizeof(int)) != cudaSuccess || cudaMemcpy(cu.p, hcu.data(), B * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess)
+      return fail(nullptr, B200T5_ECUDA, "encoder_attn: offsets");
   }
   const size_t smem = encoder_attn_smem_bytes(S);
   cudaError_t e = smem <= 96 * 1024 ? cudaSuccess : cudaErrorInvalidValue;
   if (e == cudaSuccess) {
     encoder_attn_kernel<<<dim3((S + kEncQ - 1) / kEncQ, B * H), kEncThreads, smem, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const act_t*>(qkv), static_cast<act_t*>(ctx), rel_bias, key_ok, extent, S, H);
+        static_cast<const act_t*>(qkv), static_cast<act_t*>(ctx), rel_bias, key_ok, extent, impl == 1 ? cu.as<int>() : nullptr, S, H);
     e = cudaGetLastError();
   }
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "encoder_attn: %s", cudaGetErrorString(e));

@@ -1,11 +1,13 @@
-// Persistent warp-specialised bf16 GEMM for sm_100a:
+// Persistent warp-specialised bf16 GEMM for sm_90a (H100):
 //   D[M,N] = A[M,K] * W[N,K]^T      (both operands K-major, i.e. nn.Linear layout)
-// TMA (128-B swizzle) -> smem ring -> tcgen05.mma (one elected thread) -> fp32
-// accumulators double-buffered in TMEM -> epilogue warps (tcgen05.ld) apply a
-// fused epilogue functor and write HBM directly.
+// TMA (128-B swizzle) -> smem ring -> wgmma (two consumer warpgroups, 64 tile rows each, fp32 accumulators in
+// registers) -> accumulators staged as fp32 rows in shared memory -> the epilogue functor reads 32-column chunks of
+// one row per thread, applies the fused epilogue and writes HBM directly.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer,
-// warps 2..5 = epilogue (warp w owns TMEM lanes 32*(w%4)..+31 = tile rows).
+// Warp roles (288 threads): warps 0..7 = two consumer warpgroups (MMA, then epilogue), warp 8 = TMA producer.
+// The staging tile aliases the pipeline ring: it is written once both warpgroups' MMAs of the tile have completed,
+// and the producer starts the next tile's loads once every epilogue thread has read its rows. Tiles with BN <= 128
+// keep a CTA near 100 KB so that two CTAs share an SM and one's epilogue overlaps the other's main loop.
 //
 // The epilogue functors are where the T5 rounding contract lives: HF eager bf16
 // rounds every Linear output to bf16 before anything else touches it
@@ -19,8 +21,8 @@ namespace b200 {
 
 constexpr int kBM = 128;
 constexpr int kBK = 64;
-constexpr int kGemmThreads = 192;      // 2 control warps + 4 epilogue warps
-constexpr int kGemmThreadsWide = 320;  // 2 control warps + 8 epilogue warps (big tiles: the epilogue is the bottleneck)
+constexpr int kGemmThreads = 288;     // 2 consumer warpgroups + 1 producer warp
+constexpr int kGemmConsumers = 256;
 constexpr int kEpiSmemBytes = 8192;  // per-CTA scratch the epilogue functor may stage tables in
 
 template <int BN>
@@ -29,12 +31,13 @@ struct GemmCfg {
   static constexpr int kABytes = kBM * kBK * 2;
   static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  // Big tiles (encoder, M = B*S) take the whole SM; the small-N decode tiles keep <= ~100 KB so that
-  // two CTAs of concurrently running decode chains can share an SM.
-  static constexpr int kStagesRaw = (196 * 1024) / kStageBytes;
-  static constexpr int kStages = BN <= 64 ? ((100 * 1024) / kStageBytes) : (kStagesRaw > 8 ? 8 : kStagesRaw);
-  static constexpr int kTmemCols = (2 * BN) < 32 ? 32 : 2 * BN;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/ + kEpiSmemBytes;
+  static constexpr int kStages = BN >= 256 ? 4 : (96 * 1024) / kStageBytes;
+  static constexpr int kRingBytes = kStages * kStageBytes;
+  static constexpr int kStageLd = BN + 4;  // floats per staged row; +4 keeps a warp's per-row 16-B reads conflict-free
+  static constexpr int kStagingBytes = kBM * kStageLd * 4;
+  static_assert(kStagingBytes <= kRingBytes, "the staged tile aliases the ring");
+  static constexpr int kSmemBytes = kRingBytes + 1024 /*align*/ + 256 /*barriers*/ + kEpiSmemBytes;
+  static constexpr int kCtasPerSm = BN <= 128 ? 2 : 1;
 };
 
 struct TileCoord {
@@ -52,78 +55,90 @@ DEVINL TileCoord tile_coord(int tile, int tiles_m, int tiles_n, int m_fastest) {
   return c;
 }
 
-// Epilogue warps: a warp may only touch the TMEM lane quarter 32*(warp%4), so 4 warps cover a tile's
-// 128 rows; the big tiles (BN = 256) run 8 epilogue warps - two per lane quarter, each taking half of
-// the tile's 32-column chunks - because with 4 the epilogue (not the MMA) bounds the kernel: measured
-// on B200, tensor pipe active 27 % for the GeGLU tile and 34 % for the K = 768 residual tile
-// (profiles/encoder_ncu_r1.md).
-template <int BN>
-struct EpiWarps {
-  static constexpr int kCount = BN >= 256 ? 8 : 4;
-  static constexpr int kThreads = 64 + 32 * kCount;
-};
+DEVINL void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kGemmConsumers) : "memory"); }
 
-template <int BN, class Epi>
-__global__ void __launch_bounds__(EpiWarps<BN>::kThreads, (BN <= 64 ? 2 : 1))
+// One k-block (128 B of K per row) of this warpgroup's 64 x BN product: 4 wgmma of 32 B each.
+template <int BN, bool kTf32>
+DEVINL void wgmma_kblock(float (&acc)[BN / 2], uint32_t a_addr, uint32_t b_addr) {
+  const uint64_t a_desc = make_desc_sw128_kmajor(a_addr);
+  const uint64_t b_desc = make_desc_sw128_kmajor(b_addr);
+#pragma unroll
+  for (int k = 0; k < kBK / 16; ++k) wgmma_k32B<BN, kTf32>(acc, a_desc + 2 * k, b_desc + 2 * k);
+}
+
+// Writes a warpgroup's wgmma accumulators (rows row0 .. row0+63 of the tile) into the fp32 staging rows.
+template <int BN>
+DEVINL void stage_acc(float* stg, int row0, const float (&acc)[BN / 2]) {
+  const int t = threadIdx.x & 127;
+  const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2);
+  const int c = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    *reinterpret_cast<float2*>(stg + r * GemmCfg<BN>::kStageLd + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2*>(stg + (r + 8) * GemmCfg<BN>::kStageLd + 8 * j + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+  }
+}
+
+// kTf32 / a_kblocks: fp32 operands consumed as tf32 (the fp16 build's fp32-weight `wo` product): a k-block is 32
+// elements (the same 128-byte rows), K counts the columns of W' = [W_hi | W_lo], and A has only a_kblocks k-blocks
+// and is walked twice (kb % a_kblocks), so the accumulator receives A . W_hi^T + A . W_lo^T.
+// kBBox: rows per TMA box of the weight tensor map (the weight tile is loaded in BN / kBBox boxes).
+template <int BN, class Epi, bool kTf32 = false, int kBBox = BN>
+__global__ void __launch_bounds__(kGemmThreads, GemmCfg<BN>::kCtasPerSm)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N,
-                    int K, int m_fastest, typename Epi::Params ep) {
+                    int K, int m_fastest, typename Epi::Params ep, int a_kblocks) {
   using Cfg = GemmCfg<BN>;
+  static_assert(BN % kBBox == 0, "box");
+  constexpr int kbk = kTf32 ? kBK / 2 : kBK;  // elements per k-block (128 bytes)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kRingBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::kStages;
-  uint64_t* tfull = bars + 2 * Cfg::kStages;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  uint8_t* epi_smem = smem + Cfg::kStages * Cfg::kStageBytes + 256;
+  uint64_t* stg_free = bars + 2 * Cfg::kStages;  // every epilogue thread has read the staged tile
+  uint8_t* epi_smem = smem + Cfg::kRingBytes + 256;
+  float* stg = reinterpret_cast<float*>(smem);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int tiles_m = (M + kBM - 1) / kBM;
   const int tiles_n = (N + BN - 1) / BN;
   const int num_tiles = tiles_m * tiles_n;
-  const int kblocks = (K + kBK - 1) / kBK;
+  const int kblocks = (K + kbk - 1) / kbk;
+  if (a_kblocks <= 0) a_kblocks = kblocks;
 
   pdl_launch_dependents();
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < Cfg::kStages; ++i) {
-        mbar_init(&full[i], 1);
-        mbar_init(&empty[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&tfull[i], 1);
-        mbar_init(&tempty[i], EpiWarps<BN>::kCount);
-      }
-      mbar_fence_init();
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < Cfg::kStages; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 2);  // one arrival per consumer warpgroup
     }
-    __syncwarp();
-    tmem_alloc<Cfg::kTmemCols>(tmem_slot);
+    mbar_init(stg_free, kGemmConsumers);
+    mbar_fence_init();
   }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
   // PDL: everything above overlapped the previous kernel's tail. Each role waits for the previous
   // kernel (griddepcontrol.wait) only right before it first touches memory that kernel may have
   // written; the weights (B operand) never depend on it and are prefetched into L2 before the wait.
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ------------------------------------------------------------ TMA producer
     if (lane == 0) {
+      tma_prefetch_desc(&tmA);
+      tma_prefetch_desc(&tmB);
       if (static_cast<int>(blockIdx.x) < num_tiles) {
         const TileCoord tc0 = tile_coord(blockIdx.x, tiles_m, tiles_n, m_fastest);
-        for (int kb = 0; kb < kblocks; ++kb) tma_prefetch_l2_2d(&tmB, kb * kBK, tc0.n_tile * BN);
+        for (int kb = 0; kb < kblocks; ++kb)
+          for (int p = 0; p < BN / kBBox; ++p) tma_prefetch_l2_2d(&tmB, kb * kbk, tc0.n_tile * BN + p * kBBox);
       }
       pdl_wait();
       int stage = 0;
-      uint32_t phase = 0;
+      uint32_t phase = 0, sphase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        if (tile != static_cast<int>(blockIdx.x)) {
+          mbar_wait(stg_free, sphase);  // the previous tile's staged accumulators (aliasing the ring) have been read
+          sphase ^= 1u;
+        }
         const TileCoord tc = tile_coord(tile, tiles_m, tiles_n, m_fastest);
         const int m0 = tc.m_tile * kBM, n0 = tc.n_tile * BN;
         for (int kb = 0; kb < kblocks; ++kb) {
@@ -131,77 +146,59 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           uint8_t* sA = smem + stage * Cfg::kStageBytes;
           uint8_t* sB = sA + Cfg::kABytes;
           mbar_arrive_expect_tx(&full[stage], Cfg::kStageBytes);
-          tma_load_2d(sA, &tmA, &full[stage], kb * kBK, m0);
-          tma_load_2d(sB, &tmB, &full[stage], kb * kBK, n0);
-          if (++stage == Cfg::kStages) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_act(kBM, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty[as], aphase ^ 1u);
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(as * BN);
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after_sync();
-          const uint32_t a_addr = smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint64_t a_desc = make_desc_sw128_kmajor(a_addr);
-          const uint64_t b_desc = make_desc_sw128_kmajor(a_addr + Cfg::kABytes);
+          tma_load_2d(sA, &tmA, &full[stage], (kb % a_kblocks) * kbk, m0);
 #pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {
-            // advance 16 bf16 = 32 B along K inside the 128-B swizzle row: +2 in the (addr>>4) field
-            umma_f16_ss(d_tmem, a_desc + static_cast<uint64_t>(2 * k), b_desc + static_cast<uint64_t>(2 * k), idesc,
-                         (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty[stage]);
+          for (int p = 0; p < BN / kBBox; ++p) tma_load_2d(sB + p * kBBox * 128, &tmB, &full[stage], kb * kbk, n0 + p * kBBox);
           if (++stage == Cfg::kStages) {
             stage = 0;
             phase ^= 1u;
           }
         }
-        umma_commit(&tfull[as]);
-        as ^= 1;
-        if (as == 0) aphase ^= 1u;
       }
     }
   } else {
-    // ------------------------------------------------------------ epilogue warps
-    const int q = warp & 3;
-    constexpr int kParts = EpiWarps<BN>::kCount / 4;  // column parts of a tile row
-    const int part = (warp - 2) >> 2;
-    int as = 0;
-    uint32_t aphase = 0;
-    Epi::prologue(ep, epi_smem, static_cast<int>(threadIdx.x) - 64, 32 * EpiWarps<BN>::kCount);  // constant tables; overlaps the main loop
+    // ------------------------------------------------------------ consumer warpgroups
+    const int wg = warp >> 2;
+    const int et = threadIdx.x;  // 0..255
+    Epi::prologue(ep, epi_smem, et, kGemmConsumers);  // constant tables; overlaps the main loop
     pdl_wait();
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const TileCoord tc = tile_coord(tile, tiles_m, tiles_n, m_fastest);
-      const int m = tc.m_tile * kBM + q * 32 + lane;
-      mbar_wait(&tfull[as], aphase);
-      tc_fence_after_sync();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(as * BN);
-      Epi::template run<BN>(ep, taddr, m, m < M, tc.n_tile, N, epi_smem, part, kParts);
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[as]);
-      as ^= 1;
-      if (as == 0) aphase ^= 1u;
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < kblocks; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t a_addr = smem_u32(smem + stage * Cfg::kStageBytes) + wg * 64 * 128;
+        wgmma_fence_acc(acc);
+        wgmma_fence();
+        wgmma_kblock<BN, kTf32>(acc, a_addr, smem_u32(smem + stage * Cfg::kStageBytes + Cfg::kABytes));
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs are done: hand its stage back to the producer
+        wgmma_fence_acc(acc);
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == Cfg::kStages) {
+          stage = 0;
+          phase ^= 1u;
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+      // both warpgroups' MMAs are complete before the staging rows overwrite the ring
+      consumers_sync();
+      stage_acc<BN>(stg, wg * 64, acc);
+      consumers_sync();
+      const int row = et & (kBM - 1), part = et >> 7;
+      const int m = tc.m_tile * kBM + row;
+      const uint32_t waddr = (smem_u32(stg) >> 2) + static_cast<uint32_t>(row * Cfg::kStageLd);
+      Epi::template run<BN>(ep, waddr, m, m < M, tc.n_tile, N, epi_smem, part, 2);
+      mbar_arrive(stg_free);
     }
-  }
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
   }
 }
 
@@ -210,7 +207,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 // (acc[] holds their bit patterns). `chunk_pre` fetches whatever the chunk needs that does not
 // depend on the accumulator (so callers can issue it early); `chunk` applies the T5 rounding
 // contract and writes HBM. Paired functors (GeGLU) consume two chunks: gate and up.
-// The persistent kernel above feeds chunks straight from TMEM (`run`); the split-K kernel
+// The persistent kernel above feeds chunks from its staged accumulator rows (`run`); the split-K kernel
 // (gemm_splitk.cuh) feeds them from the cluster-reduced partial sums.
 
 DEVINL void round_pack_32(const uint32_t (&acc)[32], uint32_t (&out)[16]) {
@@ -238,11 +235,11 @@ DEVINL void store_row_chunk_f32(float* dst, const float (&v)[32], int n0, int N)
 
 struct NoPre {};
 
-// Drives an unpaired functor over the BN columns of this thread's TMEM row, fetching the
+// Drives an unpaired functor over the BN columns of this thread's staged row, fetching the
 // pre-operands of chunk c+1 before chunk c is processed.
 // `part` of `parts`: the epilogue warp handles chunks [part*C/parts, (part+1)*C/parts) of the C = BN/32 chunks.
 template <int BN, class Epi>
-DEVINL void run_chunks_from_tmem(const typename Epi::Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N,
+DEVINL void run_chunks(const typename Epi::Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N,
                                  const uint8_t* epi_smem, int part, int parts) {
   constexpr int C = BN / 32;
   const int c_lo = part * C / parts, c_hi = (part + 1) * C / parts;
@@ -254,10 +251,9 @@ DEVINL void run_chunks_from_tmem(const typename Epi::Params& p, uint32_t taddr, 
     for (int u = 0; u < 2; ++u) {
       if (c + u < c_hi) {
         uint32_t acc[32];
-        tmem_ld_32x32(taddr + (c + u) * 32, acc);
+        acc_ld_32(taddr + (c + u) * 32, acc);
         const int n0 = n_tile * BN + (c + u) * 32;
         if (m_ok && c + u + 1 < c_hi && n0 + 32 < N) Epi::chunk_pre(p, m, n0 + 32, N, pre[(u + 1) & 1]);
-        tmem_ld_wait();
         if (m_ok && n0 < N) Epi::chunk(p, acc, m, n0, N, epi_smem, pre[u & 1]);
       }
     }
@@ -283,7 +279,7 @@ struct EpiStore {
   template <int BN>
   static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t* es,
                          int part, int parts) {
-    run_chunks_from_tmem<BN, EpiStore>(p, taddr, m, m_ok, n_tile, N, es, part, parts);
+    run_chunks<BN, EpiStore>(p, taddr, m, m_ok, n_tile, N, es, part, parts);
   }
 };
 
@@ -333,7 +329,7 @@ struct EpiResidual {
   template <int BN>
   static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t* es,
                          int part, int parts) {
-    run_chunks_from_tmem<BN, EpiResidual>(p, taddr, m, m_ok, n_tile, N, es, part, parts);
+    run_chunks<BN, EpiResidual>(p, taddr, m, m_ok, n_tile, N, es, part, parts);
   }
 };
 #else
@@ -391,7 +387,7 @@ struct EpiResidual {
   template <int BN>
   static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t* es,
                          int part, int parts) {
-    run_chunks_from_tmem<BN, EpiResidual>(p, taddr, m, m_ok, n_tile, N, es, part, parts);
+    run_chunks<BN, EpiResidual>(p, taddr, m, m_ok, n_tile, N, es, part, parts);
   }
 };
 
@@ -513,9 +509,8 @@ struct EpiGeglu {
 #pragma unroll 1
     for (int c = part * C / parts; c < (part + 1) * C / parts; ++c) {
       uint32_t g[32], u[32];
-      tmem_ld_32x32(taddr + c * 32, g);
-      tmem_ld_32x32(taddr + HALF + c * 32, u);
-      tmem_ld_wait();
+      acc_ld_32(taddr + c * 32, g);
+      acc_ld_32(taddr + HALF + c * 32, u);
       const int f0 = n_tile * HALF + c * 32;
       if (m_ok && f0 < p.F) chunk2(p, g, u, m, f0, epi_smem);
     }
@@ -552,7 +547,7 @@ struct EpiCrossKV {
   template <int BN>
   static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t* es,
                          int part, int parts) {
-    run_chunks_from_tmem<BN, EpiCrossKV>(p, taddr, m, m_ok, n_tile, N, es, part, parts);
+    run_chunks<BN, EpiCrossKV>(p, taddr, m, m_ok, n_tile, N, es, part, parts);
   }
 };
 
@@ -592,7 +587,7 @@ struct EpiQkvDecode {
   template <int BN>
   static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t* es,
                          int part, int parts) {
-    run_chunks_from_tmem<BN, EpiQkvDecode>(p, taddr, m, m_ok, n_tile, N, es, part, parts);
+    run_chunks<BN, EpiQkvDecode>(p, taddr, m, m_ok, n_tile, N, es, part, parts);
   }
 };
 
@@ -610,16 +605,17 @@ struct EpiArgmax {
     int step_stride = 0;  // 1 = slot pool: per-row positions
   };
   static DEVINL void prologue(const Params&, uint8_t*, int, int = 128) {}
+  // a row's arg-max is not split: the first of the `parts` threads of each row takes the whole row
   template <int BN>
-  static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t*, int, int) {
+  static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t*, int part, int) {
+    if (part != 0) return;
     float best = -INFINITY;
     int bidx = n_tile * BN;  // all -inf (cannot happen with finite logits) -> first column, like torch
     const bool block_eos = m_ok && p.step[m * p.step_stride] < p.min_new;
 #pragma unroll 1
     for (int c = 0; c < BN / 32; ++c) {
       uint32_t acc[32];
-      tmem_ld_32x32(taddr + c * 32, acc);
-      tmem_ld_wait();
+      acc_ld_32(taddr + c * 32, acc);
       const int n0 = n_tile * BN + c * 32;
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
@@ -647,12 +643,11 @@ struct EpiStoreF32 {
   };
   static DEVINL void prologue(const Params&, uint8_t*, int, int = 128) {}
   template <int BN>
-  static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t*, int, int) {
+  static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t*, int part, int parts) {
 #pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
+    for (int c = part * (BN / 32) / parts; c < (part + 1) * (BN / 32) / parts; ++c) {
       uint32_t acc[32];
-      tmem_ld_32x32(taddr + c * 32, acc);
-      tmem_ld_wait();
+      acc_ld_32(taddr + c * 32, acc);
       const int n0 = n_tile * BN + c * 32;
       if (m_ok) {
 #pragma unroll
@@ -666,9 +661,9 @@ struct EpiStoreF32 {
 // ======================================================================== host launch
 // Opt in to the large dynamic shared memory carve-out once per process/device
 // (done at b200t5_create so it never happens inside a stream capture).
-template <int BN, class Epi>
+template <int BN, class Epi, bool kTf32 = false, int kBBox = BN>
 cudaError_t prepare_gemm() {
-  return cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  return cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, Epi, kTf32, kBBox>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                               GemmCfg<BN>::kSmemBytes);
 }
 
@@ -707,14 +702,16 @@ cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t 
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
-template <int BN, class Epi>
+// a_kblocks: see kTf32 at the kernel (0 = A spans all of K)
+template <int BN, class Epi, bool kTf32 = false, int kBBox = BN>
 cudaError_t launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, int m_fastest,
-                        const typename Epi::Params& ep, int num_sms, cudaStream_t stream, bool pdl = false) {
+                        const typename Epi::Params& ep, int num_sms, cudaStream_t stream, bool pdl = false, int a_kblocks = 0) {
   using Cfg = GemmCfg<BN>;
   const int tiles = ((M + kBM - 1) / kBM) * ((N + BN - 1) / BN);
-  const int grid = tiles < num_sms ? tiles : num_sms;
-  return launch_kernel(gemm_bf16_tn_kernel<BN, Epi>, dim3(grid), dim3(EpiWarps<BN>::kThreads), Cfg::kSmemBytes, stream, pdl,
-                       tmA, tmB, M, N, K, m_fastest, ep);
+  const int slots = num_sms * Cfg::kCtasPerSm;
+  const int grid = tiles < slots ? tiles : slots;
+  return launch_kernel(gemm_bf16_tn_kernel<BN, Epi, kTf32, kBBox>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, pdl,
+                       tmA, tmB, M, N, K, m_fastest, ep, a_kblocks);
 }
 
 }  // namespace b200

@@ -1,243 +1,33 @@
-// CTA-pair bf16 GEMM for the big encoder products:  D[M,N] = A[M,K] * W[N,K]^T  with
-// tcgen05.mma.cta_group::2 - two CTAs on the two SMs of a TPC execute ONE 256 x 256 x 16 MMA.
+// Encoder GEMMs (M = packed prompt rows, tens of thousands):  D[M,N] = A[M,K] * W[N,K]^T  on 128 x 256 tiles.
 //
-// Why: with the single-CTA 128 x 256 tile of gemm.cuh every k-block moves 48 KB into shared
-// memory and the tensor core reads 48 KB back out of it per 512 MMA cycles - 188 B/clk against
-// the SM's 128 B/clk of shared-memory bandwidth. ncu on B200 shows exactly that bound: l1tex
-// throughput 77 %, tensor pipe active 56 %, 1070 TFLOP/s (profiles/encoder_ncu_r1.md). In pair
-// mode each CTA stages its own 128 rows of A and only HALF of the weight tile (16 + 16 KB per
-// k-block): the operand traffic per SM drops by a third and the pipe can be kept busy.
+// The encoder's tensor maps (tm2_*) have 128-row boxes for both operands; this configuration of the persistent
+// wgmma kernel (gemm.cuh) loads each 256-row weight tile as two such boxes. A 128 x 256 tile is the largest the
+// two consumer warpgroups hold in registers (128 fp32 accumulators per thread) and gives the best operand reuse
+// per byte of shared memory: per k-block 48 KB are staged for 128 x 256 x 64 MACs.
 //
-// Roles per CTA (as gemm.cuh): warp 0 = TMA producer, warp 1 = TMEM allocation and (leader CTA
-// only) the MMA issuer, warps 2.. = epilogue (8, or 16 for GeGLU). Barriers:
-//   full[s]    leader's; armed by the leader's producer with the bytes of BOTH CTAs, completed by
-//              both CTAs' TMA loads (cp.async.bulk.tensor...cta_group::2 with the barrier address
-//              mapped into the leader CTA);
-//   empty[s]   one per CTA, released for both by tcgen05.commit...multicast::cluster (mask 0b11);
-//   tfull[a]   one per CTA (multicast commit): this CTA's 128 x 256 accumulator is complete;
-//   tempty[a]  leader's; the epilogue warps of both CTAs (the peer's arrive remotely) hand a buffer back.
-// TMEM: 512 columns per CTA (two accumulator buffers), allocated collectively with cta_group::2.
-#pragma once
-#include "gemm.cuh"
-#include "gemm_splitk.cuh"  // cluster PTX helpers
-
-namespace b200 {
-
-constexpr int k2ctaBN = 256;
-constexpr int k2ctaStages = 6;
-constexpr int k2ctaStageBytes = kBM * kBK * 2 + 128 * kBK * 2;  // own A rows + own half of the weight tile: 32 KB
-// epilogue warps per CTA: 8 (two per TMEM lane quarter); the GeGLU epilogue (a table lookup per output) takes 16
-template <class Epi>
-struct PairEpi {
-  static constexpr int kWarps = Epi::kPaired ? 16 : 8;
-  static constexpr int kThreads = 64 + 32 * kWarps;
-};
-constexpr int k2ctaSmemBytes = k2ctaStages * k2ctaStageBytes + 1024 /*align*/ + 256 /*barriers*/ + kEpiSmemBytes;
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-rank bit of a shared::cluster address: the even CTA of the pair
-
-DEVINL void tma_load_2d_pair(void* smem_dst, const CUtensorMap* m, uint64_t* leader_bar, int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(leader_bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-DEVINL void umma_f16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
-}
-DEVINL void umma_tf32_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
-}
-// All MMAs issued so far by this thread: arrive on the barrier at this offset in BOTH CTAs of the pair.
-DEVINL void umma_commit_pair(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(static_cast<uint16_t>(3))
-               : "memory");
-}
-DEVINL void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
-}
-DEVINL void tmem_alloc_pair_512(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(smem_result)) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-DEVINL void tmem_dealloc_pair_512(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, 512;" ::"r"(taddr) : "memory");
-}
-
-// tmA: box 64 x 128 rows of A; tmB: box 64 x 128 rows of W. grid = 2 * pairs (persistent), cluster (2,1,1).
 // kTf32 (fp16 build, the fp32-weight `wo` product): both operands are fp32 in memory and consumed as tf32, a
 // k-block is 32 elements (the same 128-byte rows) and K counts the columns of W' = [W_hi | W_lo], the two
 // tf32 pieces of the fp32 weight side by side; A has only a_kblocks k-blocks and is walked twice (kb % a_kblocks),
 // so the accumulator receives A . W_hi^T + A . W_lo^T.
-template <class Epi, bool kTf32 = false>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(PairEpi<Epi>::kThreads, 1)
-gemm_bf16_tn_2cta_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N,
-                         int K, typename Epi::Params ep, int a_kblocks) {
-  constexpr int BN = k2ctaBN;
-  constexpr int kbk = kTf32 ? kBK / 2 : kBK;  // elements per k-block (128 bytes)
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + k2ctaStages * k2ctaStageBytes);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + k2ctaStages;
-  uint64_t* tfull = bars + 2 * k2ctaStages;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  uint8_t* epi_smem = smem + k2ctaStages * k2ctaStageBytes + 256;
+#pragma once
+#include "gemm.cuh"
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int rank = static_cast<int>(cluster_ctarank());
-  const bool leader = rank == 0;
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  const int tiles_m = (M + 2 * kBM - 1) / (2 * kBM);
-  const int tiles_n = (N + BN - 1) / BN;
-  const int num_tiles = tiles_m * tiles_n;
-  const int kblocks = (K + kbk - 1) / kbk;
-  if (a_kblocks <= 0) a_kblocks = kblocks;
+namespace b200 {
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < k2ctaStages; ++i) {
-        mbar_init(&full[i], 1);
-        mbar_init(&empty[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&tfull[i], 1);
-        mbar_init(&tempty[i], 2 * PairEpi<Epi>::kWarps);  // the epilogue warps of both CTAs of the pair
-      }
-      mbar_fence_init();
-    }
-    __syncwarp();
-    tmem_alloc_pair_512(tmem_slot);  // collective: warp 1 of both CTAs
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  cluster_arrive_release();  // barriers of both CTAs exist before anything is signalled across the pair
-  cluster_wait_acquire();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ------------------------------------------------------------ TMA producer (both CTAs)
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += npairs) {
-        const int n_tile = tile % tiles_n, m_tile = tile / tiles_n;
-        const int m0 = m_tile * 2 * kBM + rank * kBM, n0 = n_tile * BN + rank * 128;
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1u);
-          uint8_t* sA = smem + stage * k2ctaStageBytes;
-          if (leader) mbar_arrive_expect_tx(&full[stage], 2u * k2ctaStageBytes);
-          tma_load_2d_pair(sA, &tmA, &full[stage], (kb % a_kblocks) * kbk, m0);
-          tma_load_2d_pair(sA + kBM * kBK * 2, &tmB, &full[stage], kb * kbk, n0);
-          if (++stage == k2ctaStages) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer (leader CTA only)
-    if (leader && lane == 0) {
-      constexpr uint32_t idesc = kTf32 ? make_idesc_tf32(2 * kBM, BN) : make_idesc_act(2 * kBM, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int tile = pair; tile < num_tiles; tile += npairs) {
-        mbar_wait(&tempty[as], aphase ^ 1u);
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(as * BN);
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after_sync();
-          const uint32_t a_addr = smem_u32(smem + stage * k2ctaStageBytes);
-          const uint64_t a_desc = make_desc_sw128_kmajor(a_addr);
-          const uint64_t b_desc = make_desc_sw128_kmajor(a_addr + kBM * kBK * 2);
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {  // 32 bytes of K per instruction in either kind
-            if constexpr (kTf32)
-              umma_tf32_ss_pair(d_tmem, a_desc + static_cast<uint64_t>(2 * k), b_desc + static_cast<uint64_t>(2 * k), idesc,
-                                (kb | k) != 0 ? 1u : 0u);
-            else
-              umma_f16_ss_pair(d_tmem, a_desc + static_cast<uint64_t>(2 * k), b_desc + static_cast<uint64_t>(2 * k), idesc,
-                               (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit_pair(&empty[stage]);
-          if (++stage == k2ctaStages) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        umma_commit_pair(&tfull[as]);
-        as ^= 1;
-        if (as == 0) aphase ^= 1u;
-      }
-    }
-  } else {
-    // ------------------------------------------------------------ epilogue warps (both CTAs, own 128 rows)
-    const int q = warp & 3;
-    const int part = (warp - 2) >> 2;
-    int as = 0;
-    uint32_t aphase = 0;
-    Epi::prologue(ep, epi_smem, static_cast<int>(threadIdx.x) - 64, 32 * PairEpi<Epi>::kWarps);
-    for (int tile = pair; tile < num_tiles; tile += npairs) {
-      const int n_tile = tile % tiles_n, m_tile = tile / tiles_n;
-      const int m = m_tile * 2 * kBM + rank * kBM + q * 32 + lane;
-      mbar_wait(&tfull[as], aphase);
-      tc_fence_after_sync();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(as * BN);
-      Epi::template run<BN>(ep, taddr, m, m < M, n_tile, N, epi_smem, part, PairEpi<Epi>::kWarps / 4);
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_leader(&tempty[as]);
-      as ^= 1;
-      if (as == 0) aphase ^= 1u;
-    }
-  }
-  // neither CTA may release its shared memory / TMEM while the pair's MMAs or remote arrivals can still touch it
-  tc_fence_before_sync();
-  __syncthreads();
-  cluster_arrive_release();
-  cluster_wait_acquire();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc_pair_512(tmem_base);
-  }
-}
+constexpr int k2ctaBN = 256;
+constexpr int k2ctaBox = 128;
 
 template <class Epi, bool kTf32 = false>
 cudaError_t prepare_gemm_2cta() {
-  return cudaFuncSetAttribute(gemm_bf16_tn_2cta_kernel<Epi, kTf32>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2ctaSmemBytes);
+  return prepare_gemm<k2ctaBN, Epi, kTf32, k2ctaBox>();
 }
 
-// a_kblocks: see kTf32 above (0 = A spans all of K)
+// a_kblocks: see kTf32 above (0 = A spans all of K). Tiles are visited n-fastest: the CTAs that run at the same
+// time share the rows of A.
 template <class Epi, bool kTf32 = false>
 cudaError_t launch_gemm_2cta(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K,
                              const typename Epi::Params& ep, int num_sms, cudaStream_t stream, int a_kblocks = 0) {
-  const int tiles = ((M + 2 * kBM - 1) / (2 * kBM)) * ((N + k2ctaBN - 1) / k2ctaBN);
-  int pairs = num_sms / 2;
-  if (tiles < pairs) pairs = tiles;
-  gemm_bf16_tn_2cta_kernel<Epi, kTf32><<<dim3(2 * pairs), dim3(PairEpi<Epi>::kThreads), k2ctaSmemBytes, stream>>>(tmA, tmB, M, N, K, ep, a_kblocks);
-  return cudaGetLastError();
+  return launch_gemm<k2ctaBN, Epi, kTf32, k2ctaBox>(tmA, tmB, M, N, K, 0, ep, num_sms, stream, false, a_kblocks);
 }
 
 }  // namespace b200

@@ -3,36 +3,31 @@
 //   cluster's CTAs, partial sums reduced through distributed shared memory.
 //
 // Why: with M = 256 a decode GEMM has only (M/128)*(N/BN) output tiles, and every tile's CTA
-// must pull (128 + BN) * K * 2 bytes through ONE SM's L2 port (~40-60 B/clk). For N = 768,
-// K = 2048 that is 650 KB per CTA = 6-8 us on 48 SMs while 100 SMs idle (measured: 10-12 us per
-// launch, profiles/launches_r1.csv). Cutting K over a cluster of S CTAs divides the per-SM bytes
-// by S and multiplies the number of busy SMs by S; the reduction costs one DSMEM pass.
+// must pull (128 + BN) * K * 2 bytes through ONE SM. For N = 768, K = 2048 that is 650 KB per CTA
+// on 12 of the 132 SMs. Cutting K over a cluster of S CTAs divides the per-SM bytes by S and
+// multiplies the number of busy SMs by S; the reduction costs one DSMEM pass.
 //
-// Per CTA (192 threads, same roles as gemm.cuh): warp 0 = TMA producer (the weight slices do not
-// depend on the previous kernel and are requested BEFORE griddepcontrol.wait), warp 1 = TMEM
-// owner + tcgen05.mma issuer, warps 2..5 = epilogue. After its MMAs complete each CTA holds a
-// 128 x BN fp32 partial tile in TMEM. Reduce-scatter by ROWS: rank r of the cluster owns tile
-// rows [r*128/S, (r+1)*128/S); every epilogue thread (= one tile row) sends its row to the
-// owner's `red` buffer slot [src rank][row] with st.shared::cluster, a cluster barrier
-// (release/acquire) publishes the writes, and the owner sums the S partials in rank order
-// (deterministic) and feeds 32-column chunks to the same epilogue functors the persistent GEMM
-// uses (gemm.cuh), so the T5 rounding contract is shared.
+// Per CTA (288 threads, the roles of gemm.cuh): warp 8 = TMA producer (the weight slices do not
+// depend on the previous kernel and are requested BEFORE griddepcontrol.wait), warps 0..7 = two
+// consumer warpgroups, each running wgmma over 64 tile rows with fp32 accumulators in registers.
+// Reduce-scatter by ROWS: rank r of the cluster owns tile rows [r*128/S, (r+1)*128/S); every
+// consumer thread sends its accumulator fragments to the owner's `red` buffer slot [src rank][row]
+// with st.shared::cluster, a cluster barrier (release/acquire) publishes the writes, and the owner
+// sums the S partials in rank order (deterministic) and feeds 32-column chunks to the same epilogue
+// functors the persistent GEMM uses (gemm.cuh), so the T5 rounding contract is shared.
 //
-// Footprint: the number of pipeline stages is a launch parameter, so that a CTA (115-140 KB) can be sized to fit on
+// Footprint: the number of pipeline stages is a launch parameter, so that a CTA can be sized to fit on
 // an SM next to the resident CTAs of the other row-chain's cross-attention stream (attention_cross_stream.cuh).
-// (Round 2: keeping each rank's OWN rows in TMEM instead of sending them to itself saves 1/S of `red` but leaves the
-// reduction to the 128/S threads whose TMEM lanes hold those rows - measured +8 ms per batch; reverted.)
-// (Measured alternatives, round 1: st.async with a receiver-side mbarrier instead of the release fence +
-// cluster barrier, 194.8 vs 188.3 ms per batch; staging the rows locally and moving them with one
-// cp.async.bulk per destination rank, 195.3 ms; normalising the A tile in shared memory instead of a separate
-// RMSNorm kernel, 201.1 vs 189.1 ms; an A-multicast kernel without reduction, 201.4 vs 191.0 ms -
-// profiles/decode_trace_r1.md.)
 #pragma once
 #include "gemm.cuh"
 
 namespace b200 {
 
-constexpr int kSkThreads = 192;
+constexpr int kSkThreads = kGemmThreads;  // 2 consumer warpgroups + 1 producer warp
+// Register cap: one split-K CTA (288 threads) must fit on an SM next to two CTAs of the other row-chain's
+// cross-attention stream kernel (2 x 160 threads x 64 registers): (65536 - 20480) / 288 -> 152 per thread.
+// Left to __launch_bounds__(288, 1), ptxas takes 168 and only one stream CTA fits beside the GEMM.
+constexpr int kSkMaxRegs = 152;
 constexpr int kSkMaxSplit = 8;
 constexpr int kSkMaxStages = 4;
 
@@ -72,8 +67,8 @@ DEVINL uint32_t mapa_shared(uint32_t cta_addr, uint32_t rank) {
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(cta_addr), "r"(rank));
   return r;
 }
-DEVINL void st_cluster_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+DEVINL void st_cluster_v2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
 
 DEVINL void add32_smem(uint32_t (&acc)[32], const float* src) {
@@ -89,9 +84,9 @@ DEVINL void add32_smem(uint32_t (&acc)[32], const float* src) {
 }
 
 // grid = (S, tiles_n, tiles_m), cluster = (S, 1, 1); S in {1,2,4,8} divides 128.
-// kTf32 / a_kblocks: as in gemm_2cta.cuh (fp32 operands consumed as tf32, W' = [W_hi | W_lo], A walked twice).
+// kTf32 / a_kblocks: as in gemm.cuh (fp32 operands consumed as tf32, W' = [W_hi | W_lo], A walked twice).
 template <int BN, class Epi, bool kTf32 = false>
-__global__ void __launch_bounds__(kSkThreads, 1)
+__global__ void __maxnreg__(kSkMaxRegs)
 gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N,
                    int K, typename Epi::Params ep, int a_kblocks, int stages) {
   using Cfg = SkCfg<BN>;
@@ -101,8 +96,6 @@ gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + stages * Cfg::kStageBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + kSkMaxStages;
-  uint64_t* tfull = bars + 2 * kSkMaxStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tfull + 1);
   float* red = reinterpret_cast<float*>(smem + stages * Cfg::kStageBytes + 256);
 
   const int warp = threadIdx.x >> 5;
@@ -121,30 +114,20 @@ gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 
   pdl_launch_dependents();
   cluster_arrive_relaxed();  // #1: "this CTA runs" - peers wait for it before touching our shared memory
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < stages; ++i) {
-        mbar_init(&full[i], 1);
-        mbar_init(&empty[i], 1);
-      }
-      mbar_init(tfull, 1);
-      mbar_fence_init();
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < stages; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 2);  // one arrival per consumer warpgroup
     }
-    __syncwarp();
-    tmem_alloc<BN>(tmem_slot);
+    mbar_fence_init();
   }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ------------------------------------------------------------ TMA producer
     if (lane == 0) {
+      tma_prefetch_desc(&tmA);
+      tma_prefetch_desc(&tmB);
       const int first = nkb < stages ? nkb : stages;
       // weights first: they never depend on the previous kernel
       for (int i = 0; i < first; ++i) {
@@ -172,48 +155,12 @@ gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     cluster_wait_acquire();    // #1
     cluster_arrive_release();  // #2
     cluster_wait_acquire();
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = kTf32 ? make_idesc_tf32(kBM, BN) : make_idesc_act(kBM, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int i = 0; i < nkb; ++i) {
-        mbar_wait(&full[stage], phase);
-        tc_fence_after_sync();
-        const uint32_t a_addr = smem_u32(smem + stage * Cfg::kStageBytes);
-        const uint64_t a_desc = make_desc_sw128_kmajor(a_addr);
-        const uint64_t b_desc = make_desc_sw128_kmajor(a_addr + Cfg::kABytes);
-#pragma unroll
-        for (int k = 0; k < kBK / 16; ++k) {  // 32 bytes of K per instruction in either kind
-          if constexpr (kTf32)
-            umma_tf32_ss(tmem_base, a_desc + static_cast<uint64_t>(2 * k), b_desc + static_cast<uint64_t>(2 * k), idesc,
-                         (i | k) != 0 ? 1u : 0u);
-          else
-            umma_f16_ss(tmem_base, a_desc + static_cast<uint64_t>(2 * k), b_desc + static_cast<uint64_t>(2 * k), idesc,
-                        (i | k) != 0 ? 1u : 0u);
-        }
-        umma_commit(&empty[stage]);
-        if (++stage == stages) {
-          stage = 0;
-          phase ^= 1u;
-        }
-      }
-      umma_commit(tfull);
-    }
-    __syncwarp();
-    cluster_wait_acquire();    // #1
-    cluster_arrive_release();  // #2
-    cluster_wait_acquire();
-    tc_fence_after_sync();
-    tmem_dealloc<BN>(tmem_base);
   } else {
-    // ------------------------------------------------------------ epilogue warps
-    const int et = static_cast<int>(threadIdx.x) - 64;  // 0..127
-    const int q = warp & 3;                             // TMEM lane quarter this warp may read
-    const int row = q * 32 + lane;                      // tile row held by this thread
+    // ------------------------------------------------------------ consumer warpgroups: MMA, scatter, reduce + epilogue
+    const int et = threadIdx.x;  // 0..255
+    const int wg = warp >> 2;
     const int rows_per = kBM / S;
-    if constexpr (Epi::kPaired) Epi::prologue(ep, epi_smem, et);  // gelu table; overlaps the main loop
+    if constexpr (Epi::kPaired) Epi::prologue(ep, epi_smem, et, kGemmConsumers);  // gelu table; overlaps the main loop
     constexpr int kChunks = Epi::kPaired ? BN / 64 : BN / 32;
     const int items = rows_per * kChunks;
     pdl_wait();
@@ -226,30 +173,51 @@ gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         if (et < items && m < M && n0t + c * 32 < N) Epi::chunk_pre(ep, m, n0t + c * 32, N, pre0);
       }
     }
-    mbar_wait(tfull, 0);
-    tc_fence_after_sync();
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    {
+      int stage = 0, prev = -1;
+      uint32_t phase = 0;
+      for (int i = 0; i < nkb; ++i) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t a_addr = smem_u32(smem + stage * Cfg::kStageBytes) + wg * 64 * 128;
+        wgmma_fence_acc(acc);
+        wgmma_fence();
+        wgmma_kblock<BN, kTf32>(acc, a_addr, smem_u32(smem + stage * Cfg::kStageBytes + Cfg::kABytes));
+        wgmma_commit();
+        wgmma_wait<1>();
+        wgmma_fence_acc(acc);
+        if (prev >= 0 && (et & 127) == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == stages) {
+          stage = 0;
+          phase ^= 1u;
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+    }
     cluster_wait_acquire();  // #1: every CTA of the cluster is running, its `red` buffer may be written
     {
-      // (every lane of the warp executes the TMEM loads: tcgen05.ld is warp-collective)
-      const int dst_rank = row / rows_per;
-      const int slot = rank * rows_per + (row - dst_rank * rows_per);
-      const uint32_t dst = mapa_shared(smem_u32(red + static_cast<size_t>(slot) * Cfg::kRedLd), static_cast<uint32_t>(dst_rank));
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        uint32_t acc[32];
-        tmem_ld_32x32(taddr + c * 32, acc);
-        tmem_ld_wait();
+      // reduce-scatter by rows: tile row r goes to slot [rank][r % rows_per] of rank r / rows_per
+      const int t = et & 127;
+      const int rbase = wg * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
+      const int c = 2 * (t & 3);
 #pragma unroll
-        for (int v = 0; v < 8; ++v)
-          st_cluster_v4(dst + (c * 32 + v * 4) * 4, acc[4 * v], acc[4 * v + 1], acc[4 * v + 2], acc[4 * v + 3]);
+      for (int half = 0; half < 2; ++half) {
+        const int row = rbase + 8 * half;
+        const int dst_rank = row / rows_per;
+        const int slot = rank * rows_per + (row - dst_rank * rows_per);
+        const uint32_t dst = mapa_shared(smem_u32(red + static_cast<size_t>(slot) * Cfg::kRedLd + c), static_cast<uint32_t>(dst_rank));
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) st_cluster_v2(dst + 32 * j, acc[4 * j + 2 * half], acc[4 * j + 2 * half + 1]);
       }
     }
-    tc_fence_before_sync();
     cluster_arrive_release();  // #2: partials published
     cluster_wait_acquire();
 #pragma unroll 1
-    for (int it = et; it < items; it += 128) {
+    for (int it = et; it < items; it += kGemmConsumers) {
       const int rl = it / kChunks, c = it - rl * kChunks;
       const int m = m0 + rank * rows_per + rl;
       if (m >= M) continue;

@@ -5,11 +5,11 @@ The reference's seam is duck-typed (NLP_workloads/Anyscale_job/predictor.py):
     self.model.device                                      :98
     self.model.generate(**generate_kwargs) -> LongTensor   :102  (consumed by tokenizer.batch_decode :104)
 so passing ``model_cls=B200T5ForConditionalGeneration`` to ``BatchPredictor.from_checkpoint``
-(notebook lines 875-883) swaps the Hugging Face eager model for the sm_100a kernels behind
+(notebook lines 875-883) swaps the Hugging Face eager model for the sm_90a kernels behind
 libb200t5.so without touching the predictor.
 
 PyTorch is used for device memory and streams only; all arithmetic runs in the CUDA library.
-There is no CPU path: constructing the model without a B200 raises.
+There is no CPU path: constructing the model without an H100 raises.
 """
 from __future__ import annotations
 
@@ -28,7 +28,7 @@ import torch
 from . import _lib
 from .synth import read_safetensors
 
-_POOL_MAX_S = 512  # the slot pool admits prompts through the packed tcgen05 encoder (csrc: kEncTcMaxS)
+_POOL_MAX_S = 512  # the slot pool admits prompts through the packed encoder (csrc: kEncPackMaxS)
 _HF_DEFAULT_MAX_LENGTH = 20  # GenerationConfig default the notebook's single-prompt cell relies on (NB:577)
 
 _IGNORED_WEIGHTS = ("decoder.block.0.layer.1.EncDecAttention.relative_attention_bias.weight",)
@@ -44,14 +44,14 @@ def _ptr(t: Optional[torch.Tensor]):
 
 
 class B200T5ForConditionalGeneration:
-    """FLAN-T5 greedy generation on one B200. API subset of transformers.T5ForConditionalGeneration
+    """FLAN-T5 greedy generation on one H100. API subset of transformers.T5ForConditionalGeneration
     that the workshop's predictor and notebook cells touch."""
 
     main_input_name = "input_ids"
 
     def __init__(self, config: Dict[str, Any], device: torch.device, compute_dtype: torch.dtype = torch.bfloat16):
         if device.type != "cuda":
-            raise RuntimeError("B200T5ForConditionalGeneration runs on a B200 only; there is no CPU fallback")
+            raise RuntimeError("B200T5ForConditionalGeneration runs on an H100 only; there is no CPU fallback")
         if compute_dtype not in (torch.bfloat16, torch.float16):
             raise ValueError(f"compute dtype must be bfloat16 or float16, got {compute_dtype}")
         # one shared library per numerics contract: bf16 everywhere, or the notebook's literal torch_dtype=float16
@@ -88,7 +88,7 @@ class B200T5ForConditionalGeneration:
         self._index = index
         self.last_lengths: Optional[torch.Tensor] = None
         # generate() switches to the continuous-batching path for batches larger than pool_size; that path runs
-        # pool_slots decode slots (512 measured best on B200 for FLAN-T5-base: +18 % over 256, profiles/stream_r1.md)
+        # pool_slots decode slots (tools/bench_stream.py measures the choice)
         self.pool_size = int(os.environ.get("B200T5_POOL", "256"))
         # one handle = one execution plan: calls are serialised. Two host threads may alternate on it (the detokenise /
         # DataFrame tail of block i overlaps the GPU part of block i+1: rayshim/train.py:_overlap_tail).
@@ -235,10 +235,10 @@ class B200T5ForConditionalGeneration:
         for k in ("temperature", "top_k", "top_p", "repetition_penalty", "no_repeat_ngram_size", "num_return_sequences"):
             v = unused.get(k)
             if v is not None and not (isinstance(v, (int, float)) and v == 1):
-                raise NotImplementedError(f"generate({k}=...) is not supported by the B200 path")
+                raise NotImplementedError(f"generate({k}=...) is not supported by the CUDA path")
         for k in ("logits_processor", "stopping_criteria", "forced_bos_token_id", "decoder_input_ids", "encoder_outputs"):
             if unused.get(k) is not None:  # (may be tensors: no truth-value tests)
-                raise NotImplementedError(f"generate({k}=...) is not supported by the B200 path")
+                raise NotImplementedError(f"generate({k}=...) is not supported by the CUDA path")
         gp = self._gen_params(max_new_tokens, max_length, min_new_tokens, min_length, eos_token_id, pad_token_id,
                               decoder_start_token_id, poll_interval)
         host = torch.as_tensor(input_ids)
@@ -267,7 +267,7 @@ class B200T5ForConditionalGeneration:
                 # admits prompts from host memory as slots free up (its entry point takes host buffers).
                 out_np, _ = self.generate_stream(ids.cpu().numpy(), None if mask is None else mask.cpu().numpy(), _gen_params=gp)
                 return torch.from_numpy(out_np).to(self._device)
-            # prompts the slot pool cannot take (it needs the packed tcgen05 encoder, S <= 512): static batches
+            # prompts the slot pool cannot take (it needs the packed encoder, S <= 512): static batches
             outs = [self._generate_static(ids[lo:lo + self.pool_size], None if mask is None else mask[lo:lo + self.pool_size], gp)
                     for lo in range(0, B, self.pool_size)]
             width = max(o.shape[1] for o in outs)

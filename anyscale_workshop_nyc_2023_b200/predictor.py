@@ -2,7 +2,7 @@
 
 Interface source: NLP_workloads/Anyscale_job/predictor.py:14-106 (identical copy in the notebook,
 Model_finetuning_and_batch_inference.ipynb:760-852). Names, argument meaning and error behaviour
-are kept so the notebook cells run unchanged; the body is written for the B200 path:
+are kept so the notebook cells run unchanged; the body is written for the CUDA path:
 
   * columns are staged through pinned host memory (one set of buffers per calling thread) and copied with
     non-blocking H2D copies; a batch larger than the model's pool of decode slots is handed over in HOST memory

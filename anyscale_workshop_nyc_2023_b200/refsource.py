@@ -3,11 +3,9 @@
 `NLP_workloads/Anyscale_job/predictor.py` (HuggingFaceModelPredictor, :14-106) and `utils.py`
 (preprocess_function, :6-33) are plain Python whose only obstacle offline is `import ray` at module top
 (predictor.py:7). With the shim registered under the name `ray` (rayshim.install()) they import as they are,
-straight from the reference checkout - nothing is copied into this repository. The checkout exists in the build
-container (/root/reference, or $B200T5_REFERENCE_ROOT) and NOT on the GPU boxes, so callers must handle `None`:
+straight from a reference checkout - nothing is copied into this repository. A checkout is used only where
+$B200T5_REFERENCE_ROOT names one, so callers must handle `None`:
 
-  * tests/test_reference_predictor_cpu.py drives the unmodified class through the shim's BatchPredictor exactly as
-    flan-t5-batch-inference.py:119-138 does and pins this package's mirror (predictor.py) to it;
   * bench.py's CPU arm uses it when available (`cpu_baseline.kind == "reference"`), the mirror otherwise ("port").
 """
 from __future__ import annotations
@@ -23,8 +21,14 @@ _JOB_DIR = Path("NLP_workloads") / "Anyscale_job"
 
 
 def reference_root() -> Optional[Path]:
-    root = Path(os.environ.get("B200T5_REFERENCE_ROOT", "/root/reference"))
-    return root if (root / _JOB_DIR / "predictor.py").is_file() else None
+    env = os.environ.get("B200T5_REFERENCE_ROOT")
+    if not env:
+        return None
+    root = Path(env)
+    try:
+        return root if (root / _JOB_DIR / "predictor.py").is_file() else None
+    except OSError:  # not readable by this user
+        return None
 
 
 def _load(path: Path, name: str) -> ModuleType:

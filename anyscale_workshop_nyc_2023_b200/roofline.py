@@ -6,7 +6,23 @@ GPU (tests/test_roofline_cpu.py pins it to SURVEY's table) and against the libra
 Element size 2 bytes (bf16 / fp16); activations, ids and logits are excluded, as in SURVEY 8d."""
 from __future__ import annotations
 
-from typing import Iterable, Optional
+import json
+from pathlib import Path
+from typing import Iterable, Optional, Tuple
+
+# NVIDIA H100 SXM data sheet (a card allowed 700 W): HBM3 bandwidth and dense BF16 tensor throughput
+H100_HBM_GBS = 3350.0
+H100_BF16_TFLOPS = 989.0
+
+
+def peaks(root: Path) -> Tuple[float, float, str]:
+    """(HBM GB/s, bf16 TFLOP/s, source) the roofline fractions are taken against: the measured figures in
+    `root / MEASURED_PEAKS.json` when that file exists, otherwise the H100 SXM data sheet."""
+    f = Path(root) / "MEASURED_PEAKS.json"
+    if f.exists():
+        pk = json.loads(f.read_text())
+        return float(pk["hbm_gbs"]), float(pk.get("bf16_tflops_sustained", H100_BF16_TFLOPS)), "measured (MEASURED_PEAKS.json)"
+    return H100_HBM_GBS, H100_BF16_TFLOPS, "H100 SXM data sheet (HBM3 3.35 TB/s, dense BF16 989 TFLOP/s at 700 W)"
 
 
 def step_weight_elements(spec) -> int:

@@ -63,8 +63,8 @@ class T5Spec:
     # 1.0 = modeling_t5.py:_init_weights, attention scores of unit variance, as in a trained checkpoint. The two
     # test-sized models keep the 4.0 their committed golden fixtures were generated with (peaked attention on 2-3
     # layers and short prompts); on the 12-24-layer FLAN-T5 shapes with 512 keys that setting makes the network
-    # numerically chaotic - stock transformers bf16 on GPU vs CPU agree on < 5 % of arg-maxes, mean |dlogit| 0.6
-    # (profiles/parity_headline_r2.md) - so no implementation can be compared with another one on it.
+    # numerically chaotic - stock transformers bf16 on GPU and on CPU rarely agree on an arg-max - so no
+    # implementation can be compared with another one on it.
     q_init_gain: float = 1.0
 
     @property

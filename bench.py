@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - the reference's headline workload on B200: FLAN-T5 greedy batch inference,
+"""bench.py - the reference's headline workload on one H100: FLAN-T5 greedy batch inference,
 512-token prompts -> 128 generated tokens, batch 256 (BASELINE.json configs[1]).
 
 A "step" is one pass of the hot path over one 256-prompt batch (tokenised synthetic prompts,
@@ -21,6 +21,7 @@ seeded random FLAN-T5-base weights: no checkpoints or datasets exist offline).
 
 python bench.py --gpus N --steps K --warmup W            (N>1: launched by torch.distributed.run)
 python bench.py --impl reference ...                     (reference arm: the CPU path only)
+python bench.py ... --dump-outputs DIR                   (GPU arm: the last timed step's generated tokens -> DIR/tokens.npy)
 """
 from __future__ import annotations
 
@@ -59,6 +60,9 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--hf-gpu-batches", type=int, default=2, help="timed 256-prompt batches of the HF-eager-on-GPU incumbent (0 = skip)")
     ap.add_argument("--parity-rows", type=int, default=16, help="rows of the last timed batch checked against HF on this GPU (0 = skip)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step returned (token ids [batch, new+1], float64) to DIR/tokens.npy; "
+                         "inputs and weights are seeded, so two builds can be compared output for output")
     return ap.parse_args()
 
 
@@ -86,7 +90,7 @@ def effective_cores() -> int:
 
 
 def workload_name(a):
-    # BASELINE.json: configs[1] = FLAN-T5-base, batch 256, 512-in/128-out on one B200 (the config the metric is
+    # BASELINE.json: configs[1] = FLAN-T5-base, batch 256, 512-in/128-out on one GPU (the config the metric is
     # quoted on); configs[3] = the same shape with FLAN-T5-large (HBM-roofline report); configs[0] is the CPU case
     tag = {"flan-t5-base": "BASELINE configs[1]", "flan-t5-large": "BASELINE configs[3] shape", "flan-t5-small": "configs[0] model at the configs[1] shape"}
     std = a.batch == 256 and a.seq == 512 and a.new == 128 and a.lengths == "full"
@@ -237,7 +241,7 @@ def main_reference(a):
 
 # --------------------------------------------------------------------------- HF on the same GPU: parity + incumbent
 def hf_gpu_legs(a, ckpt, spec, last_batch, last_out, dtype, model=None):
-    """transformers' eager model in the same dtype on this GPU (torch 2.11 + cuBLAS: 'the existing Blackwell path').
+    """transformers' eager model in the same dtype on this GPU (torch 2.11 + cuBLAS: 'the existing Hopper path').
     (1) parity of a sample of the last TIMED batch, (2) its own throughput on the same workload."""
     import numpy as np
     import torch
@@ -274,7 +278,7 @@ def hf_gpu_legs(a, ckpt, spec, last_batch, last_out, dtype, model=None):
         }
         if model is not None:
             # every decision with HF's own tokens fed back (nothing excluded, no divergence to compound): the
-            # B200 arg-max at each of the rows x T positions against HF's, and the logit error itself
+            # CUDA-path arg-max at each of the rows x T positions against HF's, and the logit error itself
             mine = model.decode_logits(ids[sub], mask[sub], ref[:, :-1]).float().cpu().numpy()
             mine[:, :, spec.eos_token_id] = -np.inf
             same = mine.argmax(-1) == lg.argmax(-1)
@@ -315,7 +319,7 @@ def hf_gpu_legs(a, ckpt, spec, last_batch, last_out, dtype, model=None):
     return out
 
 
-# --------------------------------------------------------------------------- B200 arm
+# --------------------------------------------------------------------------- GPU arm
 def main_b200(a):
     import numpy as np
     import torch
@@ -328,7 +332,7 @@ def main_b200(a):
 
     rank, world, local = dist_env()
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py --impl b200 needs a B200; there is no CPU fallback (use --impl reference)")
+        raise SystemExit("bench.py --impl b200 needs an H100; there is no CPU fallback (use --impl reference)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -400,6 +404,10 @@ def main_b200(a):
     elapsed_ms = e0.elapsed_time(e1)
     clocks = sampler.stop()
     last_out = out.cpu().numpy()  # the last TIMED batch's tokens: checked against HF below, outside the timed region
+    if a.dump_outputs and rank == 0:
+        dump = Path(a.dump_outputs)
+        dump.mkdir(parents=True, exist_ok=True)
+        np.save(dump / "tokens.npy", last_out.astype(np.float64))  # token ids < 2**53: exact in float64
 
     if rank == 0:
         log(f"device-resident: {elapsed_ms / K:.1f} ms/step")
@@ -434,20 +442,7 @@ def main_b200(a):
     elapsed_ms = max_over_ranks(elapsed_ms, dev)
     e2e_ms = max_over_ranks(e2e_ms, dev)
 
-    peaks_file = ROOT / "MEASURED_PEAKS.json"
-    if peaks_file.exists():
-        pk = json.loads(peaks_file.read_text())
-        hbm_peak, tf_peak, peak_src = float(pk["hbm_gbs"]), float(pk.get("bf16_tflops_sustained", 1458.8)), "measured (MEASURED_PEAKS.json)"
-    else:
-        hbm_peak, tf_peak, peak_src = 6650.0, 1400.0, "fallback (B200_PROFILING.md)"
-    # DRAM bytes per launch of the roofline kernel from the committed `ncu --set full` capture (per batch row, scaled
-    # to the rows one in-situ launch covers): only valid for the captured configuration (base, S=512, full-length)
-    traffic = None
-    tf = ROOT / "profiles" / "cross_attn_traffic.json"
-    if tf.exists() and a.model == "flan-t5-base" and (S, a.lengths) == (512, "full"):
-        tj = json.loads(tf.read_text()).get("attn_cross_stream_kernel" if xattn_kernel else "attn_decode_kernel<false>")
-        if tj:
-            traffic = tj["dram_bytes_per_launch"] * rows_per_launch / float(tj["rows_per_launch"])
+    hbm_peak, tf_peak, peak_src = roofline.peaks(ROOT)
 
     kv_gb = roofline.cross_attention_bytes_per_launch(spec, [S] * B) * spec.num_decoder_layers / 1e9
     w_gb = 2.0 * roofline.step_weight_elements(spec) / 1e9
@@ -470,7 +465,7 @@ def main_b200(a):
             "config": {"workload": workload_name(a), "global_batch": world * B, "prompts_per_rank_step": B,
                        "parallelism": f"dataset sharded over {world} replica(s), no collective",
                        "l2": f"inputs exceed L2 (cross-KV arena {kv_gb:.1f} GB and {w_gb:.2f} GB of decoder weights "
-                             "are streamed every step vs 126 MB L2)",
+                             "are streamed every step vs 50 MB L2)",
                        "forced_length": "min_new_tokens == max_new_tokens", "row_chains": n_chains,
                        "host": "dedicated scoring process: gc.freeze() after the model is loaded, as rayshim/pool.py workers do"},
             "prompts_per_s": world * K * B / (elapsed_ms / 1e3),
@@ -489,7 +484,7 @@ def main_b200(a):
             "roofline": {"bound": "hbm", "kernel": "cross-attention decode: " + ("attn_cross_stream_kernel (TMA ring + mma.sync)" if xattn_kernel else "attn_decode_kernel<false> (per-thread loads)")
                                    + "; chosen per call from the prompt fill (B200T5_XATTN=ldg|stream|auto)",
                          "achieved": ach_situ, "peak": hbm_peak, "unit": "GB/s",
-                         "frac": (ach_situ / hbm_peak) if ach_situ else None, "traffic": traffic, "peak_source": peak_src,
+                         "frac": (ach_situ / hbm_peak) if ach_situ else None, "peak_source": peak_src,
                          "frac_per_launch_in_situ": (ach_launch / hbm_peak) if ach_launch else None,
                          "in_situ": {"rows_per_launch": rows_per_launch, "launches_timed": prof["launches"],
                                      "algo_bytes_per_launch": prof["bytes_per_launch"], "us_per_launch": prof["us_per_launch"],

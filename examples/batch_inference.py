@@ -2,7 +2,7 @@
 cells at :260-296 preprocess, :875-883 BatchPredictor.from_checkpoint, :908-913 predict, :934 join) as one script,
 with the ONE edit the drop-in asks for: `model_cls`.
 
-    python examples/batch_inference.py --model-cls b200            # B200 path (needs a B200)
+    python examples/batch_inference.py --model-cls b200            # H100 path (needs an H100)
     python examples/batch_inference.py --model-cls hf --n 8        # the dependency's own model on CPU (reference path)
 
 Ray is not installable offline, so `import ray` resolves to the in-repo shim (rayshim.install()), which serves exactly
@@ -39,7 +39,7 @@ class HFModelOnCpu:
 
     @staticmethod
     def from_pretrained(path, **kw):
-        from oracle.hf_anchor import load_hf_model  # the example's CPU leg only; the B200 path never imports oracle/
+        from oracle.hf_anchor import load_hf_model  # the example's CPU leg only; the CUDA path never imports oracle/
 
         return load_hf_model(path, dtype=torch.float32, device="cpu")
 
@@ -47,7 +47,7 @@ class HFModelOnCpu:
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--model-cls", default="b200", choices=["b200", "hf"])
-    ap.add_argument("--model", default=None, help="flan-t5-small | flan-t5-base | flan-t5-large | tiny (default: base on B200, tiny on CPU)")
+    ap.add_argument("--model", default=None, help="flan-t5-small | flan-t5-base | flan-t5-large | tiny (default: base on H100, tiny on CPU)")
     ap.add_argument("--n", type=int, default=1024)
     ap.add_argument("--batch-size", type=int, default=4096, help="rows handed to the predictor at once; > 256 uses the slot pool")
     ap.add_argument("--max-new-tokens", type=int, default=128)

@@ -1,6 +1,6 @@
 /*
  * b200t5.h - C ABI of libb200t5.so: FLAN-T5 (T5 v1.1, gated-GELU) greedy generation on one
- * NVIDIA B200 (sm_100a), the hot path of the workshop's batch-inference loop.
+ * NVIDIA H100 (sm_90a), the hot path of the workshop's batch-inference loop.
  *
  * What this boundary replaces in the reference (ray-project/anyscale-workshop-nyc-2023):
  * the reference has no FFI of its own; its plug-in seam is the Python attribute
@@ -44,7 +44,7 @@ extern "C" {
 
 #define B200T5_OK 0
 #define B200T5_EINVAL (-1)  /* bad argument / unsupported configuration */
-#define B200T5_ENODEV (-2)  /* no sm_100 device */
+#define B200T5_ENODEV (-2)  /* no sm_90 device */
 #define B200T5_ECUDA (-3)   /* CUDA runtime / driver error */
 #define B200T5_ESTATE (-4)  /* call order violated (e.g. generate before finalize) */
 #define B200T5_ENOMEM (-5)
@@ -178,9 +178,9 @@ int b200t5_decode_logits(b200t5_handle h, const int64_t* input_ids, const int64_
 int b200t5_relative_bucket(int relative_position, int bidirectional, int num_buckets, int max_distance);
 
 /* Single-kernel hooks: all pointers are device pointers, bf16 unless noted. */
-/* C[M,N] = bf16(A[M,K] W[N,K]^T) via the tcgen05 GEMM; mode 0 plain, 1 += residual R (in C),
+/* C[M,N] = bf16(A[M,K] W[N,K]^T) via the wgmma GEMM; mode 0 plain, 1 += residual R (in C),
  * 2 GeGLU (W rows interleaved per bn/2, C is [M,N/2]), 3 fp32 output (C is float*). bn in {32,64,128,256};
- * bn = 512 selects the CTA-pair kernel (tcgen05 cta_group::2, 256 x 256 tiles, GeGLU interleave per 128), modes 0-2. */
+ * bn = 512 selects the encoder configuration (128 x 256 tiles, weight in 128-row boxes, GeGLU interleave per 128), modes 0-2. */
 int b200t5_test_gemm(int device, const void* A, const void* W, void* C, int M, int N, int K, int bn, int mode,
                      int pow_mode, void* stream);
 /* Same contract through the cluster split-K kernel the decode step uses (csrc/gemm_splitk.cuh):
@@ -191,7 +191,7 @@ int b200t5_test_gemm_splitk(int device, const void* A, const void* W, void* C, i
                             int mode, int pow_mode, void* aux, int Tmax, int step, void* stream);
 /* fp16 build (libb200t5_f16.so) only: the fp32-weight feed-forward output projection (transformers keeps T5's `wo`
  * in fp32 under torch_dtype=float16), R += A . W^T computed as two tf32 tensor-core passes over W = W_hi + W_lo.
- * A [M,F] fp32 (fp16-representable values), W [N,F] fp32, R [M,N] fp32 in/out; kernel 0 = CTA-pair (encoder),
+ * A [M,F] fp32 (fp16-representable values), W [N,F] fp32, R [M,N] fp32 in/out; kernel 0 = the encoder GEMM,
  * 1 = cluster split-K (decode; bn 64|128, split 1|2|4|8). The bf16 build returns B200T5_EINVAL. */
 int b200t5_test_ffo(int device, const void* A, const void* W, void* R, int M, int N, int F, int kernel, int bn, int split,
                     void* stream);
@@ -202,7 +202,8 @@ int b200t5_test_rmsnorm(int device, const void* x, const void* w, void* y, int M
 int b200t5_test_attn_decode(int device, int self, const void* q, const void* K, const void* V, void* ctx, int B,
                             int H, int Tk, const int32_t* extent, const uint8_t* key_ok, int step,
                             const float* dist_bias, void* stream);
-/* impl 0: mma.sync kernel (any S); impl 1: tcgen05/TMEM kernel (S <= 512). Query rows >= extent[b] are not written. */
+/* The mma.sync encoder attention; impl 0: rows b * S + i, impl 1: the packed-row addressing the encoder uses (row offsets
+ * cu[b] = b * S), where query rows >= extent[b] are not written. */
 int b200t5_test_encoder_attn(int device, const void* qkv, void* ctx, const float* rel_bias, const uint8_t* key_ok,
                              const int32_t* extent, int B, int S, int H, int impl, void* stream);
 /* out[i] = bf16(gelu_new(gate[i]) * up[i]). mode 0: the GeGLU epilogue's path (exhaustive gelu table);

@@ -34,10 +34,11 @@ def test_every_declared_symbol_is_exported_and_bound(flavour):
 
 
 @pytest.mark.parametrize("flavour", ["bf16", "fp16"])
-def test_library_is_sm100a_tcgen05(flavour):
+def test_library_is_sm90a_wgmma(flavour):
     sass = subprocess.run(["cuobjdump", "-sass", str(_lib.LIB_PATHS[flavour])], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass or "SM100" in sass.upper()
-    for needle in ("UTCHMMA", "UTMALDG", "LDTM", "UTCBAR"):
+    assert "sm_90a" in sass
+    assert "sm_100" not in sass
+    for needle in ("HGMMA", "UTMALDG", "SYNCS"):
         assert needle in sass
 
 

@@ -1,5 +1,5 @@
 """CPU-only: the bench.py contract the driver depends on, exercised through the reference arm (the only arm that runs
-without a GPU) on a tiny configuration, plus the loud failure of the product arm when there is no B200."""
+without a GPU) on a tiny configuration, plus the loud failure of the product arm when there is no GPU."""
 import json
 import subprocess
 import sys

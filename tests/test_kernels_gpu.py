@@ -1,4 +1,4 @@
-"""Per-kernel parity on a B200: every CUDA kernel is called through the C ABI (include/b200t5.h)
+"""Per-kernel parity on an H100: every CUDA kernel is called through the C ABI (include/b200t5.h)
 and compared with a plain PyTorch restatement of the same op that rounds where HF eager rounds
 (SURVEY Appendix A). Tolerances are written next to each assertion."""
 import ctypes as C
@@ -36,7 +36,7 @@ def ulp_close(a, b, ulps=1.0):
     (128, 256, 64, 256), (128, 256, 128, 256), (256, 512, 768, 256), (300, 520, 264, 256),
     (4096, 2304, 768, 256), (8, 2304, 768, 64), (256, 768, 768, 32), (256, 768, 2048, 32),
     (256, 1000, 512, 128), (200, 136, 64, 64),
-    # bn = 512: CTA-pair kernel (tcgen05 cta_group::2, 256 x 256 tiles)
+    # bn = 512: the encoder configuration (128 x 256 tiles, weight tile loaded as two 128-row TMA boxes)
     (256, 256, 64, 512), (512, 768, 768, 512), (4096, 2304, 768, 512), (300, 520, 264, 512), (1000, 1000, 2048, 512),
 ])
 def test_gemm_store(lib, M, N, K, bn):
@@ -468,7 +468,7 @@ def test_encoder_attn(lib, B, S, H, impl):
     scores = scores + pb
     p = torch.softmax(scores.float(), dim=-1).to(torch.bfloat16)
     ref = torch.matmul(p.float(), v.float()).bfloat16().permute(0, 2, 1, 3).reshape(B * S, I)
-    # padded query rows are never observed downstream (the tcgen05 kernel skips fully padded tiles)
+    # padded query rows are never observed downstream (with packed-row addressing, impl 1, they are not computed)
     valid_rows = (torch.arange(S, device="cuda")[None, :] < extent[:, None]).reshape(-1) & ok.reshape(-1)
     out, refv = ctx[valid_rows], ref[valid_rows]
     assert torch.isfinite(out.float()).all()
@@ -479,7 +479,7 @@ def test_encoder_attn(lib, B, S, H, impl):
 
 # ------------------------------------------------------------------------------------------------ fp16 build
 @pytest.mark.parametrize("M,N,F,kernel,bn,split", [
-    (512, 768, 2048, 0, 0, 0),      # encoder shape, CTA-pair kernel
+    (512, 768, 2048, 0, 0, 0),      # encoder shape, encoder GEMM configuration
     (300, 520, 1000, 0, 0, 0),      # ragged everything; F not a multiple of the 32-element k-block
     (256, 768, 2048, 1, 64, 4),     # decode shape, cluster split-K
     (128, 512, 1024, 1, 128, 2),
@@ -488,10 +488,9 @@ def test_encoder_attn(lib, B, S, H, impl):
 def test_fp32_weight_ffo_via_two_tf32_passes(M, N, F, kernel, bn, split):
     """`wo` under torch_dtype=float16 is an fp32 Linear (transformers keeps it in fp32): R += A . W^T with fp32 W.
     The tensor cores only offer tf32 (10 mantissa bits); the library multiplies by W_hi and W_lo, both tf32-exact,
-    in one K-loop. Error metric: max |err| / sum_k |a||w| against an fp64 product. Measured on B200: 2e-7 .. 2.4e-6
-    (growing with K: the tensor core's fp32 accumulation truncates, unlike cuBLAS SGEMM's FMA chain at 2e-7 .. 4e-7),
-    35x .. 1000x below a single tf32 pass (8e-5 .. 2.5e-4) and far below the fp16 rounding (4.9e-4) that follows it
-    in T5LayerNorm."""
+    in one K-loop. Error metric: max |err| / sum_k |a||w| against an fp64 product; it grows with K (the tensor
+    core's fp32 accumulation truncates) and must stay far below a single tf32 pass (8e-5 .. 2.5e-4) and the fp16
+    rounding (4.9e-4) that follows it in T5LayerNorm."""
     lib16 = _lib.load("fp16")
     g = torch.Generator(device="cuda").manual_seed(M + 3 * N + 7 * F)
     A = (torch.randn(M, F, device="cuda", generator=g)).half().float()          # fp16 values, as the GeGLU epilogue writes them

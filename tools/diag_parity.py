@@ -1,4 +1,4 @@
-"""Noise-floor calibration on a B200: how far apart are independent bf16 implementations of the
+"""Noise-floor calibration on an H100: how far apart are independent bf16 implementations of the
 same T5 forward?  ours (CUDA kernels) / HF eager bf16 on GPU (cuBLAS) / HF eager bf16 on CPU,
 all measured against HF fp32 on CPU ("truth"). Writes gpurun_out/diag_parity.json."""
 import json

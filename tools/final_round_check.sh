@@ -1,4 +1,4 @@
-# round-end verification on one B200: GPU test suite, smoke, the headline bench and the supplementary bench lines
+# round-end verification on one H100: GPU test suite, smoke, the headline bench and the supplementary bench lines
 mkdir -p gpurun_out
 set -x
 timeout 900 python -m pytest tests -m gpu -q 2>&1 | tail -3

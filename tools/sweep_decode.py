@@ -1,4 +1,4 @@
-"""Decode-step knob sweep on one B200 without reloading the model: every configuration is a set of
+"""Decode-step knob sweep on one H100 without reloading the model: every configuration is a set of
 b200t5_set_option values; for each, the decode loop and encoder times (CUDA events inside the library) of a few
 forced-length generate calls and the in-situ duration of the cross-attention launches (%globaltimer stamps).
 
@@ -14,6 +14,7 @@ import torch
 
 ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
+from anyscale_workshop_nyc_2023_b200 import roofline  # noqa: E402
 from anyscale_workshop_nyc_2023_b200.modeling import B200T5ForConditionalGeneration  # noqa: E402
 from anyscale_workshop_nyc_2023_b200.synth import SPECS, synthetic_token_batch  # noqa: E402
 from anyscale_workshop_nyc_2023_b200.workload import checkpoint_dir  # noqa: E402
@@ -59,7 +60,7 @@ def main():
                 dec.append(st["decode_ms"])
                 enc.append(st["encoder_ms"])
             rec = {"config": cfg, "decode_ms": min(dec), "decode_ms_all": dec, "encoder_ms": min(enc), "launches": st["kernel_launches"],
-                   "decode_frac_of_hbm": st["decode_algo_bytes"] / (min(dec) / 1e3) / 1e9 / 6572.2}
+                   "decode_frac_of_hbm": st["decode_algo_bytes"] / (min(dec) / 1e3) / 1e9 / roofline.peaks(ROOT)[0]}
             toks = out.cpu()
             if base_tokens is None:
                 base_tokens = toks

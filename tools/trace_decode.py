@@ -1,4 +1,4 @@
-"""Kernel timeline of a few decode steps on a B200 (CUPTI via torch.profiler: every kernel in the
+"""Kernel timeline of a few decode steps on an H100 (CUPTI via torch.profiler: every kernel in the
 process is traced, including the graph-launched ones of libb200t5). Writes gpurun_out/trace_<tag>.json
 with (name, start_us, dur_us, stream) tuples; analyse with tools/analyze_trace.py."""
 import json
