@@ -88,6 +88,7 @@ SIGNATURES = {
     "b200t5_decode_logits": (_i, [_vp, _i64p, _i64p, _i, _i, _i64p, _i, _vp, _vp]),
     "b200t5_relative_bucket": (_i, [_i, _i, _i, _i]),
     "b200t5_test_gemm": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "b200t5_test_enc_gemm": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp]),
     "b200t5_test_gemm_splitk": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
     "b200t5_test_ffo": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "b200t5_test_rmsnorm": (_i, [_i, _vp, _vp, _vp, _i, _i, C.c_float, _vp]),

@@ -308,6 +308,9 @@ struct b200t5_ctx {
   };
   bool pack_rows = true;  // encoder on the valid rows only (variable-length packing); B200T5_PACK=0: all B*S rows as the reference does
   bool use_2cta = true;   // encoder GEMMs on the 128 x 256 tile configuration (gemm_2cta.cuh); B200T5_2CTA=0 selects the G_*256 kernels
+  // 128 x 256 encoder GEMMs through gemm_enc_ws_kernel (epilogue warps overlap the next tile's main loop) rather than
+  // gemm_bf16_tn_kernel; bit-identical results. B200T5_ENC_GEMM, option "enc_gemm" 0|1.
+  bool enc_gemm_ws = true;
   bool self_block = true;  // decoder self-attention with a 4-warp CTA per (row, head): two memory round trips whatever t is
                            // B200T5_SELF=warp selects one warp per (row, head)
   // Cross-attention of the decode step: the TMA-ring + mma.sync stream kernel (attention_cross_stream.cuh: small
@@ -416,6 +419,7 @@ template <class Epi>
 static cudaError_t run_gemm_2cta(b200t5_ctx* h, const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K,
                                  const typename Epi::Params& ep, cudaStream_t s) {
   h->launches++;
+  if (h->enc_gemm_ws) return launch_gemm_enc_ws<Epi>(tmA, tmB, M, N, K, ep, h->num_sms, s);
   return launch_gemm_2cta<Epi>(tmA, tmB, M, N, K, ep, h->num_sms, s);
 }
 
@@ -436,6 +440,7 @@ static cudaError_t run_gemm_sk(b200t5_ctx* h, const b200t5_ctx::SkChoice& ch, co
 static cudaError_t run_ffo_2cta(b200t5_ctx* h, const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N,
                                 const EpiResidual::Params& ep, cudaStream_t s) {
   h->launches++;
+  if (!B200T5_F16 && h->enc_gemm_ws) return launch_gemm_enc_ws<EpiResidual>(tmA, tmB, M, N, h->ffo_k, ep, h->num_sms, s);
   return launch_gemm_2cta<EpiResidual, B200T5_F16 != 0>(tmA, tmB, M, N, h->ffo_k, ep, h->num_sms, s, B200T5_F16 ? h->ffo_k / 64 : 0);
 }
 static cudaError_t run_ffo_sk(b200t5_ctx* h, const b200t5_ctx::SkChoice& ch, const CUtensorMap& tmA, const CUtensorMap& tmB,
@@ -470,6 +475,10 @@ static cudaError_t init_kernel_attrs() {
   if ((e = prepare_gemm_2cta<EpiResidual>()) != cudaSuccess) return e;
   if ((e = prepare_gemm_2cta<EpiGeglu>()) != cudaSuccess) return e;
   if ((e = prepare_gemm_2cta<EpiCrossKV>()) != cudaSuccess) return e;
+  if ((e = prepare_gemm_enc_ws<EpiStore>()) != cudaSuccess) return e;
+  if ((e = prepare_gemm_enc_ws<EpiResidual>()) != cudaSuccess) return e;
+  if ((e = prepare_gemm_enc_ws<EpiGeglu>()) != cudaSuccess) return e;
+  if ((e = prepare_gemm_enc_ws<EpiCrossKV>()) != cudaSuccess) return e;
 #define PREPSK(BN, EPI) \
   if ((e = prepare_gemm_splitk<BN, EPI>()) != cudaSuccess) return e;
   PREPSK(64, EpiStore) PREPSK(128, EpiStore) PREPSK(64, EpiResidual) PREPSK(128, EpiResidual)
@@ -569,6 +578,7 @@ extern "C" int b200t5_create(const b200t5_config* cfg, int device, b200t5_handle
   if (const char* pr_env = getenv("B200T5_PRIO")) h->small_prio = atoi(pr_env);
   if (const char* pk_env = getenv("B200T5_PACK")) h->pack_rows = atoi(pk_env) != 0;
   if (const char* tc_env = getenv("B200T5_2CTA")) h->use_2cta = atoi(tc_env) != 0;
+  if (const char* eg_env = getenv("B200T5_ENC_GEMM")) h->enc_gemm_ws = atoi(eg_env) != 0;
   if (const char* sf_env = getenv("B200T5_SELF")) h->self_block = strcmp(sf_env, "warp") != 0;
   if (const char* xa_env = getenv("B200T5_XATTN")) h->xattn_mode = strcmp(xa_env, "ldg") == 0 ? 0 : strcmp(xa_env, "stream") == 0 ? 1 : 2;
   if (const char* xs_env = getenv("B200T5_XS_STAGES")) {
@@ -1792,7 +1802,8 @@ extern "C" int b200t5_bench_cross_attn(b200t5_handle h, int reps, int rows_per_l
 // step graph. Names: "chains" (row-chains per step, 0 = default), "xattn" (decode cross-attention: 0 = per-thread-load
 // kernel, 1 = TMA stream kernel, 2 = per call by prompt fill), "xattn_stages", "xattn_late_pdl", "xattn_serialize",
 // "xattn_l2pf", "pdl", "admit_overlap", "sk_stages64", "sk_stages128", "profile_xattn" (1 = every cross-attention launch
-// inside the step graph stamps %globaltimer; read with b200t5_get_xattn_profile; off in any timed region).
+// inside the step graph stamps %globaltimer; read with b200t5_get_xattn_profile; off in any timed region), "enc_gemm"
+// (128 x 256 encoder GEMMs: 1 = epilogue-overlapped kernel, 0 = the kernel whose epilogue follows each main loop).
 extern "C" int b200t5_set_option(b200t5_handle h, const char* name, int value) {
   if (!h || !name) return fail(h, B200T5_EINVAL, "null argument");
   const std::string n(name);
@@ -1809,6 +1820,7 @@ extern "C" int b200t5_set_option(b200t5_handle h, const char* name, int value) {
   else if (n == "sk_stages64") h->sk_stages64 = value;
   else if (n == "sk_stages128") h->sk_stages128 = value;
   else if (n == "profile_xattn") h->profile_xattn = value != 0;
+  else if (n == "enc_gemm") h->enc_gemm_ws = value != 0;
   else return fail(h, B200T5_EINVAL, "unknown option '%s'", name);
   CU_OK(h, cudaSetDevice(h->device));
   CU_OK(h, cudaDeviceSynchronize());
@@ -1960,6 +1972,47 @@ extern "C" int b200t5_test_gemm(int device, const void* A, const void* W, void* 
     if (bn == 128) e = run_gemm(&dummy, mk(ta, tb, M, N, K, G_LOGITS128, 1), &ep, s);
   }
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_gemm(bn=%d, mode=%d): %s", bn, mode, cudaGetErrorString(e));
+  return B200T5_OK;
+#endif
+}
+
+extern "C" int b200t5_test_enc_gemm(int device, const void* A, const void* W, void* C, int M, int N, int K, int kernel,
+                                    int mode, int pow_mode, const int* row_b, const int* row_s, int B, int H, int S,
+                                    void* stream) {
+#if B200T5_F16
+  return fail(nullptr, B200T5_EINVAL, "the single-kernel test hooks exist in the bf16 build only (libb200t5.so)");
+#else
+  const int sms = hook_device(device);
+  if (sms < 0) return sms;
+  if (K % 8) return fail(nullptr, B200T5_EINVAL, "K must be a multiple of 8");
+  if (kernel != 0 && kernel != 1) return fail(nullptr, B200T5_EINVAL, "test_enc_gemm: kernel in {0, 1}");
+  if (mode == 3 && (H < 1 || S < 1 || B < 1 || N % (H * 64) || (!row_b) != (!row_s) || (!row_b && M != B * S)))
+    return fail(nullptr, B200T5_EINVAL, "test_enc_gemm: bad cross-KV arguments");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUtensorMap ta, tb;
+  if (!make_tmap(&ta, A, M, K, 128) || !make_tmap(&tb, W, N, K, k2ctaBox)) return fail(nullptr, B200T5_ECUDA, "%s", g_err);
+  b200t5_ctx dummy;
+  dummy.num_sms = sms;
+  dummy.enc_gemm_ws = kernel == 1;
+  cudaError_t e = cudaErrorInvalidValue;
+  act_t* Cb = static_cast<act_t*>(C);
+  if (mode == 0) {
+    EpiStore::Params ep{Cb, N};
+    e = run_gemm_2cta<EpiStore>(&dummy, ta, tb, M, N, K, ep, s);
+  } else if (mode == 1) {
+    EpiResidual::Params ep{Cb, Cb, N};
+    e = run_gemm_2cta<EpiResidual>(&dummy, ta, tb, M, N, K, ep, s);
+  } else if (mode == 2) {
+    GeluLut lut;
+    int lrc = ensure_gelu_lut(nullptr, pow_mode, &lut);
+    if (lrc != B200T5_OK) return lrc;
+    EpiGeglu::Params ep{Cb, N / 2, lut};
+    e = run_gemm_2cta<EpiGeglu>(&dummy, ta, tb, M, N, K, ep, s);
+  } else if (mode == 3) {
+    EpiCrossKV::Params ep{Cb, B, H, S, row_b, row_s};
+    e = run_gemm_2cta<EpiCrossKV>(&dummy, ta, tb, M, N, K, ep, s);
+  }
+  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_enc_gemm(kernel=%d, mode=%d): %s", kernel, mode, cudaGetErrorString(e));
   return B200T5_OK;
 #endif
 }

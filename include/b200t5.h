@@ -149,7 +149,9 @@ int b200t5_bench_cross_attn(b200t5_handle h, int reps, int rows_per_launch, floa
  * "xattn_stages" (8 KB ring stages per CTA), "xattn_late_pdl", "xattn_serialize", "xattn_l2pf", "pdl", "admit_overlap",
  * "sk_stages64", "sk_stages128" (pipeline stages of
  * the split-K decode GEMM tiles, 0 = default), "profile_xattn" (1 = every cross-attention launch inside the step graph
- * records %globaltimer stamps; never on in a timed region). */
+ * records %globaltimer stamps; never on in a timed region), "enc_gemm" (the 128 x 256 encoder GEMMs: 1 = default,
+ * epilogue warps drain each tile while the next tile's MMAs run; 0 = the kernel whose epilogue follows each main loop;
+ * bit-identical results; environment variable B200T5_ENC_GEMM at create time). */
 int b200t5_set_option(b200t5_handle h, const char* name, int value);
 /* With "profile_xattn" on: mean in-situ duration (first CTA start to last CTA end) of the cross-attention launches the
  * step graph made since the option was set, how many there were, and the algorithmic bytes of one such launch; and,
@@ -183,6 +185,12 @@ int b200t5_relative_bucket(int relative_position, int bidirectional, int num_buc
  * bn = 512 selects the encoder configuration (128 x 256 tiles, weight in 128-row boxes, GeGLU interleave per 128), modes 0-2. */
 int b200t5_test_gemm(int device, const void* A, const void* W, void* C, int M, int N, int K, int bn, int mode,
                      int pow_mode, void* stream);
+/* The 128 x 256 encoder GEMM as the encoder launches it; kernel 0 = the kernel whose epilogue follows each main loop,
+ * 1 = the epilogue-overlapped kernel (option "enc_gemm"). mode 0 plain, 1 += residual R (in C), 2 GeGLU (W rows
+ * interleaved per 128, C is [M,N/2]), 3 cross-attention K/V scatter: C is the arena [N/(H*64)][B][H][S][64] and row m
+ * is position row_s[m] of prompt row_b[m] (both NULL: m = b*S + s, M = B*S). B, H, S are read in mode 3 only. */
+int b200t5_test_enc_gemm(int device, const void* A, const void* W, void* C, int M, int N, int K, int kernel, int mode,
+                         int pow_mode, const int* row_b, const int* row_s, int B, int H, int S, void* stream);
 /* Same contract through the cluster split-K kernel the decode step uses (csrc/gemm_splitk.cuh):
  * bn in {64,128}; split in {1,2,4,8} CTAs per cluster along K (reduced automatically when K has
  * fewer 64-wide k-blocks); mode 0 plain, 1 += residual (in C), 2 GeGLU, 4 decoder QKV: C is the q

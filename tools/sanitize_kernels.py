@@ -54,6 +54,23 @@ def main():
             _lib.check(lib.b200t5_test_gemm(DEV, P(A), P(W), P(out), M, N, K, bn, 0, 0, None))
             torch.cuda.synchronize()
             close(out, A.float() @ W.float().T)
+    if section("enc_gemm"):
+        # both 128 x 256 encoder kernels, every encoder epilogue; 18 x 8-9 tiles exceed the SM count, so some CTAs take
+        # a second tile and the staging-buffer handshake turns over
+        M, K, H, Bx, Sx = 2200, 64, 2, 4, 550
+        A = rnd(M, K)
+        for mode, N in ((0, 2056), (1, 2048), (2, 2048), (3, 2048)):
+            W = rnd(N, K, seed=mode)
+            outs = []
+            for kernel in (0, 1):
+                if mode == 3:
+                    out = torch.zeros(N // (H * 64), Bx, H, Sx, 64, device="cuda", dtype=torch.bfloat16)
+                else:
+                    out = rnd(M, N // 2 if mode == 2 else N, seed=7)
+                _lib.check(lib.b200t5_test_enc_gemm(DEV, P(A), P(W), P(out), M, N, K, kernel, mode, 0, None, None, Bx, H, Sx, None))
+                torch.cuda.synchronize()
+                outs.append(out)
+            assert torch.equal(outs[0], outs[1])
     if section("splitk"):
         for bn, split, mode, (M, N, K) in ((64, 4, 0, (130, 192, 256)), (64, 2, 1, (37, 128, 128)), (128, 2, 0, (130, 264, 128)),
                                            (64, 8, 1, (256, 64, 512)), (64, 1, 0, (16, 64, 64))):
