@@ -53,6 +53,24 @@ class GenParams(C.Structure):
     ]
 
 
+class LogitsParams(C.Structure):
+    _fields_ = [
+        ("repetition_penalty", C.c_double),
+        ("encoder_repetition_penalty", C.c_double),
+        ("no_repeat_ngram_size", C.c_int32),
+        ("encoder_no_repeat_ngram_size", C.c_int32),
+        ("suppress_tokens", C.c_void_p),
+        ("n_suppress_tokens", C.c_int32),
+        ("begin_suppress_tokens", C.c_void_p),
+        ("n_begin_suppress_tokens", C.c_int32),
+        ("eos_token_ids", C.c_void_p),
+        ("n_eos_token_ids", C.c_int32),
+        ("bad_words_ids", C.c_void_p),
+        ("bad_words_offsets", C.c_void_p),
+        ("n_bad_words", C.c_int32),
+    ]
+
+
 class Stats(C.Structure):
     _fields_ = [
         ("encoder_ms", C.c_float),
@@ -79,11 +97,17 @@ SIGNATURES = {
     "b200t5_generate": (_i, [_vp, _i64p, _i64p, _i, _i, C.POINTER(GenParams), _i64p, _i32p, _vp]),
     "b200t5_generate_host": (_i, [_vp, _i64p, _i64p, _i, _i, C.POINTER(GenParams), _i64p, _i32p]),
     "b200t5_generate_stream": (_i, [_vp, _i64p, _i64p, C.c_int64, _i, C.POINTER(GenParams), _i, _i, _i64p, _i32p]),
+    "b200t5_generate_ex": (_i, [_vp, _i64p, _i64p, _i, _i, C.POINTER(GenParams), C.POINTER(LogitsParams), _i64p, _i32p, _vp]),
+    "b200t5_generate_host_ex": (_i, [_vp, _i64p, _i64p, _i, _i, C.POINTER(GenParams), C.POINTER(LogitsParams), _i64p, _i32p]),
+    "b200t5_generate_stream_ex": (_i, [_vp, _i64p, _i64p, C.c_int64, _i, C.POINTER(GenParams), C.POINTER(LogitsParams), _i, _i,
+                                       _i64p, _i32p]),
     "b200t5_get_stats": (_i, [_vp, C.POINTER(Stats)]),
     "b200t5_bench_cross_attn": (_i, [_vp, _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_double), _vp]),
     "b200t5_set_option": (_i, [_vp, C.c_char_p, _i]),
     "b200t5_get_xattn_profile": (_i, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_int64), C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "b200t5_test_lm_argmax": (_i, [_i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "b200t5_test_lm_process": (_i, [_i, _vp, _vp, _i, _i, _i, _i, _i, _i, C.POINTER(LogitsParams), _i64p, _i64p, _i, _i64p,
+                                    _vp, _vp]),
     "b200t5_encode": (_i, [_vp, _i64p, _i64p, _i, _i, _vp, _vp]),
     "b200t5_decode_logits": (_i, [_vp, _i64p, _i64p, _i, _i, _i64p, _i, _vp, _vp]),
     "b200t5_relative_bucket": (_i, [_i, _i, _i, _i]),

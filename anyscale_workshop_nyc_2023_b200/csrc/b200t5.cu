@@ -14,6 +14,7 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
 #include <map>
 #include <memory>
 #include <string>
@@ -178,7 +179,7 @@ struct DevBuf {
 };
 
 // Which epilogue/tile a GEMM uses.
-enum GemmKind { G_STORE256, G_RES256, G_GEGLU256, G_CROSSKV256, G_QKVDEC64, G_STORE32, G_RES32, G_GEGLU64, G_ARGMAX128, G_LOGITS128 };
+enum GemmKind { G_STORE256, G_RES256, G_GEGLU256, G_CROSSKV256, G_QKVDEC64, G_STORE32, G_RES32, G_GEGLU64, G_ARGMAX128, G_LOGITS128, G_ARGMAXPROC128 };
 
 struct GemmOp {
   CUtensorMap tmA, tmB;
@@ -200,6 +201,78 @@ struct DecLayerW {
 
 constexpr int kMaxChains = 8;
 constexpr int kStepsPerGraph = 8;
+
+// Host form of a call's logits processors (b200t5_logits_params after validation; logits_process.cuh).
+struct ProcHost {
+  bool on = false;
+  ProcCfg cfg{};
+  std::vector<uint32_t> stat;        // [3][W]: suppressed + one-token bad words, begin-suppressed, EOS ids
+  std::vector<int> bad_ids, bad_off;  // bad words of two or more tokens
+};
+
+// Device state of the processors for `rows` rows (logits_process.cuh: ProcDev). The step graph bakes these
+// addresses: a reallocation means a new graph.
+struct ProcBufs {
+  DevBuf cfg, seen, enc, banned, stat, list, cnt, enc_ids, bad_ids, bad_off;
+  int rows = 0, S = 0, W = 0, ban_cap = 0;
+  size_t n_bad_ids = 0, n_bad_off = 0;
+  bool fits(int r, int s, int w, int cap, size_t nbi, size_t nbo) const {
+    return cfg.p && rows == r && S == s && W == w && ban_cap >= cap && n_bad_ids >= nbi && n_bad_off >= nbo;
+  }
+  cudaError_t alloc(int r, int s, int w, int cap, size_t nbi, size_t nbo) {
+    rows = r;
+    S = s;
+    W = w;
+    ban_cap = cap;
+    n_bad_ids = nbi;
+    n_bad_off = nbo;
+    const size_t bm = static_cast<size_t>(r) * w * 4;
+    cudaError_t e = cudaSuccess;
+    if (e == cudaSuccess) e = cfg.alloc(sizeof(ProcCfg));
+    if (e == cudaSuccess) e = seen.alloc(bm);
+    if (e == cudaSuccess) e = enc.alloc(bm);
+    if (e == cudaSuccess) e = banned.alloc(bm);
+    if (e == cudaSuccess) e = stat.alloc(static_cast<size_t>(3) * w * 4);
+    if (e == cudaSuccess) e = list.alloc(static_cast<size_t>(r) * cap * 4);
+    if (e == cudaSuccess) e = cnt.alloc(static_cast<size_t>(r) * 4);
+    if (e == cudaSuccess) e = enc_ids.alloc(static_cast<size_t>(r) * s * 4);
+    if (e == cudaSuccess) e = bad_ids.alloc(nbi * 4);
+    if (e == cudaSuccess) e = bad_off.alloc(nbo * 4);
+    if (e != cudaSuccess && cfg.p) {  // fits() is false until a complete allocation
+      cudaFree(cfg.p);
+      cfg.p = nullptr;
+    }
+    return e;
+  }
+  ProcDev dev(int row0 = 0) const {
+    ProcDev d;
+    d.cfg = cfg.as<ProcCfg>();
+    d.seen = seen.as<uint32_t>();
+    d.enc = enc.as<uint32_t>();
+    d.banned = banned.as<uint32_t>();
+    d.stat = stat.as<uint32_t>();
+    d.ban_list = list.as<int>();
+    d.ban_cnt = cnt.as<int>();
+    d.enc_ids = enc_ids.as<int>();
+    d.bad_ids = bad_ids.as<int>();
+    d.bad_off = bad_off.as<int>();
+    d.ban_cap = ban_cap;
+    d.S = S;
+    d.W = W;
+    d.row0 = row0;
+    return d;
+  }
+  // a call's values; pageable sources: each copy has left the host buffer when it returns
+  cudaError_t upload(const ProcHost& ph, cudaStream_t s) {
+    cudaError_t e = cudaMemcpyAsync(cfg.p, &ph.cfg, sizeof(ProcCfg), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(stat.p, ph.stat.data(), ph.stat.size() * 4, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && !ph.bad_ids.empty())
+      e = cudaMemcpyAsync(bad_ids.p, ph.bad_ids.data(), ph.bad_ids.size() * 4, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && !ph.bad_off.empty())
+      e = cudaMemcpyAsync(bad_off.p, ph.bad_off.data(), ph.bad_off.size() * 4, cudaMemcpyHostToDevice, s);
+    return e;
+  }
+};
 
 struct Plan {
   int B = 0, S = 0, Tmax = 0;
@@ -225,6 +298,10 @@ struct Plan {
   // slot pool (b200t5_generate_stream): per-slot position and result row, admission lists, [N, Tmax+1] results
   DevBuf pos, out_row, admit;
   DevBuf stream_out, stream_len;
+  // logits processors (allocated by the first call that uses them); proc_on: this call's step runs EpiArgmaxProc
+  ProcBufs proc;
+  bool proc_on = false;
+  int g_proc = -1;
   size_t stream_cap = 0;   // rows stream_out / stream_len hold (the step graph bakes their addresses)
   bool stream_mode = false;
   int g_stream = -1;
@@ -410,6 +487,8 @@ static cudaError_t run_gemm(b200t5_ctx* h, const GemmOp& g, const void* ep, cuda
       return launch_gemm<128, EpiArgmax>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiArgmax::Params*>(ep), h->num_sms, s, pdl);
     case G_LOGITS128:
       return launch_gemm<128, EpiStoreF32>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiStoreF32::Params*>(ep), h->num_sms, s, pdl);
+    case G_ARGMAXPROC128:
+      return launch_gemm<128, EpiArgmaxProc>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiArgmaxProc::Params*>(ep), h->num_sms, s, pdl);
   }
   return cudaErrorInvalidValue;
 }
@@ -468,7 +547,7 @@ static cudaError_t init_kernel_attrs() {
 #define PREP(BN, EPI)                         \
   if ((e = prepare_gemm<BN, EPI>()) != cudaSuccess) return e;
   PREP(256, EpiStore) PREP(256, EpiResidual) PREP(256, EpiGeglu) PREP(256, EpiCrossKV) PREP(64, EpiQkvDecode)
-  PREP(32, EpiStore) PREP(32, EpiResidual) PREP(64, EpiGeglu) PREP(128, EpiArgmax) PREP(128, EpiStoreF32)
+  PREP(32, EpiStore) PREP(32, EpiResidual) PREP(64, EpiGeglu) PREP(128, EpiArgmax) PREP(128, EpiStoreF32) PREP(128, EpiArgmaxProc)
   PREP(64, EpiStore) PREP(128, EpiStore)
 #undef PREP
   if ((e = prepare_gemm_2cta<EpiStore>()) != cudaSuccess) return e;
@@ -1289,14 +1368,21 @@ static int chain_head(b200t5_ctx* h, cudaStream_t s, const ChainView& v, float* 
     int* pidx = p.pidx.as<int>() + static_cast<size_t>(v.b0) * p.n_vtiles;
     const bool sm = p.stream_mode;
     EpiArgmax::Params ep{pval, pidx, p.n_vtiles, sm ? p.pos.as<int>() + v.b0 : &st->step, static_cast<int>(eos), min_new, sm ? 1 : 0};
-    CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, G_ARGMAX128, 1), &ep, s, pdl));
+    const ProcDev pd = p.proc_on ? p.proc.dev(v.b0) : ProcDev();
+    if (p.proc_on) {
+      EpiArgmaxProc::Params epp{ep, pd, nullptr, 0};
+      CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, G_ARGMAXPROC128, 1), &epp, s, pdl));
+    } else {
+      CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, G_ARGMAX128, 1), &ep, s, pdl));
+    }
     // static batch: rows b0.. of the plan's [B, T+1] result; slot pool: row out_row[slot] of the [N, T+1] result
     long long* oid = sm ? p.stream_out.as<long long>() : p.out_ids.as<long long>() + static_cast<size_t>(v.b0) * (T + 1);
     int* olen = sm ? p.stream_len.as<int>() : p.out_len.as<int>() + v.b0;
-    CU_OK(h, launch_kernel(finalize_step_kernel, dim3(v.nb), dim3(128), 0, s, pdl, pval, pidx, p.n_vtiles, st,
-                           p.unfinished.as<int>() + v.b0, oid, olen, T + 1, eos, pad, h->shared.as<act_t>(), v.dx, d,
-                           p.live_extent.as<int>() + v.b0, sm ? p.pos.as<int>() + v.b0 : static_cast<int*>(nullptr),
-                           sm ? p.out_row.as<int>() + v.b0 : static_cast<const int*>(nullptr), T));
+    CU_OK(h, launch_kernel(p.proc_on ? finalize_step_kernel<true> : finalize_step_kernel<false>, dim3(v.nb), dim3(128), 0, s,
+                           pdl, pval, pidx, p.n_vtiles, st, p.unfinished.as<int>() + v.b0, oid, olen, T + 1, eos, pad,
+                           h->shared.as<act_t>(), v.dx, d, p.live_extent.as<int>() + v.b0,
+                           sm ? p.pos.as<int>() + v.b0 : static_cast<int*>(nullptr),
+                           sm ? p.out_row.as<int>() + v.b0 : static_cast<const int*>(nullptr), T, pd));
     h->launches++;
   }
   return B200T5_OK;
@@ -1375,7 +1461,8 @@ static int run_decode_step(b200t5_ctx* h, cudaStream_t s, bool fork, float* logi
   return B200T5_OK;
 }
 
-// Graph of one decode step; eos/pad/min_new are baked in, so the graph is rebuilt when they change.
+// Graph of one decode step; eos/pad/min_new are baked in, so the graph is rebuilt when they change. Whether logits
+// processors run is baked in too (their values are read from device memory at replay).
 // The cross-attention kernel is baked in as well: `fill` = valid prompt tokens / (B * S) of the batch at hand.
 constexpr double kXattnStreamFill = 0.9;
 static int pick_xattn(const b200t5_ctx* h, double fill) {
@@ -1385,7 +1472,8 @@ static int ensure_graph(b200t5_ctx* h, long long eos, long long pad, int min_new
   Plan& p = *h->plan;
   const int want = pick_xattn(h, fill);
   p.xattn_stream = want != 0;
-  if (p.gexec && p.g_eos == eos && p.g_pad == pad && p.g_min_new == min_new && p.g_stream == (p.stream_mode ? 1 : 0) && p.g_xattn == want)
+  if (p.gexec && p.g_eos == eos && p.g_pad == pad && p.g_min_new == min_new && p.g_stream == (p.stream_mode ? 1 : 0) && p.g_xattn == want &&
+      p.g_proc == (p.proc_on ? 1 : 0))
     return B200T5_OK;
   if (p.gexec) cudaGraphExecDestroy(p.gexec);
   if (p.graph) cudaGraphDestroy(p.graph);
@@ -1412,6 +1500,7 @@ static int ensure_graph(b200t5_ctx* h, long long eos, long long pad, int min_new
   p.g_min_new = min_new;
   p.g_stream = p.stream_mode ? 1 : 0;
   p.g_xattn = want;
+  p.g_proc = p.proc_on ? 1 : 0;
   return B200T5_OK;
 }
 
@@ -1420,6 +1509,105 @@ static int validate(b200t5_ctx* h, int B, int S, const b200t5_gen_params* gp) {
   if (!h->finalized) return fail(h, B200T5_ESTATE, "model not finalized");
   if (B < 1 || S < 1 || B > 65535) return fail(h, B200T5_EINVAL, "bad batch shape B=%d S=%d", B, S);
   if (gp && (gp->max_new_tokens < 1 || gp->max_new_tokens > 4096)) return fail(h, B200T5_EINVAL, "max_new_tokens=%d out of range", gp->max_new_tokens);
+  return B200T5_OK;
+}
+
+// b200t5_logits_params -> ProcHost, with transformers' argument checks (ValueError there, B200T5_EINVAL here).
+// NULL, or values that change nothing (penalties 1.0, n-gram sizes 0, no ids, EOS list = {eos}), leave ph->on false.
+static int parse_logits_params(b200t5_ctx* h, int V, const b200t5_logits_params* lp, long long eos, ProcHost* ph) {
+  *ph = ProcHost();
+  if (!lp) return B200T5_OK;
+  const int W = (V + 31) / 32;
+  ProcCfg& c = ph->cfg;
+  ph->stat.assign(static_cast<size_t>(3) * W, 0u);
+  bool on = false;
+  if (!(lp->repetition_penalty > 0) || !(lp->encoder_repetition_penalty > 0))
+    return fail(h, B200T5_EINVAL, "repetition penalties must be > 0 (got %g, %g)", lp->repetition_penalty, lp->encoder_repetition_penalty);
+  if (lp->repetition_penalty != 1.0) {
+    c.rep_pen = 1;
+    c.rep_neg = static_cast<float>(lp->repetition_penalty);
+    c.rep_pos = static_cast<float>(1.0 / lp->repetition_penalty);
+    on = true;
+  }
+  if (lp->encoder_repetition_penalty != 1.0) {
+    c.enc_pen = 1;
+    const double pe = 1.0 / lp->encoder_repetition_penalty;  // transformers stores the encoder penalty inverted
+    c.enc_neg = static_cast<float>(pe);
+    c.enc_pos = static_cast<float>(1.0 / pe);
+    on = true;
+  }
+  if (lp->no_repeat_ngram_size < 0 || lp->encoder_no_repeat_ngram_size < 0)
+    return fail(h, B200T5_EINVAL, "n-gram sizes must be >= 0");
+  c.ngram = lp->no_repeat_ngram_size;
+  c.enc_ngram = lp->encoder_no_repeat_ngram_size;
+  on = on || c.ngram > 0 || c.enc_ngram > 0;
+  auto mark = [&](int which, const int32_t* ids, int n, const char* what) -> int {
+    if (n < 0 || (n > 0 && !ids)) return fail(h, B200T5_EINVAL, "bad %s list", what);
+    for (int i = 0; i < n; ++i) {
+      if (ids[i] < 0 || ids[i] >= V) return fail(h, B200T5_EINVAL, "%s id %d outside [0, %d)", what, ids[i], V);
+      ph->stat[static_cast<size_t>(which) * W + (ids[i] >> 5)] |= 1u << (ids[i] & 31);
+      on = true;
+    }
+    return B200T5_OK;
+  };
+  TRY(mark(0, lp->suppress_tokens, lp->n_suppress_tokens, "suppress_tokens"));
+  TRY(mark(1, lp->begin_suppress_tokens, lp->n_begin_suppress_tokens, "begin_suppress_tokens"));
+  if (lp->n_eos_token_ids < 0 || lp->n_eos_token_ids > kProcMaxEos || (lp->n_eos_token_ids > 0 && !lp->eos_token_ids))
+    return fail(h, B200T5_EINVAL, "eos_token_ids: 0..%d ids", kProcMaxEos);
+  if (lp->n_eos_token_ids == 0) {
+    if (eos >= 0 && eos < V) c.eos[c.n_eos++] = static_cast<int>(eos);
+  } else {
+    for (int i = 0; i < lp->n_eos_token_ids; ++i) {
+      const int e = lp->eos_token_ids[i];
+      if (e < 0 || e >= V) return fail(h, B200T5_EINVAL, "eos id %d outside [0, %d)", e, V);
+      if (e != eos) on = true;
+      c.eos[c.n_eos++] = e;
+    }
+  }
+  for (int i = 0; i < c.n_eos; ++i) ph->stat[static_cast<size_t>(2) * W + (c.eos[i] >> 5)] |= 1u << (c.eos[i] & 31);
+  const int nb = lp->n_bad_words;
+  if (nb < 0 || (nb > 0 && (!lp->bad_words_ids || !lp->bad_words_offsets)) || (nb > 0 && lp->bad_words_offsets[0] != 0))
+    return fail(h, B200T5_EINVAL, "bad_words: bad offsets");
+  for (int i = 0; i < nb; ++i) {
+    const int lo = lp->bad_words_offsets[i], hi = lp->bad_words_offsets[i + 1];
+    if (hi <= lo) return fail(h, B200T5_EINVAL, "bad_words: sequence %d is empty", i);
+    for (int k = lo; k < hi; ++k)
+      if (lp->bad_words_ids[k] < 0 || lp->bad_words_ids[k] >= V)
+        return fail(h, B200T5_EINVAL, "bad_words: id %d outside [0, %d)", lp->bad_words_ids[k], V);
+    if (hi - lo == 1) {
+      const int tok = lp->bad_words_ids[lo];
+      bool is_eos = false;
+      for (int q = 0; q < c.n_eos; ++q) is_eos = is_eos || c.eos[q] == tok;
+      if (is_eos) continue;  // transformers drops [eos] from bad_words_ids
+      ph->stat[tok >> 5] |= 1u << (tok & 31);
+    } else {
+      if (ph->bad_off.empty()) ph->bad_off.push_back(0);
+      ph->bad_ids.insert(ph->bad_ids.end(), lp->bad_words_ids + lo, lp->bad_words_ids + hi);
+      ph->bad_off.push_back(static_cast<int>(ph->bad_ids.size()));
+    }
+    c.bad_add = 1;
+    on = true;
+  }
+  c.n_bad = ph->bad_off.empty() ? 0 : static_cast<int>(ph->bad_off.size()) - 1;
+  ph->on = on;
+  return B200T5_OK;
+}
+
+// Make the plan's processor state fit this call and queue its values on `s` (before the step graph is captured or
+// launched). A reallocation drops the step graph, which bakes the addresses.
+static int setup_proc(b200t5_ctx* h, const ProcHost& ph, cudaStream_t s) {
+  Plan& p = *h->plan;
+  p.proc_on = ph.on;
+  if (!ph.on) return B200T5_OK;
+  const int W = (h->c.V + 31) / 32;
+  const int cap = std::min(W * 32, p.Tmax + 1 + p.S + ph.cfg.n_bad);  // distinct bans of one step, at most
+  if (!p.proc.fits(p.B, p.S, W, cap, ph.bad_ids.size(), ph.bad_off.size())) {
+    CU_OK(h, cudaStreamSynchronize(s));
+    CU_OK(h, p.proc.alloc(p.B, p.S, W, std::max(cap, p.proc.ban_cap), std::max<size_t>(ph.bad_ids.size(), 2 * p.proc.n_bad_ids),
+                          std::max<size_t>(ph.bad_off.size(), 2 * p.proc.n_bad_off)));
+    p.g_proc = -1;
+  }
+  CU_OK(h, p.proc.upload(ph, s));
   return B200T5_OK;
 }
 
@@ -1448,7 +1636,7 @@ static void fill_stats_model(b200t5_ctx* h, int steps) {
 }
 
 static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* mask, int B, int S,
-                         const b200t5_gen_params* gp, long long* out_ids, int* out_len, cudaStream_t s) {
+                         const b200t5_gen_params* gp, const ProcHost& ph, long long* out_ids, int* out_len, cudaStream_t s) {
   const Cfg& c = h->c;
   const long long eos = gp->eos_token_id >= 0 ? gp->eos_token_id : c.eos;
   const long long pad = gp->pad_token_id >= 0 ? gp->pad_token_id : c.pad;
@@ -1460,6 +1648,7 @@ static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* m
   TRY(ensure_plan(h, B, S, T));
   Plan& p = *h->plan;
   p.stream_mode = false;
+  TRY(setup_proc(h, ph, s));
   h->launches = 0;
   CU_OK(h, cudaEventRecord(h->ev[0], s));
   TRY(run_encoder(h, ids, mask, s));
@@ -1471,6 +1660,10 @@ static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* m
   decode_init_kernel<<<B, 128, 0, s>>>(p.state.as<DecodeState>(), p.unfinished.as<int>(), p.out_ids.as<long long>(),
                                        p.out_len.as<int>(), T + 1, B, start, pad, h->shared.as<act_t>(), p.dx.as<res_t>(), c.d);
   h->launches++;
+  if (p.proc_on) {
+    proc_reset_kernel<<<B, 128, 0, s>>>(p.proc.dev(), nullptr, ids, p.out_ids.as<long long>(), T + 1, nullptr, 1);
+    h->launches++;
+  }
   CU_OK(h, cudaGetLastError());
   CU_OK(h, cudaEventRecord(h->ev[1], s));
   int steps = 0;
@@ -1501,19 +1694,39 @@ static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* m
   return B200T5_OK;
 }
 
-extern "C" int b200t5_generate(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
-                               const b200t5_gen_params* params, int64_t* out_ids, int32_t* out_len, void* stream) {
+static long long call_eos(const b200t5_ctx* h, const b200t5_gen_params* gp) {
+  return gp->eos_token_id >= 0 ? gp->eos_token_id : h->c.eos;
+}
+
+extern "C" int b200t5_generate_ex(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                                  const b200t5_gen_params* params, const b200t5_logits_params* logits, int64_t* out_ids,
+                                  int32_t* out_len, void* stream) {
   TRY(validate(h, B, S, params));
   if (!params || !input_ids || !out_ids || !out_len) return fail(h, B200T5_EINVAL, "null argument");
+  ProcHost ph;
+  TRY(parse_logits_params(h, h->c.V, logits, call_eos(h, params), &ph));
   CU_OK(h, cudaSetDevice(h->device));
   return generate_impl(h, reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(attention_mask),
-                       B, S, params, reinterpret_cast<long long*>(out_ids), out_len, static_cast<cudaStream_t>(stream));
+                       B, S, params, ph, reinterpret_cast<long long*>(out_ids), out_len, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b200t5_generate(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                               const b200t5_gen_params* params, int64_t* out_ids, int32_t* out_len, void* stream) {
+  return b200t5_generate_ex(h, input_ids, attention_mask, B, S, params, nullptr, out_ids, out_len, stream);
 }
 
 extern "C" int b200t5_generate_host(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B,
                                     int S, const b200t5_gen_params* params, int64_t* out_ids, int32_t* out_len) {
+  return b200t5_generate_host_ex(h, input_ids, attention_mask, B, S, params, nullptr, out_ids, out_len);
+}
+
+extern "C" int b200t5_generate_host_ex(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B,
+                                       int S, const b200t5_gen_params* params, const b200t5_logits_params* logits,
+                                       int64_t* out_ids, int32_t* out_len) {
   TRY(validate(h, B, S, params));
   if (!params || !input_ids || !out_ids || !out_len) return fail(h, B200T5_EINVAL, "null argument");
+  ProcHost ph;
+  TRY(parse_logits_params(h, h->c.V, logits, call_eos(h, params), &ph));
   CU_OK(h, cudaSetDevice(h->device));
   TRY(ensure_plan(h, B, S, params->max_new_tokens));
   Plan& p = *h->plan;
@@ -1531,7 +1744,7 @@ extern "C" int b200t5_generate_host(b200t5_handle h, const int64_t* input_ids, c
   CU_OK(h, tmp_ids.alloc(static_cast<size_t>(B) * (T + 1) * 8));
   CU_OK(h, tmp_len.alloc(static_cast<size_t>(B) * 4));
   TRY(generate_impl(h, p.ids_dev.as<long long>(), attention_mask ? p.mask_dev.as<long long>() : nullptr, B, S, params,
-                    tmp_ids.as<long long>(), tmp_len.as<int>(), s));
+                    ph, tmp_ids.as<long long>(), tmp_len.as<int>(), s));
   CU_OK(h, cudaMemcpyAsync(p.h_out, tmp_ids.p, static_cast<size_t>(B) * (T + 1) * 8, cudaMemcpyDeviceToHost, s));
   CU_OK(h, cudaMemcpyAsync(p.h_len, tmp_len.p, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToHost, s));
   CU_OK(h, cudaStreamSynchronize(s));
@@ -1552,8 +1765,16 @@ extern "C" int b200t5_generate_host(b200t5_handle h, const int64_t* input_ids, c
 extern "C" int b200t5_generate_stream(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int64_t N,
                                       int S, const b200t5_gen_params* gp, int pool, int admit_min, int64_t* out_ids,
                                       int32_t* out_len) {
+  return b200t5_generate_stream_ex(h, input_ids, attention_mask, N, S, gp, nullptr, pool, admit_min, out_ids, out_len);
+}
+
+extern "C" int b200t5_generate_stream_ex(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int64_t N,
+                                         int S, const b200t5_gen_params* gp, const b200t5_logits_params* logits, int pool,
+                                         int admit_min, int64_t* out_ids, int32_t* out_len) {
   if (!h) return fail(nullptr, B200T5_EINVAL, "null handle");
   if (!gp || !input_ids || !out_ids || !out_len) return fail(h, B200T5_EINVAL, "null argument");
+  ProcHost ph;
+  TRY(parse_logits_params(h, h->c.V, logits, call_eos(h, gp), &ph));
   if (N < 1 || N > (1ll << 30)) return fail(h, B200T5_EINVAL, "bad prompt count N=%lld", static_cast<long long>(N));
   if (pool < 1) pool = 256;
   if (pool > N) pool = static_cast<int>(N);
@@ -1583,6 +1804,7 @@ extern "C" int b200t5_generate_stream(b200t5_handle h, const int64_t* input_ids,
     p.g_stream = -1;
   }
   p.stream_mode = true;
+  TRY(setup_proc(h, ph, s));
   double fill = 1.0;
   if (attention_mask) {  // fill of the first prompts (up to four pools' worth): picks the cross-attention kernel
     const long long rows = N < 4LL * B ? N : 4LL * B;
@@ -1625,6 +1847,11 @@ extern "C" int b200t5_generate_stream(b200t5_handle h, const int64_t* input_ids,
                                          p.key_ok.as<unsigned char>(), p.live_key_ok.as<unsigned char>(), S, start,
                                          h->shared.as<act_t>(), p.dx.as<res_t>(), c.d);
     h->launches++;
+    if (p.proc_on) {  // the admitted slots' processor state, from their prompts (still in ids_dev) and start token
+      proc_reset_kernel<<<k, 128, 0, s>>>(p.proc.dev(), p.admit.as<int>() + B, p.ids_dev.as<long long>(),
+                                          p.stream_out.as<long long>(), T + 1, p.out_row.as<int>(), 1);
+      h->launches++;
+    }
     CU_OK(h, cudaGetLastError());
     CU_OK(h, cudaEventRecord(h->admitted_ev, s));  // the staging buffers may be reused after this point
     for (int b = 0; b < B; ++b)
@@ -2042,14 +2269,66 @@ extern "C" int b200t5_test_lm_argmax(int device, const void* x, const void* W, i
   EpiArgmax::Params ep{pval.as<float>(), pidx.as<int>(), n_tiles, &st.as<DecodeState>()->step, eos, min_new, 0};
   cudaError_t e = run_gemm(&dummy, mk(ta, tb, M, V, K, G_ARGMAX128, 1), &ep, s, false);
   if (e == cudaSuccess)
-    e = launch_kernel(finalize_step_kernel, dim3(M), dim3(128), 0, s, false, pval.as<float>(), pidx.as<int>(), n_tiles, st.as<DecodeState>(),
+    e = launch_kernel(finalize_step_kernel<false>, dim3(M), dim3(128), 0, s, false, pval.as<float>(), pidx.as<int>(), n_tiles, st.as<DecodeState>(),
                       unf.as<int>(), out.as<long long>(), len.as<int>(), out_ld, static_cast<long long>(-1), static_cast<long long>(0),
                       static_cast<const act_t*>(W), xn.as<res_t>(), K, ext.as<int>(), static_cast<int*>(nullptr),
-                      static_cast<const int*>(nullptr), 1 << 30);
+                      static_cast<const int*>(nullptr), 1 << 30, ProcDev());
   if (e == cudaSuccess)
     e = cudaMemcpy2DAsync(tokens, 8, out.as<long long>() + step + 1, static_cast<size_t>(out_ld) * 8, 8, M, cudaMemcpyDeviceToDevice, s);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s);
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_lm_argmax: %s", cudaGetErrorString(e));
+  return B200T5_OK;
+}
+
+// lm_head + logits processors + arg-max exactly as chain_head launches them with processors on: the row state is
+// built by proc_reset_kernel from the given history and prompts, then EpiArgmaxProc and finalize_step_kernel<true>.
+extern "C" int b200t5_test_lm_process(int device, const void* x, const void* W, int M, int V, int K, int step, int eos,
+                                      int min_new, const b200t5_logits_params* logits, const int64_t* hist,
+                                      const int64_t* enc_ids, int S, int64_t* tokens, float* vals, void* stream) {
+  const int sms = hook_device(device);
+  if (sms < 0) return sms;
+  if (!x || !W || !tokens || !hist || !enc_ids || M < 1 || V < 2 || K % 8 || step < 0 || S < 1)
+    return fail(nullptr, B200T5_EINVAL, "test_lm_process: bad argument");
+  ProcHost ph;
+  int rc = parse_logits_params(nullptr, V, logits, eos, &ph);
+  if (rc != B200T5_OK) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUtensorMap ta, tb;
+  if (!make_tmap(&ta, x, M, K, 128) || !make_tmap(&tb, W, V, K, 128)) return fail(nullptr, B200T5_ECUDA, "%s", g_err);
+  const int n_tiles = (V + 127) / 128, out_ld = step + 2, Wd = (V + 31) / 32;
+  DevBuf pval, pidx, st, unf, out, len, xn, ext;
+  ProcBufs pb;
+  if (pval.alloc(static_cast<size_t>(M) * n_tiles * 4) != cudaSuccess || pidx.alloc(static_cast<size_t>(M) * n_tiles * 4) != cudaSuccess ||
+      st.alloc(sizeof(DecodeState)) != cudaSuccess || unf.alloc(static_cast<size_t>(M) * 4) != cudaSuccess ||
+      out.alloc(static_cast<size_t>(M) * out_ld * 8) != cudaSuccess || len.alloc(static_cast<size_t>(M) * 4) != cudaSuccess ||
+      xn.alloc(static_cast<size_t>(M) * K * sizeof(res_t)) != cudaSuccess || ext.alloc(static_cast<size_t>(M) * 4) != cudaSuccess ||
+      pb.alloc(M, S, Wd, std::min(Wd * 32, step + 2 + S + ph.cfg.n_bad), ph.bad_ids.size(), ph.bad_off.size()) != cudaSuccess)
+    return fail(nullptr, B200T5_ENOMEM, "test_lm_process: allocation failed");
+  b200t5_ctx dummy;
+  dummy.num_sms = sms;
+  decode_init_kernel<<<M, 128, 0, s>>>(st.as<DecodeState>(), unf.as<int>(), out.as<long long>(), len.as<int>(), out_ld, M, 0, 0,
+                                       static_cast<const act_t*>(W), xn.as<res_t>(), K);
+  cudaError_t e = cudaMemcpy2DAsync(out.p, static_cast<size_t>(out_ld) * 8, hist, static_cast<size_t>(step + 1) * 8,
+                                    static_cast<size_t>(step + 1) * 8, M, cudaMemcpyDeviceToDevice, s);
+  if (e == cudaSuccess) e = pb.upload(ph, s);
+  if (e == cudaSuccess) {
+    set_state_kernel<<<1, 1, 0, s>>>(st.as<DecodeState>(), step);
+    proc_reset_kernel<<<M, 128, 0, s>>>(pb.dev(), nullptr, reinterpret_cast<const long long*>(enc_ids), out.as<long long>(),
+                                        out_ld, nullptr, step + 1);
+    e = cudaGetLastError();
+  }
+  const ProcDev pd = pb.dev();
+  EpiArgmaxProc::Params ep{{pval.as<float>(), pidx.as<int>(), n_tiles, &st.as<DecodeState>()->step, eos, min_new, 0}, pd, vals, V};
+  if (e == cudaSuccess) e = run_gemm(&dummy, mk(ta, tb, M, V, K, G_ARGMAXPROC128, 1), &ep, s, false);
+  if (e == cudaSuccess)
+    e = launch_kernel(finalize_step_kernel<true>, dim3(M), dim3(128), 0, s, false, pval.as<float>(), pidx.as<int>(), n_tiles, st.as<DecodeState>(),
+                      unf.as<int>(), out.as<long long>(), len.as<int>(), out_ld, static_cast<long long>(-1), static_cast<long long>(0),
+                      static_cast<const act_t*>(W), xn.as<res_t>(), K, ext.as<int>(), static_cast<int*>(nullptr),
+                      static_cast<const int*>(nullptr), 1 << 30, pd);
+  if (e == cudaSuccess)
+    e = cudaMemcpy2DAsync(tokens, 8, out.as<long long>() + step + 1, static_cast<size_t>(out_ld) * 8, 8, M, cudaMemcpyDeviceToDevice, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_lm_process: %s", cudaGetErrorString(e));
   return B200T5_OK;
 }
 

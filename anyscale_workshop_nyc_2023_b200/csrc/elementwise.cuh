@@ -1,6 +1,7 @@
 // Memory-bound row kernels: embedding gather, T5 RMSNorm, mask preparation,
 // per-step arg-max finalisation + stopping bookkeeping.
 #pragma once
+#include "logits_process.cuh"
 #include "ptx.cuh"
 
 namespace b200 {
@@ -288,12 +289,15 @@ __global__ void admit_slots_kernel(const int* __restrict__ slots, const int* __r
 // Slot-pool mode (pos != nullptr, b200t5_generate_stream): every slot has its own position pos[b] and writes to
 // row out_row[b] of an [N, out_ld] result; a slot also finishes when it has emitted max_new tokens, idle slots
 // (unfinished == 0) write nothing and stay at position 0.
+// kProc (logits processors active): a row finishes on any of the call's EOS ids, and a row that goes on marks its
+// token as seen and computes the bans of its next step (logits_process.cuh).
+template <bool kProc>
 __global__ void finalize_step_kernel(const float* __restrict__ pval, const int* __restrict__ pidx, int n_tiles,
                                      DecodeState* st, int* __restrict__ unfinished,
                                      long long* __restrict__ out_ids, int* __restrict__ out_len, int out_ld,
                                      long long eos_tok, long long pad_tok, const act_t* __restrict__ E,
                                      res_t* __restrict__ x, int d, int* __restrict__ live_extent,
-                                     int* __restrict__ pos, const int* __restrict__ out_row, int max_new) {
+                                     int* __restrict__ pos, const int* __restrict__ out_row, int max_new, ProcDev pd) {
   pdl_launch_dependents();
   pdl_wait();
   const int b = blockIdx.x;
@@ -320,6 +324,7 @@ __global__ void finalize_step_kernel(const float* __restrict__ pval, const int* 
   __shared__ float s_v[32];
   __shared__ int s_i[32];
   __shared__ long long s_tok;
+  __shared__ int s_go;
   const int warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
   if (lane_id() == 0) {
     s_v[warp] = best;
@@ -340,7 +345,7 @@ __global__ void finalize_step_kernel(const float* __restrict__ pval, const int* 
     bool fin = false;
     if (unf) {
       out_len[row] = t + 1;
-      fin = tok == eos_tok || (pos != nullptr && t + 1 >= max_new);
+      fin = (kProc ? proc_is_eos(*pd.cfg, tok) : tok == eos_tok) || (pos != nullptr && t + 1 >= max_new);
       if (fin) {
         unfinished[b] = 0;
         live_extent[b] = 0;
@@ -349,11 +354,19 @@ __global__ void finalize_step_kernel(const float* __restrict__ pval, const int* 
     }
     if (pos != nullptr) pos[b] = (unf && !fin) ? t + 1 : 0;
     s_tok = (pos != nullptr && fin) ? pad_tok : tok;
+    if constexpr (kProc) {
+      s_go = unf && !fin;
+      if (unf && !fin && pd.cfg->rep_pen) bit_set(pd.seen + static_cast<size_t>(pd.row0 + b) * pd.W, static_cast<int>(tok));
+    }
   }
   __syncthreads();
   const uint4* src = reinterpret_cast<const uint4*>(E + static_cast<size_t>(s_tok) * d);
   res_t* dst = x + static_cast<size_t>(b) * d;
   for (int i = threadIdx.x; i < d / 8; i += blockDim.x) store_res8_from_act(dst + i * 8, src[i]);
+  if constexpr (kProc) {
+    // the row's decoder ids are now its result row up to column t + 1 (written above, visible after the barrier)
+    if (s_go) proc_new_bans(pd, pd.row0 + b, out_ids + static_cast<size_t>(out_row != nullptr ? out_row[b] : b) * out_ld, t + 2, true);
+  }
 }
 
 // End of a step (joins every chain). With in-situ profiling on, fold the cross-attention launch stamps of this

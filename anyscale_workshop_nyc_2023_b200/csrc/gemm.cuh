@@ -15,6 +15,7 @@
 // so each functor first rounds the fp32 accumulator to bf16 and only then fuses
 // the residual add / GeGLU / KV scatter / arg-max.
 #pragma once
+#include "logits_process.cuh"
 #include "ptx.cuh"
 
 namespace b200 {
@@ -631,6 +632,68 @@ struct EpiArgmax {
     if (m_ok) {
       p.pval[static_cast<size_t>(m) * p.n_tiles + n_tile] = best;
       p.pidx[static_cast<size_t>(m) * p.n_tiles + n_tile] = bidx;
+    }
+  }
+};
+
+// ---- lm_head + logits processors + greedy arg-max (logits_process.cuh): the same (max, lowest index) partials as
+// EpiArgmax, from the logits after transformers' greedy processors. Each logit is rounded to act_t and widened to fp32
+// (HF's `.to(torch.float32)`), then in HF's order: encoder repetition penalty, repetition penalty (on the already
+// penalised value), + 0 when bad words are active (HF adds a zero bias), and -inf where the row's next-step bans, the
+// static mask, the begin-suppress mask (step 0) or the EOS mask (step < min_new) has the column's bit. `vals`
+// (test hook only, else nullptr) receives the processed values [M, ldv].
+struct EpiArgmaxProc {
+  struct Params {
+    EpiArgmax::Params a;
+    ProcDev pd;
+    float* vals;
+    int ldv;
+  };
+  static DEVINL void prologue(const Params&, uint8_t*, int, int = 128) {}
+  template <int BN>
+  static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t*, int part, int) {
+    static_assert(BN % 32 == 0, "one bitmap word per 32 columns");
+    if (part != 0) return;
+    const ProcCfg& cf = *p.pd.cfg;
+    const int W = p.pd.W;
+    const size_t rw = static_cast<size_t>(p.pd.row0 + m) * W;
+    const int t = m_ok ? p.a.step[m * p.a.step_stride] : 1;
+    const bool enc_pen = cf.enc_pen, rep_pen = cf.rep_pen, bad_add = cf.bad_add;
+    const float en = cf.enc_neg, ep = cf.enc_pos, rn = cf.rep_neg, rp = cf.rep_pos;
+    float best = -INFINITY;
+    int bidx = n_tile * BN;
+#pragma unroll 1
+    for (int c = 0; c < BN / 32; ++c) {
+      uint32_t acc[32];
+      acc_ld_32(taddr + c * 32, acc);
+      const int n0 = n_tile * BN + c * 32;
+      const int w = n0 >> 5;
+      uint32_t ban = 0, seen = 0, enc = 0;
+      if (m_ok && w < W) {
+        ban = p.pd.banned[rw + w] | p.pd.stat[w];
+        if (t == 0) ban |= p.pd.stat[W + w];
+        if (t < p.a.min_new) ban |= p.pd.stat[2 * W + w];
+        if (rep_pen) seen = p.pd.seen[rw + w];
+        if (enc_pen) enc = p.pd.enc[rw + w];
+      }
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const int n = n0 + j;
+        float v = act_round(__uint_as_float(acc[j]));
+        if ((enc >> j) & 1u) v = v < 0.f ? v * en : v * ep;
+        if ((seen >> j) & 1u) v = v < 0.f ? v * rn : v * rp;
+        if (bad_add) v = v + 0.f;
+        if (n >= N || ((ban >> j) & 1u)) v = -INFINITY;
+        if (p.vals != nullptr && m_ok && n < N) p.vals[static_cast<size_t>(m) * p.ldv + n] = v;
+        if (v > best) {
+          best = v;
+          bidx = n;
+        }
+      }
+    }
+    if (m_ok) {
+      p.a.pval[static_cast<size_t>(m) * p.a.n_tiles + n_tile] = best;
+      p.a.pidx[static_cast<size_t>(m) * p.a.n_tiles + n_tile] = bidx;
     }
   }
 };

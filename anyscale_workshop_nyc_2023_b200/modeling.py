@@ -35,6 +35,115 @@ _IGNORED_WEIGHTS = ("decoder.block.0.layer.1.EncDecAttention.relative_attention_
 _ALIASES = ("encoder.embed_tokens.weight", "decoder.embed_tokens.weight")
 
 
+# transformers' greedy-mode logits processors the CUDA path applies (b200t5_logits_params, csrc/logits_process.cuh)
+LOGITS_PROCESSOR_KWARGS = ("repetition_penalty", "encoder_repetition_penalty", "no_repeat_ngram_size",
+                           "encoder_no_repeat_ngram_size", "bad_words_ids", "suppress_tokens", "begin_suppress_tokens")
+
+
+class _LogitsArgs:
+    """A validated set of logits processors: the C struct plus the arrays its pointers refer to."""
+
+    def __init__(self, params: _lib.LogitsParams, arrays, eos_ids):
+        self.params = params
+        self._arrays = arrays  # keeps the buffers the struct points to alive
+        self.eos_ids = eos_ids
+
+    def ref(self):
+        return C.byref(self.params)
+
+
+def _eos_ids(eos_token_id):
+    """eos_token_id as a list without repeats (None stays None)."""
+    if eos_token_id is None:
+        return None
+    if isinstance(eos_token_id, torch.Tensor):
+        eos_token_id = eos_token_id.tolist()
+    if isinstance(eos_token_id, (list, tuple)):
+        if not eos_token_id:
+            raise ValueError("eos_token_id must not be an empty list")
+        return list(dict.fromkeys(int(e) for e in eos_token_id))
+    return [int(eos_token_id)]
+
+
+def _id_list(name, v, vocab_size):
+    ids = [int(t) for t in (v.tolist() if isinstance(v, torch.Tensor) else v)]
+    bad = [t for t in ids if t < 0 or t >= vocab_size]
+    if bad:
+        raise ValueError(f"`{name}` contains ids outside [0, {vocab_size}): {bad}")
+    return ids
+
+
+def logits_processor_args(kw: Dict[str, Any], eos_ids, default_eos: int, vocab_size: int) -> Optional[_LogitsArgs]:
+    """Validate the processor kwargs of a generate call as transformers does (ValueError where its processors raise)
+    and build b200t5_logits_params. Returns None when nothing would change greedy decoding: no-op values
+    (repetition_penalty=1.0, no_repeat_ngram_size=0, suppress_tokens=[], ...) count as absent, as in transformers."""
+    p = _lib.LogitsParams(repetition_penalty=1.0, encoder_repetition_penalty=1.0)
+    arrays = []
+    active = False
+
+    def arr(ids):
+        a = np.ascontiguousarray(ids, dtype=np.int32)
+        arrays.append(a)
+        return a.ctypes.data_as(C.c_void_p)
+
+    for name in ("repetition_penalty", "encoder_repetition_penalty"):
+        v = kw.get(name)
+        if v is None:
+            continue
+        v = float(v)
+        if not v > 0:
+            raise ValueError(f"`{name}` has to be a strictly positive float, but is {v}")
+        setattr(p, name, v)
+        active = active or v != 1.0
+    for name in ("no_repeat_ngram_size", "encoder_no_repeat_ngram_size"):
+        v = kw.get(name)
+        if v is None:
+            continue
+        if isinstance(v, bool) or int(v) != v or v < 0:
+            raise ValueError(f"`{name}` has to be a non-negative integer, but is {v}")
+        setattr(p, name, int(v))
+        active = active or int(v) > 0
+    for name, ptr, cnt in (("suppress_tokens", "suppress_tokens", "n_suppress_tokens"),
+                           ("begin_suppress_tokens", "begin_suppress_tokens", "n_begin_suppress_tokens")):
+        v = kw.get(name)
+        if v is None:
+            continue
+        ids = _id_list(name, v, vocab_size)
+        if ids:
+            setattr(p, ptr, arr(ids))
+            setattr(p, cnt, len(ids))
+            active = True
+    eos_list = eos_ids if eos_ids else [default_eos]
+    bw = kw.get("bad_words_ids")
+    if bw is not None:
+        if not isinstance(bw, (list, tuple)) or len(bw) == 0:
+            raise ValueError(f"`bad_words_ids` has to be a non-empty list, but is {bw}.")
+        if any(not isinstance(w, (list, tuple)) for w in bw):
+            raise ValueError(f"`bad_words_ids` has to be a list of lists, but is {bw}.")
+        seqs = []
+        for w in bw:
+            ids = _id_list("bad_words_ids", w, vocab_size)
+            if not ids:
+                raise ValueError(f"`bad_words_ids` contains an empty sequence: {bw}")
+            if len(ids) == 1 and ids[0] in eos_list:
+                continue  # transformers drops [eos] (NoBadWordsLogitsProcessor)
+            seqs.append(ids)
+        if not seqs:  # transformers: the remaining sequence bias must not be empty
+            raise ValueError(f"`bad_words_ids` bans nothing but the EOS token: {bw}")
+        off = np.cumsum([0] + [len(w) for w in seqs])
+        p.bad_words_ids = arr([t for w in seqs for t in w])
+        p.bad_words_offsets = arr(off)
+        p.n_bad_words = len(seqs)
+        active = True
+    if eos_ids is not None and len(eos_ids) > 1:
+        if len(eos_ids) > 16:
+            raise ValueError("at most 16 eos_token_id values are supported")
+        p.eos_token_ids = arr(eos_ids)
+        p.n_eos_token_ids = len(eos_ids)
+        active = True
+    return _LogitsArgs(p, arrays, eos_list) if active else None
+
+
 def _chk(model, rc: int, handle=None) -> None:
     _lib.check(rc, handle, model._lib)
 
@@ -205,10 +314,8 @@ class B200T5ForConditionalGeneration:
             raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
         if min_new_tokens is None:
             min_new_tokens = max(int(min_length) - 1, 0) if min_length else 0
-        if isinstance(eos_token_id, (list, tuple)):
-            if len(eos_token_id) != 1:
-                raise NotImplementedError("multiple eos_token_id values are not supported")
-            eos_token_id = eos_token_id[0]
+        if isinstance(eos_token_id, (list, tuple, torch.Tensor)):
+            eos_token_id = _eos_ids(eos_token_id)[0]  # the rest go to the logits processors (_logits_args)
         return _lib.GenParams(
             max_new_tokens=int(max_new_tokens), min_new_tokens=int(min(min_new_tokens, max_new_tokens)),
             eos_token_id=-1 if eos_token_id is None else int(eos_token_id),
@@ -216,6 +323,10 @@ class B200T5ForConditionalGeneration:
             decoder_start_token_id=-1 if decoder_start_token_id is None else int(decoder_start_token_id),
             poll_interval=int(poll_interval),
         )
+
+    def _logits_args(self, kw: Dict[str, Any], eos_token_id) -> Optional[_LogitsArgs]:
+        default_eos = self.generation_config.eos_token_id
+        return logits_processor_args(kw, _eos_ids(eos_token_id), default_eos, self.config.vocab_size)
 
     @torch.no_grad()
     def generate(self, input_ids=None, attention_mask=None, *, max_new_tokens=None, max_length=None,
@@ -225,14 +336,17 @@ class B200T5ForConditionalGeneration:
         """Greedy `generate`: returns int64 [B, 1+T'] on `self.device`, column 0 the decoder start
         token, rows padded after their EOS, T' = steps until every row finished (<= max_new_tokens).
         `labels` (which the reference passes, JOB/utils.py:31) and other HF kwargs that do not
-        change greedy decoding are accepted and ignored, as HF itself does (generation/utils.py:583)."""
+        change greedy decoding are accepted and ignored, as HF itself does (generation/utils.py:583).
+        transformers' greedy logits processors are applied on the GPU: repetition_penalty,
+        encoder_repetition_penalty, no_repeat_ngram_size, encoder_no_repeat_ngram_size, bad_words_ids,
+        suppress_tokens, begin_suppress_tokens, and eos_token_id given as a list."""
         if input_ids is None:
             input_ids = unused.pop("inputs", None)
         if input_ids is None:
             raise ValueError("input_ids is required")
         if do_sample or (num_beams is not None and num_beams != 1):
             raise NotImplementedError("only greedy decoding (do_sample=False, num_beams=1) is implemented")
-        for k in ("temperature", "top_k", "top_p", "repetition_penalty", "no_repeat_ngram_size", "num_return_sequences"):
+        for k in ("temperature", "top_k", "top_p", "num_return_sequences"):
             v = unused.get(k)
             if v is not None and not (isinstance(v, (int, float)) and v == 1):
                 raise NotImplementedError(f"generate({k}=...) is not supported by the CUDA path")
@@ -241,13 +355,14 @@ class B200T5ForConditionalGeneration:
                 raise NotImplementedError(f"generate({k}=...) is not supported by the CUDA path")
         gp = self._gen_params(max_new_tokens, max_length, min_new_tokens, min_length, eos_token_id, pad_token_id,
                               decoder_start_token_id, poll_interval)
+        lp = self._logits_args(unused, eos_token_id)
         host = torch.as_tensor(input_ids)
         if host.dim() != 2:
             raise ValueError(f"input_ids must be [batch, seq], got {tuple(host.shape)}")
         if self.takes_host_batches(host.shape[0], host.shape[1]) and host.device.type == "cpu":
             # more rows than one pool of decode slots, still in host memory: the slot pool admits prompts from host
             # buffers as slots free up, so nothing is copied to the device (and back) up front
-            return self._generate_pool_from_host(host, attention_mask, gp)
+            return self._generate_pool_from_host(host, attention_mask, gp, lp)
         ids = host.to(device=self._device, dtype=torch.long).contiguous()
         B, S = ids.shape
         if ids.numel():
@@ -260,27 +375,28 @@ class B200T5ForConditionalGeneration:
             if mask.shape != ids.shape:
                 raise ValueError("attention_mask shape must match input_ids")
         else:
-            mask = self._infer_attention_mask(ids, gp)
+            mask = self._infer_attention_mask(ids, gp, lp)
         if B > self.pool_size:
             if self.takes_host_batches(B, S):
                 # more rows than one pool of decode slots: continuous batching, same tokens row for row. The pool
                 # admits prompts from host memory as slots free up (its entry point takes host buffers).
-                out_np, _ = self.generate_stream(ids.cpu().numpy(), None if mask is None else mask.cpu().numpy(), _gen_params=gp)
+                out_np, _ = self.generate_stream(ids.cpu().numpy(), None if mask is None else mask.cpu().numpy(), _gen_params=gp,
+                                                 _logits=lp)
                 return torch.from_numpy(out_np).to(self._device)
             # prompts the slot pool cannot take (it needs the packed encoder, S <= 512): static batches
-            outs = [self._generate_static(ids[lo:lo + self.pool_size], None if mask is None else mask[lo:lo + self.pool_size], gp)
+            outs = [self._generate_static(ids[lo:lo + self.pool_size], None if mask is None else mask[lo:lo + self.pool_size], gp, lp)
                     for lo in range(0, B, self.pool_size)]
             width = max(o.shape[1] for o in outs)
             pad = gp.pad_token_id if gp.pad_token_id >= 0 else self.generation_config.pad_token_id
             return torch.cat([torch.nn.functional.pad(o, (0, width - o.shape[1]), value=pad) for o in outs], dim=0)
-        return self._generate_static(ids, mask, gp)
+        return self._generate_static(ids, mask, gp, lp)
 
     def takes_host_batches(self, B: int, S: int) -> bool:
         """True when a [B, S] batch would go through the slot pool, whose entry point takes HOST buffers: a caller that
         still has the batch in host memory (predictor.py) hands it over as it is."""
         return B > self.pool_size and S <= _POOL_MAX_S and os.environ.get("B200T5_STREAM", "1") != "0"
 
-    def _generate_pool_from_host(self, ids: torch.Tensor, attention_mask, gp) -> torch.Tensor:
+    def _generate_pool_from_host(self, ids: torch.Tensor, attention_mask, gp, lp=None) -> torch.Tensor:
         ids_np = np.ascontiguousarray(ids.numpy(), dtype=np.int64)
         if ids_np.size and (int(ids_np.min()) < 0 or int(ids_np.max()) >= self.config.vocab_size):
             raise IndexError("input_ids contain token ids outside [0, vocab_size)")
@@ -289,24 +405,28 @@ class B200T5ForConditionalGeneration:
             if mask_np.shape != ids_np.shape:
                 raise ValueError("attention_mask shape must match input_ids")
         else:
-            mask_np = self._infer_mask_np(ids_np, gp)
-        out_np, _ = self.generate_stream(ids_np, mask_np, _gen_params=gp)
+            mask_np = self._infer_mask_np(ids_np, gp, lp)
+        out_np, _ = self.generate_stream(ids_np, mask_np, _gen_params=gp, _logits=lp)
         return torch.from_numpy(out_np).to(self._device)
 
-    def _infer_attention_mask(self, ids: torch.Tensor, gp) -> Optional[torch.Tensor]:
-        """GenerationMixin._prepare_attention_mask_for_generation (transformers generation/utils.py): without an
-        attention_mask the pad positions are masked when the pad token occurs in the inputs and is not the EOS
-        token; otherwise every position is attended (None = all ones for the library)."""
+    def _pad_is_eos(self, gp, lp) -> bool:
         pad = gp.pad_token_id if gp.pad_token_id >= 0 else self.generation_config.pad_token_id
         eos = gp.eos_token_id if gp.eos_token_id >= 0 else self.generation_config.eos_token_id
-        if pad is None or pad == eos:
+        return pad is None or pad == eos or (lp is not None and pad in lp.eos_ids)
+
+    def _infer_attention_mask(self, ids: torch.Tensor, gp, lp=None) -> Optional[torch.Tensor]:
+        """GenerationMixin._prepare_attention_mask_for_generation (transformers generation/utils.py): without an
+        attention_mask the pad positions are masked when the pad token occurs in the inputs and is not an EOS
+        token; otherwise every position is attended (None = all ones for the library)."""
+        pad = gp.pad_token_id if gp.pad_token_id >= 0 else self.generation_config.pad_token_id
+        if self._pad_is_eos(gp, lp):
             return None
         is_pad = ids == pad
         if not bool(is_pad.any().item()):
             return None
         return (~is_pad).to(torch.long).contiguous()
 
-    def _generate_static(self, ids: torch.Tensor, mask: Optional[torch.Tensor], gp) -> torch.Tensor:
+    def _generate_static(self, ids: torch.Tensor, mask: Optional[torch.Tensor], gp, lp=None) -> torch.Tensor:
         B, S = ids.shape
         ids = ids.contiguous()
         mask = None if mask is None else mask.contiguous()
@@ -316,62 +436,80 @@ class B200T5ForConditionalGeneration:
             lens = torch.empty((B,), dtype=torch.int32, device=self._device)
             stream = torch.cuda.current_stream(self._device)
             with self._gpu_lock:
-                _chk(self, self._lib.b200t5_generate(self._h, _ptr(ids), _ptr(mask), B, S, C.byref(gp), _ptr(out),
-                                                     _ptr(lens), C.c_void_p(stream.cuda_stream)), self._h)
+                if lp is None:
+                    rc = self._lib.b200t5_generate(self._h, _ptr(ids), _ptr(mask), B, S, C.byref(gp), _ptr(out), _ptr(lens),
+                                                   C.c_void_p(stream.cuda_stream))
+                else:
+                    rc = self._lib.b200t5_generate_ex(self._h, _ptr(ids), _ptr(mask), B, S, C.byref(gp), lp.ref(), _ptr(out),
+                                                      _ptr(lens), C.c_void_p(stream.cuda_stream))
+                _chk(self, rc, self._h)
                 self.last_lengths = lens
                 steps = int(lens.max().item())  # synchronises; HF returns exactly the steps it ran
         return out[:, : steps + 1]
 
-    def _infer_mask_np(self, ids: np.ndarray, gp) -> Optional[np.ndarray]:
+    def _infer_mask_np(self, ids: np.ndarray, gp, lp=None) -> Optional[np.ndarray]:
         pad = gp.pad_token_id if gp.pad_token_id >= 0 else self.generation_config.pad_token_id
-        eos = gp.eos_token_id if gp.eos_token_id >= 0 else self.generation_config.eos_token_id
-        if pad is None or pad == eos or not (ids == pad).any():
+        if self._pad_is_eos(gp, lp) or not (ids == pad).any():
             return None
         return np.ascontiguousarray(ids != pad, dtype=np.int64)
 
     def generate_host(self, input_ids: np.ndarray, attention_mask: Optional[np.ndarray] = None, **kw):
         """numpy in / numpy out through b200t5_generate_host (the foreign-host entry point):
-        H2D copy, generation, D2H copy and synchronisation all happen inside the library."""
+        H2D copy, generation, D2H copy and synchronisation all happen inside the library. Takes the logits
+        processor kwargs `generate` takes (through b200t5_generate_host_ex)."""
         gp = self._gen_params(kw.get("max_new_tokens"), kw.get("max_length"), kw.get("min_new_tokens"),
                               kw.get("min_length"), kw.get("eos_token_id"), kw.get("pad_token_id"),
                               kw.get("decoder_start_token_id"), kw.get("poll_interval", 8))
+        lp = self._logits_args(kw, kw.get("eos_token_id"))
         ids = np.ascontiguousarray(input_ids, dtype=np.int64)
         B, S = ids.shape
-        mask = self._infer_mask_np(ids, gp) if attention_mask is None else np.ascontiguousarray(attention_mask, dtype=np.int64)
+        mask = self._infer_mask_np(ids, gp, lp) if attention_mask is None else np.ascontiguousarray(attention_mask, dtype=np.int64)
         out = np.empty((B, gp.max_new_tokens + 1), dtype=np.int64)
         lens = np.empty((B,), dtype=np.int32)
         with self._gpu_lock:
-            _chk(self, self._lib.b200t5_generate_host(
-                self._h, ids.ctypes.data_as(C.c_void_p), None if mask is None else mask.ctypes.data_as(C.c_void_p), B, S,
-                C.byref(gp), out.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p)), self._h)
+            mp = None if mask is None else mask.ctypes.data_as(C.c_void_p)
+            if lp is None:
+                rc = self._lib.b200t5_generate_host(self._h, ids.ctypes.data_as(C.c_void_p), mp, B, S, C.byref(gp),
+                                                    out.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p))
+            else:
+                rc = self._lib.b200t5_generate_host_ex(self._h, ids.ctypes.data_as(C.c_void_p), mp, B, S, C.byref(gp), lp.ref(),
+                                                       out.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p))
+            _chk(self, rc, self._h)
         return out[:, : int(lens.max()) + 1], lens
 
     def generate_stream(self, input_ids: np.ndarray, attention_mask: Optional[np.ndarray] = None, *, pool: Optional[int] = None,
-                        admit_min: int = 0, _gen_params=None, **kw):
+                        admit_min: int = 0, _gen_params=None, _logits=None, **kw):
         """N prompts through a pool of decode slots (b200t5_generate_stream): a slot whose row has finished is
         refilled with the next prompt, so short answers do not wait for the slowest row of a fixed batch as they do
         when BatchPredictor hands `generate` one batch at a time (NB:908-913 -> JOB/predictor.py:102). Returns
         (int64 [N, 1+T'], int32 lengths [N]) with the rows in input order; every row equals what `generate` returns
-        for that prompt."""
+        for that prompt. Takes the logits processor kwargs `generate` takes (through b200t5_generate_stream_ex)."""
         gp = _gen_params or self._gen_params(kw.get("max_new_tokens"), kw.get("max_length"), kw.get("min_new_tokens"),
                                              kw.get("min_length"), kw.get("eos_token_id"), kw.get("pad_token_id"),
                                              kw.get("decoder_start_token_id"), kw.get("poll_interval", 8))
+        lp = _logits if _gen_params is not None else self._logits_args(kw, kw.get("eos_token_id"))
         ids = np.ascontiguousarray(input_ids, dtype=np.int64)
         if ids.ndim != 2:
             raise ValueError(f"input_ids must be [batch, seq], got {ids.shape}")
         N, S = ids.shape
         if ids.size and (int(ids.min()) < 0 or int(ids.max()) >= self.config.vocab_size):
             raise IndexError("input_ids contain token ids outside [0, vocab_size)")
-        mask = self._infer_mask_np(ids, gp) if attention_mask is None else np.ascontiguousarray(attention_mask, dtype=np.int64)
+        mask = self._infer_mask_np(ids, gp, lp) if attention_mask is None else np.ascontiguousarray(attention_mask, dtype=np.int64)
         if mask is not None and mask.shape != ids.shape:
             raise ValueError("attention_mask shape must match input_ids")
         out = np.empty((N, gp.max_new_tokens + 1), dtype=np.int64)
         lens = np.empty((N,), dtype=np.int32)
         with self._gpu_lock:
-            _chk(self, self._lib.b200t5_generate_stream(
-                self._h, ids.ctypes.data_as(C.c_void_p), None if mask is None else mask.ctypes.data_as(C.c_void_p), N, S,
-                C.byref(gp), int(pool or self.pool_slots), int(admit_min), out.ctypes.data_as(C.c_void_p),
-                lens.ctypes.data_as(C.c_void_p)), self._h)
+            mp = None if mask is None else mask.ctypes.data_as(C.c_void_p)
+            if lp is None:
+                rc = self._lib.b200t5_generate_stream(self._h, ids.ctypes.data_as(C.c_void_p), mp, N, S, C.byref(gp),
+                                                      int(pool or self.pool_slots), int(admit_min),
+                                                      out.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p))
+            else:
+                rc = self._lib.b200t5_generate_stream_ex(self._h, ids.ctypes.data_as(C.c_void_p), mp, N, S, C.byref(gp),
+                                                         lp.ref(), int(pool or self.pool_slots), int(admit_min),
+                                                         out.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p))
+            _chk(self, rc, self._h)
         self.last_lengths = torch.from_numpy(lens)
         return out[:, : int(lens.max()) + 1], lens
 

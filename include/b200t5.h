@@ -85,6 +85,30 @@ typedef struct b200t5_gen_params {
   int32_t poll_interval;           /* steps between device->host "all rows finished" checks; <=0: 8 */
 } b200t5_gen_params;
 
+/* Greedy-mode logits processors (transformers GenerationConfig options of the same names; generation/logits_process.py),
+ * applied in transformers' order to the lm_head logits rounded to the build's 2-byte type and widened to fp32:
+ * encoder repetition penalty, repetition penalty, no-repeat n-grams, encoder no-repeat n-grams, bad words, the EOS mask
+ * of min_new_tokens, suppressed tokens, begin-suppressed tokens; then the arg-max. Passing NULL instead of this struct
+ * is the plain greedy path; so is a struct whose every field is a no-op. Host pointers, read during the call only. */
+typedef struct b200t5_logits_params {
+  double repetition_penalty;          /* 1.0 = off; > 0. Over the decoder ids so far, the start token included */
+  double encoder_repetition_penalty;  /* 1.0 = off; > 0. Over the prompt's ids, padding positions included */
+  int32_t no_repeat_ngram_size;          /* 0 = off; over the decoder ids, the start token included */
+  int32_t encoder_no_repeat_ngram_size;  /* 0 = off; n-grams of the prompt's ids, padding included */
+  const int32_t* suppress_tokens;        /* masked at every step */
+  int32_t n_suppress_tokens;
+  const int32_t* begin_suppress_tokens;  /* masked at the first generated position only */
+  int32_t n_begin_suppress_tokens;
+  const int32_t* eos_token_ids;  /* 1..16 ids: any of them finishes a row and all are masked while fewer than
+                                  * min_new_tokens were generated; n_eos_token_ids == 0: gen_params' eos_token_id */
+  int32_t n_eos_token_ids;
+  const int32_t* bad_words_ids;      /* the sequences, concatenated */
+  const int32_t* bad_words_offsets;  /* [n_bad_words + 1]: sequence i = bad_words_ids[offsets[i] .. offsets[i+1]) */
+  int32_t n_bad_words;               /* a one-token sequence is banned at every step, except one equal to an EOS id,
+                                      * which is dropped; a longer one bans its last token when the rest of it ends
+                                      * the decoder ids */
+} b200t5_logits_params;
+
 typedef struct b200t5_stats {
   float encoder_ms;       /* encoder + cross-KV projection of the last generate call (CUDA events) */
   float decode_ms;        /* decode loop of the last generate call (CUDA events) */
@@ -133,6 +157,19 @@ int b200t5_generate_host(b200t5_handle h, const int64_t* input_ids, const int64_
 int b200t5_generate_stream(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int64_t N, int S,
                            const b200t5_gen_params* params, int pool, int admit_min, int64_t* out_ids,
                            int32_t* out_len);
+/* The three entry points above with logits processors (`logits` may be NULL: the call is exactly the one above).
+ * Every processor state lives in device memory, so the step graph captured for a set of active processors is replayed
+ * whatever their values. Ids outside [0, vocab_size), an empty bad-word sequence, a penalty <= 0 or a negative n-gram
+ * size fail with B200T5_EINVAL. */
+int b200t5_generate_ex(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                       const b200t5_gen_params* params, const b200t5_logits_params* logits, int64_t* out_ids,
+                       int32_t* out_len, void* stream);
+int b200t5_generate_host_ex(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                            const b200t5_gen_params* params, const b200t5_logits_params* logits, int64_t* out_ids,
+                            int32_t* out_len);
+int b200t5_generate_stream_ex(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int64_t N, int S,
+                              const b200t5_gen_params* params, const b200t5_logits_params* logits, int pool,
+                              int admit_min, int64_t* out_ids, int32_t* out_len);
 int b200t5_get_stats(b200t5_handle h, b200t5_stats* out);
 
 /* ---- measurement hooks (bench.py) --------------------------------------------------- */
@@ -167,6 +204,14 @@ int b200t5_get_xattn_profile(b200t5_handle h, double* avg_us_per_launch, int64_t
  * (transformers generation/utils.py:2762,2793; logits_process.py:225-233). Test hook. */
 int b200t5_test_lm_argmax(int device, const void* x, const void* W, int M, int V, int K, int step, int eos, int min_new,
                           int64_t* tokens, void* stream);
+/* One decode step of lm_head + logits processors + arg-max as the step graph runs them (csrc/gemm.cuh EpiArgmaxProc ->
+ * finalize_step_kernel): x [M,K] and W [V,K] as in b200t5_test_lm_argmax; hist int64 [M, step+1] (device) the decoder
+ * ids so far (start token first), enc_ids int64 [M,S] (device) the prompts; eos is the EOS id when `logits` lists none.
+ * tokens: int64 [M] (device); vals: fp32 [M,V] (device, may be NULL) the processed logits the arg-max ran on. Test hook;
+ * both builds. */
+int b200t5_test_lm_process(int device, const void* x, const void* W, int M, int V, int K, int step, int eos, int min_new,
+                           const b200t5_logits_params* logits, const int64_t* hist, const int64_t* enc_ids, int S,
+                           int64_t* tokens, float* vals, void* stream);
 
 /* ---- parity hooks (used by tests/ only) --------------------------------------------- */
 /* Encoder last hidden state after the final RMSNorm, bf16 [B,S,d_model] (device). */

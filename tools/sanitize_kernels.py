@@ -159,6 +159,34 @@ def main():
             ids, mask = synthetic_token_batch(20, 24, spec.vocab_size, seed=3, lengths="uniform")
             model.generate_stream(ids, mask, pool=8, max_new_tokens=4)
             del model
+    if section("logits_process"):
+        # EpiArgmaxProc + finalize_step_kernel<true> + proc_reset_kernel through the hook (a V that is no multiple of
+        # 32 or 128, bans at the vocabulary's end), then one small generate and one slot-pool run with every processor
+        M, V, K, S, step = 20, 1000, 64, 30, 4
+        xa, Wv = rnd(M, K), rnd(V, K)
+        hist = torch.randint(0, V, (M, step + 1), device="cuda")
+        enc = torch.randint(0, V, (M, S), device="cuda")
+        keep = [torch.tensor([V - 1, 3], dtype=torch.int32), torch.tensor([2, V - 1, 998, 999], dtype=torch.int32),
+                torch.tensor([0, 1, 4], dtype=torch.int32)]
+        lp = _lib.LogitsParams(repetition_penalty=1.3, encoder_repetition_penalty=0.8, no_repeat_ngram_size=2,
+                               encoder_no_repeat_ngram_size=2, suppress_tokens=keep[0].data_ptr(), n_suppress_tokens=2,
+                               bad_words_ids=keep[1].data_ptr(), bad_words_offsets=keep[2].data_ptr(), n_bad_words=2)
+        toks = torch.zeros(M, device="cuda", dtype=torch.long)
+        vals = torch.zeros(M, V, device="cuda")
+        _lib.check(lib.b200t5_test_lm_process(DEV, P(xa), P(Wv), M, V, K, step, 1, 0, C.byref(lp), P(hist), P(enc), S,
+                                              P(toks), P(vals), None))
+        torch.cuda.synchronize()
+        assert torch.equal(toks, vals.argmax(-1)) and (vals[:, V - 1] == -float("inf")).all()
+        spec = SPECS["tiny"]
+        model = B200T5ForConditionalGeneration.from_pretrained(checkpoint_dir("tiny", 1), torch_dtype=torch.bfloat16)
+        ids, mask = synthetic_token_batch(6, 24, spec.vocab_size, seed=2, lengths="uniform")
+        kw = dict(max_new_tokens=6, repetition_penalty=1.3, encoder_repetition_penalty=0.9, no_repeat_ngram_size=2,
+                  encoder_no_repeat_ngram_size=3, bad_words_ids=[[5, 9], [7]], suppress_tokens=[3],
+                  begin_suppress_tokens=[2], eos_token_id=[1, 6])
+        model.generate(input_ids=torch.from_numpy(ids), attention_mask=torch.from_numpy(mask), **kw)
+        ids, mask = synthetic_token_batch(20, 24, spec.vocab_size, seed=3, lengths="uniform")
+        model.generate_stream(ids, mask, pool=8, **kw)
+        del model
     print("sanitize_kernels: all sections ran", flush=True)
 
 
