@@ -71,6 +71,15 @@ class LogitsParams(C.Structure):
     ]
 
 
+class ScoreIO(C.Structure):
+    _fields_ = [
+        ("token_logprobs", C.c_void_p),
+        ("token_logits", C.c_void_p),
+        ("forced_ids", C.c_void_p),
+        ("forced_len", C.c_int32),
+    ]
+
+
 class Stats(C.Structure):
     _fields_ = [
         ("encoder_ms", C.c_float),
@@ -101,6 +110,12 @@ SIGNATURES = {
     "b200t5_generate_host_ex": (_i, [_vp, _i64p, _i64p, _i, _i, C.POINTER(GenParams), C.POINTER(LogitsParams), _i64p, _i32p]),
     "b200t5_generate_stream_ex": (_i, [_vp, _i64p, _i64p, C.c_int64, _i, C.POINTER(GenParams), C.POINTER(LogitsParams), _i, _i,
                                        _i64p, _i32p]),
+    "b200t5_generate_scored": (_i, [_vp, _i64p, _i64p, _i, _i, C.POINTER(GenParams), C.POINTER(LogitsParams), _i64p, _i32p,
+                                    C.POINTER(ScoreIO), _vp]),
+    "b200t5_generate_host_scored": (_i, [_vp, _i64p, _i64p, _i, _i, C.POINTER(GenParams), C.POINTER(LogitsParams), _i64p, _i32p,
+                                         C.POINTER(ScoreIO)]),
+    "b200t5_generate_stream_scored": (_i, [_vp, _i64p, _i64p, C.c_int64, _i, C.POINTER(GenParams), C.POINTER(LogitsParams), _i, _i,
+                                           _i64p, _i32p, C.POINTER(ScoreIO)]),
     "b200t5_get_stats": (_i, [_vp, C.POINTER(Stats)]),
     "b200t5_bench_cross_attn": (_i, [_vp, _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_double), _vp]),
     "b200t5_set_option": (_i, [_vp, C.c_char_p, _i]),
@@ -108,6 +123,8 @@ SIGNATURES = {
     "b200t5_test_lm_argmax": (_i, [_i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "b200t5_test_lm_process": (_i, [_i, _vp, _vp, _i, _i, _i, _i, _i, _i, C.POINTER(LogitsParams), _i64p, _i64p, _i, _i64p,
                                     _vp, _vp]),
+    "b200t5_test_lm_score": (_i, [_i, _vp, _vp, _i, _i, _i, _i, _i, _i, C.POINTER(LogitsParams), _i64p, _i64p, _i, _i64p, _i64p,
+                                  _vp, _vp, _vp, _vp]),
     "b200t5_encode": (_i, [_vp, _i64p, _i64p, _i, _i, _vp, _vp]),
     "b200t5_decode_logits": (_i, [_vp, _i64p, _i64p, _i, _i, _i64p, _i, _vp, _vp]),
     "b200t5_relative_bucket": (_i, [_i, _i, _i, _i]),

@@ -179,7 +179,7 @@ struct DevBuf {
 };
 
 // Which epilogue/tile a GEMM uses.
-enum GemmKind { G_STORE256, G_RES256, G_GEGLU256, G_CROSSKV256, G_QKVDEC64, G_STORE32, G_RES32, G_GEGLU64, G_ARGMAX128, G_LOGITS128, G_ARGMAXPROC128 };
+enum GemmKind { G_STORE256, G_RES256, G_GEGLU256, G_CROSSKV256, G_QKVDEC64, G_STORE32, G_RES32, G_GEGLU64, G_ARGMAX128, G_LOGITS128, G_ARGMAXPROC128, G_SCORE128, G_SCOREPROC128 };
 
 struct GemmOp {
   CUtensorMap tmA, tmB;
@@ -212,6 +212,15 @@ struct ProcHost {
 
 // Device state of the processors for `rows` rows (logits_process.cuh: ProcDev). The step graph bakes these
 // addresses: a reallocation means a new graph.
+// Host form of a call's scoring request (b200t5_score_io after validation). `forced`: the labels padded with -100 to
+// [rows, max_new_tokens], as the step kernels read them. lp / lg: device destinations of the two result arrays.
+struct ScoreHost {
+  bool on = false;
+  std::vector<long long> forced;
+  float* lp = nullptr;
+  float* lg = nullptr;
+};
+
 struct ProcBufs {
   DevBuf cfg, seen, enc, banned, stat, list, cnt, enc_ids, bad_ids, bad_off;
   int rows = 0, S = 0, W = 0, ban_cap = 0;
@@ -302,6 +311,15 @@ struct Plan {
   ProcBufs proc;
   bool proc_on = false;
   int g_proc = -1;
+  // token log-probabilities (allocated by the first call that asks for them); score_on: 0 = this call's step runs the
+  // plain arg-max kernels, 1 = EpiScore + finalize_step_score_kernel, 2 = those with teacher forcing. Part of the
+  // step graph's key, like proc_on.
+  DevBuf psum, fval, ftok;              // [B][n_tiles], [B], [B]
+  DevBuf score_lp, score_lg, forced;    // [B][Tmax] results and labels of a static batch
+  DevBuf stream_lp, stream_lg, stream_forced;  // [stream_cap][Tmax]: the slot pool's
+  size_t score_stream_cap = 0;
+  int score_on = 0;
+  int g_score = -1;
   size_t stream_cap = 0;   // rows stream_out / stream_len hold (the step graph bakes their addresses)
   bool stream_mode = false;
   int g_stream = -1;
@@ -489,6 +507,10 @@ static cudaError_t run_gemm(b200t5_ctx* h, const GemmOp& g, const void* ep, cuda
       return launch_gemm<128, EpiStoreF32>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiStoreF32::Params*>(ep), h->num_sms, s, pdl);
     case G_ARGMAXPROC128:
       return launch_gemm<128, EpiArgmaxProc>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiArgmaxProc::Params*>(ep), h->num_sms, s, pdl);
+    case G_SCORE128:
+      return launch_gemm<128, EpiScore<false>>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiScore<false>::Params*>(ep), h->num_sms, s, pdl);
+    case G_SCOREPROC128:
+      return launch_gemm<128, EpiScore<true>>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiScore<true>::Params*>(ep), h->num_sms, s, pdl);
   }
   return cudaErrorInvalidValue;
 }
@@ -548,6 +570,7 @@ static cudaError_t init_kernel_attrs() {
   if ((e = prepare_gemm<BN, EPI>()) != cudaSuccess) return e;
   PREP(256, EpiStore) PREP(256, EpiResidual) PREP(256, EpiGeglu) PREP(256, EpiCrossKV) PREP(64, EpiQkvDecode)
   PREP(32, EpiStore) PREP(32, EpiResidual) PREP(64, EpiGeglu) PREP(128, EpiArgmax) PREP(128, EpiStoreF32) PREP(128, EpiArgmaxProc)
+  PREP(128, EpiScore<false>) PREP(128, EpiScore<true>)
   PREP(64, EpiStore) PREP(128, EpiStore)
 #undef PREP
   if ((e = prepare_gemm_2cta<EpiStore>()) != cudaSuccess) return e;
@@ -1369,7 +1392,15 @@ static int chain_head(b200t5_ctx* h, cudaStream_t s, const ChainView& v, float* 
     const bool sm = p.stream_mode;
     EpiArgmax::Params ep{pval, pidx, p.n_vtiles, sm ? p.pos.as<int>() + v.b0 : &st->step, static_cast<int>(eos), min_new, sm ? 1 : 0};
     const ProcDev pd = p.proc_on ? p.proc.dev(v.b0) : ProcDev();
-    if (p.proc_on) {
+    const int* ftok = p.score_on == 2 ? p.ftok.as<int>() + v.b0 : nullptr;
+    float* psum = p.psum.as<float>() + static_cast<size_t>(v.b0) * p.n_vtiles;
+    if (p.score_on && p.proc_on) {
+      EpiScore<true>::Params eps{{ep, pd, nullptr, 0}, psum, p.fval.as<float>() + v.b0, ftok, nullptr, 0};
+      CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, G_SCOREPROC128, 1), &eps, s, pdl));
+    } else if (p.score_on) {
+      EpiScore<false>::Params eps{ep, psum, p.fval.as<float>() + v.b0, ftok, nullptr, 0};
+      CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, G_SCORE128, 1), &eps, s, pdl));
+    } else if (p.proc_on) {
       EpiArgmaxProc::Params epp{ep, pd, nullptr, 0};
       CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, G_ARGMAXPROC128, 1), &epp, s, pdl));
     } else {
@@ -1378,11 +1409,28 @@ static int chain_head(b200t5_ctx* h, cudaStream_t s, const ChainView& v, float* 
     // static batch: rows b0.. of the plan's [B, T+1] result; slot pool: row out_row[slot] of the [N, T+1] result
     long long* oid = sm ? p.stream_out.as<long long>() : p.out_ids.as<long long>() + static_cast<size_t>(v.b0) * (T + 1);
     int* olen = sm ? p.stream_len.as<int>() : p.out_len.as<int>() + v.b0;
-    CU_OK(h, launch_kernel(p.proc_on ? finalize_step_kernel<true> : finalize_step_kernel<false>, dim3(v.nb), dim3(128), 0, s,
-                           pdl, pval, pidx, p.n_vtiles, st, p.unfinished.as<int>() + v.b0, oid, olen, T + 1, eos, pad,
-                           h->shared.as<act_t>(), v.dx, d, p.live_extent.as<int>() + v.b0,
-                           sm ? p.pos.as<int>() + v.b0 : static_cast<int*>(nullptr),
-                           sm ? p.out_row.as<int>() + v.b0 : static_cast<const int*>(nullptr), T, pd));
+    if (p.score_on) {
+      // the result rows are indexed like the ids: b0.. of [B, T] (static batch), out_row[slot] of [N, T] (slot pool)
+      ScoreDev sd;
+      sd.psum = psum;
+      sd.fval = p.fval.as<float>() + v.b0;
+      sd.ftok = p.ftok.as<int>() + v.b0;
+      const size_t r0 = sm ? 0 : static_cast<size_t>(v.b0) * T;
+      if (p.score_on == 2) sd.forced = (sm ? p.stream_forced : p.forced).as<long long>() + r0;
+      sd.logprob = (sm ? p.stream_lp : p.score_lp).as<float>() + r0;
+      sd.logit = (sm ? p.stream_lg : p.score_lg).as<float>() + r0;
+      CU_OK(h, launch_kernel(p.proc_on ? finalize_step_score_kernel<true> : finalize_step_score_kernel<false>, dim3(v.nb), dim3(128),
+                             0, s, pdl, pval, pidx, p.n_vtiles, st, p.unfinished.as<int>() + v.b0, oid, olen, T + 1, eos, pad,
+                             h->shared.as<act_t>(), v.dx, d, p.live_extent.as<int>() + v.b0,
+                             sm ? p.pos.as<int>() + v.b0 : static_cast<int*>(nullptr),
+                             sm ? p.out_row.as<int>() + v.b0 : static_cast<const int*>(nullptr), T, pd, sd));
+    } else {
+      CU_OK(h, launch_kernel(p.proc_on ? finalize_step_kernel<true> : finalize_step_kernel<false>, dim3(v.nb), dim3(128), 0, s,
+                             pdl, pval, pidx, p.n_vtiles, st, p.unfinished.as<int>() + v.b0, oid, olen, T + 1, eos, pad,
+                             h->shared.as<act_t>(), v.dx, d, p.live_extent.as<int>() + v.b0,
+                             sm ? p.pos.as<int>() + v.b0 : static_cast<int*>(nullptr),
+                             sm ? p.out_row.as<int>() + v.b0 : static_cast<const int*>(nullptr), T, pd));
+    }
     h->launches++;
   }
   return B200T5_OK;
@@ -1462,7 +1510,8 @@ static int run_decode_step(b200t5_ctx* h, cudaStream_t s, bool fork, float* logi
 }
 
 // Graph of one decode step; eos/pad/min_new are baked in, so the graph is rebuilt when they change. Whether logits
-// processors run is baked in too (their values are read from device memory at replay).
+// processors run and whether the step scores its token (and is teacher-forced) are baked in too; their values are read
+// from device memory at replay.
 // The cross-attention kernel is baked in as well: `fill` = valid prompt tokens / (B * S) of the batch at hand.
 constexpr double kXattnStreamFill = 0.9;
 static int pick_xattn(const b200t5_ctx* h, double fill) {
@@ -1473,7 +1522,7 @@ static int ensure_graph(b200t5_ctx* h, long long eos, long long pad, int min_new
   const int want = pick_xattn(h, fill);
   p.xattn_stream = want != 0;
   if (p.gexec && p.g_eos == eos && p.g_pad == pad && p.g_min_new == min_new && p.g_stream == (p.stream_mode ? 1 : 0) && p.g_xattn == want &&
-      p.g_proc == (p.proc_on ? 1 : 0))
+      p.g_proc == (p.proc_on ? 1 : 0) && p.g_score == p.score_on)
     return B200T5_OK;
   if (p.gexec) cudaGraphExecDestroy(p.gexec);
   if (p.graph) cudaGraphDestroy(p.graph);
@@ -1501,6 +1550,7 @@ static int ensure_graph(b200t5_ctx* h, long long eos, long long pad, int min_new
   p.g_stream = p.stream_mode ? 1 : 0;
   p.g_xattn = want;
   p.g_proc = p.proc_on ? 1 : 0;
+  p.g_score = p.score_on;
   return B200T5_OK;
 }
 
@@ -1611,6 +1661,66 @@ static int setup_proc(b200t5_ctx* h, const ProcHost& ph, cudaStream_t s) {
   return B200T5_OK;
 }
 
+// b200t5_score_io -> ScoreHost for a call of `rows` rows and T = max_new_tokens. `host`: the struct's pointers are
+// host pointers (else device pointers: the labels are read back to be checked). The destinations are set by the
+// caller, which knows where the results must go.
+static int parse_score(b200t5_ctx* h, const b200t5_score_io* sc, long long rows, int T, bool host, bool proc_on, ScoreHost* sh) {
+  *sh = ScoreHost();
+  if (!sc) return B200T5_OK;
+  if (!sc->token_logprobs) return fail(h, B200T5_EINVAL, "score: token_logprobs is NULL");
+  sh->on = true;
+  if (!sc->forced_ids) return B200T5_OK;
+  const int L = sc->forced_len;
+  if (L < 1 || L > T) return fail(h, B200T5_EINVAL, "score: forced_len=%d outside [1, max_new_tokens=%d]", L, T);
+  if (proc_on) return fail(h, B200T5_EINVAL, "score: forced_ids cannot be combined with logits processors");
+  std::vector<long long> f(static_cast<size_t>(rows) * L);
+  if (host) memcpy(f.data(), sc->forced_ids, f.size() * 8);
+  else CU_OK(h, cudaMemcpy(f.data(), sc->forced_ids, f.size() * 8, cudaMemcpyDeviceToHost));
+  sh->forced.assign(static_cast<size_t>(rows) * T, -100);
+  for (long long r = 0; r < rows; ++r) {
+    bool ended = false;
+    for (int t = 0; t < L; ++t) {
+      const long long v = f[static_cast<size_t>(r) * L + t];
+      if (v == -100) {
+        if (t == 0) return fail(h, B200T5_EINVAL, "score: row %lld of forced_ids has no label", r);
+        ended = true;
+        continue;
+      }
+      if (v < 0 || v >= h->c.V) return fail(h, B200T5_EINVAL, "score: forced id %lld outside [0, %d)", v, h->c.V);
+      if (ended) return fail(h, B200T5_EINVAL, "score: row %lld of forced_ids has a label after -100", r);
+      sh->forced[static_cast<size_t>(r) * T + t] = v;
+    }
+  }
+  return B200T5_OK;
+}
+
+// Make the plan's scoring buffers fit this call (`rows` result rows: the batch, or the slot pool's capacity) and queue
+// the labels on `s`. A new allocation drops the step graph, which bakes the addresses.
+static int setup_score(b200t5_ctx* h, const ScoreHost& sh, cudaStream_t s) {
+  Plan& p = *h->plan;
+  p.score_on = sh.on ? (sh.forced.empty() ? 1 : 2) : 0;
+  if (!sh.on) return B200T5_OK;
+  const bool sm = p.stream_mode;
+  const size_t rows = sm ? p.stream_cap : static_cast<size_t>(p.B), n = rows * p.Tmax;
+  if (!p.psum.p || (sm ? p.score_stream_cap != rows : !p.score_lp.p)) {
+    CU_OK(h, cudaStreamSynchronize(s));
+    if (!p.psum.p) {
+      CU_OK(h, p.psum.alloc(static_cast<size_t>(p.B) * p.n_vtiles * 4));
+      CU_OK(h, p.fval.alloc(static_cast<size_t>(p.B) * 4));
+      CU_OK(h, p.ftok.alloc(static_cast<size_t>(p.B) * 4));
+      CU_OK(h, cudaMemset(p.fval.p, 0, p.fval.bytes));
+    }
+    CU_OK(h, (sm ? p.stream_lp : p.score_lp).alloc(n * 4));
+    CU_OK(h, (sm ? p.stream_lg : p.score_lg).alloc(n * 4));
+    CU_OK(h, (sm ? p.stream_forced : p.forced).alloc(n * 8));
+    if (sm) p.score_stream_cap = rows;
+    p.g_score = -1;
+  }
+  if (p.score_on == 2)
+    CU_OK(h, cudaMemcpyAsync((sm ? p.stream_forced : p.forced).p, sh.forced.data(), sh.forced.size() * 8, cudaMemcpyHostToDevice, s));
+  return B200T5_OK;
+}
+
 static void fill_stats_model(b200t5_ctx* h, int steps) {
   const Cfg& c = h->c;
   const Plan& p = *h->plan;
@@ -1636,7 +1746,8 @@ static void fill_stats_model(b200t5_ctx* h, int steps) {
 }
 
 static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* mask, int B, int S,
-                         const b200t5_gen_params* gp, const ProcHost& ph, long long* out_ids, int* out_len, cudaStream_t s) {
+                         const b200t5_gen_params* gp, const ProcHost& ph, const ScoreHost& sh, long long* out_ids, int* out_len,
+                         cudaStream_t s) {
   const Cfg& c = h->c;
   const long long eos = gp->eos_token_id >= 0 ? gp->eos_token_id : c.eos;
   const long long pad = gp->pad_token_id >= 0 ? gp->pad_token_id : c.pad;
@@ -1649,6 +1760,7 @@ static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* m
   Plan& p = *h->plan;
   p.stream_mode = false;
   TRY(setup_proc(h, ph, s));
+  TRY(setup_score(h, sh, s));
   h->launches = 0;
   CU_OK(h, cudaEventRecord(h->ev[0], s));
   TRY(run_encoder(h, ids, mask, s));
@@ -1662,6 +1774,11 @@ static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* m
   h->launches++;
   if (p.proc_on) {
     proc_reset_kernel<<<B, 128, 0, s>>>(p.proc.dev(), nullptr, ids, p.out_ids.as<long long>(), T + 1, nullptr, 1);
+    h->launches++;
+  }
+  if (p.score_on) {
+    score_reset_kernel<<<B, 128, 0, s>>>(p.score_lp.as<float>(), p.score_lg.as<float>(), static_cast<size_t>(B) * T, p.ftok.as<int>(), B,
+                                         nullptr, nullptr, p.score_on == 2 ? p.forced.as<long long>() : nullptr, T);
     h->launches++;
   }
   CU_OK(h, cudaGetLastError());
@@ -1689,6 +1806,10 @@ static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* m
   CU_OK(h, cudaEventRecord(h->ev[2], s));
   CU_OK(h, cudaMemcpyAsync(out_ids, p.out_ids.p, static_cast<size_t>(B) * (T + 1) * 8, cudaMemcpyDeviceToDevice, s));
   CU_OK(h, cudaMemcpyAsync(out_len, p.out_len.p, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToDevice, s));
+  if (p.score_on) {
+    CU_OK(h, cudaMemcpyAsync(sh.lp, p.score_lp.p, static_cast<size_t>(B) * T * 4, cudaMemcpyDeviceToDevice, s));
+    if (sh.lg) CU_OK(h, cudaMemcpyAsync(sh.lg, p.score_lg.p, static_cast<size_t>(B) * T * 4, cudaMemcpyDeviceToDevice, s));
+  }
   h->last_steps = steps;
   h->ev_valid = true;
   return B200T5_OK;
@@ -1698,16 +1819,28 @@ static long long call_eos(const b200t5_ctx* h, const b200t5_gen_params* gp) {
   return gp->eos_token_id >= 0 ? gp->eos_token_id : h->c.eos;
 }
 
-extern "C" int b200t5_generate_ex(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
-                                  const b200t5_gen_params* params, const b200t5_logits_params* logits, int64_t* out_ids,
-                                  int32_t* out_len, void* stream) {
+extern "C" int b200t5_generate_scored(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                                      const b200t5_gen_params* params, const b200t5_logits_params* logits, int64_t* out_ids,
+                                      int32_t* out_len, const b200t5_score_io* score, void* stream) {
   TRY(validate(h, B, S, params));
   if (!params || !input_ids || !out_ids || !out_len) return fail(h, B200T5_EINVAL, "null argument");
   ProcHost ph;
   TRY(parse_logits_params(h, h->c.V, logits, call_eos(h, params), &ph));
   CU_OK(h, cudaSetDevice(h->device));
+  ScoreHost sh;
+  TRY(parse_score(h, score, B, params->max_new_tokens, false, ph.on, &sh));
+  if (sh.on) {
+    sh.lp = score->token_logprobs;
+    sh.lg = score->token_logits;
+  }
   return generate_impl(h, reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(attention_mask),
-                       B, S, params, ph, reinterpret_cast<long long*>(out_ids), out_len, static_cast<cudaStream_t>(stream));
+                       B, S, params, ph, sh, reinterpret_cast<long long*>(out_ids), out_len, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b200t5_generate_ex(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                                  const b200t5_gen_params* params, const b200t5_logits_params* logits, int64_t* out_ids,
+                                  int32_t* out_len, void* stream) {
+  return b200t5_generate_scored(h, input_ids, attention_mask, B, S, params, logits, out_ids, out_len, nullptr, stream);
 }
 
 extern "C" int b200t5_generate(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
@@ -1723,11 +1856,19 @@ extern "C" int b200t5_generate_host(b200t5_handle h, const int64_t* input_ids, c
 extern "C" int b200t5_generate_host_ex(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B,
                                        int S, const b200t5_gen_params* params, const b200t5_logits_params* logits,
                                        int64_t* out_ids, int32_t* out_len) {
+  return b200t5_generate_host_scored(h, input_ids, attention_mask, B, S, params, logits, out_ids, out_len, nullptr);
+}
+
+extern "C" int b200t5_generate_host_scored(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B,
+                                           int S, const b200t5_gen_params* params, const b200t5_logits_params* logits,
+                                           int64_t* out_ids, int32_t* out_len, const b200t5_score_io* score) {
   TRY(validate(h, B, S, params));
   if (!params || !input_ids || !out_ids || !out_len) return fail(h, B200T5_EINVAL, "null argument");
   ProcHost ph;
   TRY(parse_logits_params(h, h->c.V, logits, call_eos(h, params), &ph));
   CU_OK(h, cudaSetDevice(h->device));
+  ScoreHost sh;
+  TRY(parse_score(h, score, B, params->max_new_tokens, true, ph.on, &sh));
   TRY(ensure_plan(h, B, S, params->max_new_tokens));
   Plan& p = *h->plan;
   cudaStream_t s = h->exec_stream;
@@ -1743,8 +1884,22 @@ extern "C" int b200t5_generate_host_ex(b200t5_handle h, const int64_t* input_ids
   const int T = params->max_new_tokens;
   CU_OK(h, tmp_ids.alloc(static_cast<size_t>(B) * (T + 1) * 8));
   CU_OK(h, tmp_len.alloc(static_cast<size_t>(B) * 4));
+  DevBuf tmp_lp, tmp_lg;
+  const size_t score_bytes = static_cast<size_t>(B) * T * 4;
+  if (sh.on) {
+    CU_OK(h, tmp_lp.alloc(score_bytes));
+    sh.lp = tmp_lp.as<float>();
+    if (score->token_logits) {
+      CU_OK(h, tmp_lg.alloc(score_bytes));
+      sh.lg = tmp_lg.as<float>();
+    }
+  }
   TRY(generate_impl(h, p.ids_dev.as<long long>(), attention_mask ? p.mask_dev.as<long long>() : nullptr, B, S, params,
-                    ph, tmp_ids.as<long long>(), tmp_len.as<int>(), s));
+                    ph, sh, tmp_ids.as<long long>(), tmp_len.as<int>(), s));
+  if (sh.on) {
+    CU_OK(h, cudaMemcpyAsync(score->token_logprobs, tmp_lp.p, score_bytes, cudaMemcpyDeviceToHost, s));
+    if (sh.lg) CU_OK(h, cudaMemcpyAsync(score->token_logits, tmp_lg.p, score_bytes, cudaMemcpyDeviceToHost, s));
+  }
   CU_OK(h, cudaMemcpyAsync(p.h_out, tmp_ids.p, static_cast<size_t>(B) * (T + 1) * 8, cudaMemcpyDeviceToHost, s));
   CU_OK(h, cudaMemcpyAsync(p.h_len, tmp_len.p, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToHost, s));
   CU_OK(h, cudaStreamSynchronize(s));
@@ -1771,6 +1926,12 @@ extern "C" int b200t5_generate_stream(b200t5_handle h, const int64_t* input_ids,
 extern "C" int b200t5_generate_stream_ex(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int64_t N,
                                          int S, const b200t5_gen_params* gp, const b200t5_logits_params* logits, int pool,
                                          int admit_min, int64_t* out_ids, int32_t* out_len) {
+  return b200t5_generate_stream_scored(h, input_ids, attention_mask, N, S, gp, logits, pool, admit_min, out_ids, out_len, nullptr);
+}
+
+extern "C" int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int64_t N,
+                                             int S, const b200t5_gen_params* gp, const b200t5_logits_params* logits, int pool,
+                                             int admit_min, int64_t* out_ids, int32_t* out_len, const b200t5_score_io* score) {
   if (!h) return fail(nullptr, B200T5_EINVAL, "null handle");
   if (!gp || !input_ids || !out_ids || !out_len) return fail(h, B200T5_EINVAL, "null argument");
   ProcHost ph;
@@ -1779,6 +1940,8 @@ extern "C" int b200t5_generate_stream_ex(b200t5_handle h, const int64_t* input_i
   if (pool < 1) pool = 256;
   if (pool > N) pool = static_cast<int>(N);
   TRY(validate(h, pool, S, gp));
+  ScoreHost sh;
+  TRY(parse_score(h, score, N, gp->max_new_tokens, true, ph.on, &sh));
   CU_OK(h, cudaSetDevice(h->device));
   const Cfg& c = h->c;
   const long long eos = gp->eos_token_id >= 0 ? gp->eos_token_id : c.eos;
@@ -1805,6 +1968,7 @@ extern "C" int b200t5_generate_stream_ex(b200t5_handle h, const int64_t* input_i
   }
   p.stream_mode = true;
   TRY(setup_proc(h, ph, s));
+  TRY(setup_score(h, sh, s));
   double fill = 1.0;
   if (attention_mask) {  // fill of the first prompts (up to four pools' worth): picks the cross-attention kernel
     const long long rows = N < 4LL * B ? N : 4LL * B;
@@ -1822,6 +1986,11 @@ extern "C" int b200t5_generate_stream_ex(b200t5_handle h, const int64_t* input_i
                                                                   p.stream_len.as<int>(), T + 1, static_cast<int>(N), B, start, pad,
                                                                   h->shared.as<act_t>(), p.dx.as<res_t>(), c.d);
     h->launches++;
+    if (p.score_on) {  // every result position 0, no slot forced until it is admitted
+      score_reset_kernel<<<1024, 128, 0, s>>>(p.stream_lp.as<float>(), p.stream_lg.as<float>(), static_cast<size_t>(N) * T,
+                                              p.ftok.as<int>(), B, nullptr, nullptr, nullptr, T);
+      h->launches++;
+    }
     CU_OK(h, cudaGetLastError());
   }
   CU_OK(h, cudaEventRecord(h->ev[1], s));
@@ -1850,6 +2019,11 @@ extern "C" int b200t5_generate_stream_ex(b200t5_handle h, const int64_t* input_i
     if (p.proc_on) {  // the admitted slots' processor state, from their prompts (still in ids_dev) and start token
       proc_reset_kernel<<<k, 128, 0, s>>>(p.proc.dev(), p.admit.as<int>() + B, p.ids_dev.as<long long>(),
                                           p.stream_out.as<long long>(), T + 1, p.out_row.as<int>(), 1);
+      h->launches++;
+    }
+    if (p.score_on == 2) {  // the admitted slots' first labels
+      score_reset_kernel<<<(k + 127) / 128, 128, 0, s>>>(nullptr, nullptr, 0, p.ftok.as<int>(), k, p.admit.as<int>() + B,
+                                                         p.admit.as<int>() + 2 * B, p.stream_forced.as<long long>(), T);
       h->launches++;
     }
     CU_OK(h, cudaGetLastError());
@@ -1938,6 +2112,11 @@ extern "C" int b200t5_generate_stream_ex(b200t5_handle h, const int64_t* input_i
   CU_OK(h, cudaEventRecord(h->ev[2], s));
   CU_OK(h, cudaMemcpyAsync(out_ids, p.stream_out.p, static_cast<size_t>(N) * (T + 1) * 8, cudaMemcpyDeviceToHost, s));
   CU_OK(h, cudaMemcpyAsync(out_len, p.stream_len.p, static_cast<size_t>(N) * 4, cudaMemcpyDeviceToHost, s));
+  if (p.score_on) {
+    CU_OK(h, cudaMemcpyAsync(score->token_logprobs, p.stream_lp.p, static_cast<size_t>(N) * T * 4, cudaMemcpyDeviceToHost, s));
+    if (score->token_logits)
+      CU_OK(h, cudaMemcpyAsync(score->token_logits, p.stream_lg.p, static_cast<size_t>(N) * T * 4, cudaMemcpyDeviceToHost, s));
+  }
   CU_OK(h, cudaStreamSynchronize(s));
   h->last_steps = steps;
   h->last_decode_bytes = 0;  // not modelled for a pool whose occupancy varies
@@ -2329,6 +2508,90 @@ extern "C" int b200t5_test_lm_process(int device, const void* x, const void* W, 
     e = cudaMemcpy2DAsync(tokens, 8, out.as<long long>() + step + 1, static_cast<size_t>(out_ld) * 8, 8, M, cudaMemcpyDeviceToDevice, s);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s);
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_lm_process: %s", cudaGetErrorString(e));
+  return B200T5_OK;
+}
+
+// lm_head + arg-max + log-sum-exp partials + their merge as chain_head launches them for a scored call (EpiScore ->
+// finalize_step_score_kernel), with the row state of b200t5_test_lm_process when `logits` has an active processor.
+extern "C" int b200t5_test_lm_score(int device, const void* x, const void* W, int M, int V, int K, int step, int eos,
+                                    int min_new, const b200t5_logits_params* logits, const int64_t* hist,
+                                    const int64_t* enc_ids, int S, const int64_t* forced, int64_t* tokens, float* logprob,
+                                    float* logit, float* vals, void* stream) {
+  const int sms = hook_device(device);
+  if (sms < 0) return sms;
+  if (!x || !W || !tokens || !logprob || !logit || M < 1 || V < 2 || K % 8 || step < 0)
+    return fail(nullptr, B200T5_EINVAL, "test_lm_score: bad argument");
+  ProcHost ph;
+  int rc = parse_logits_params(nullptr, V, logits, eos, &ph);
+  if (rc != B200T5_OK) return rc;
+  if (ph.on && (!hist || !enc_ids || S < 1)) return fail(nullptr, B200T5_EINVAL, "test_lm_score: processors need hist and enc_ids");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUtensorMap ta, tb;
+  if (!make_tmap(&ta, x, M, K, 128) || !make_tmap(&tb, W, V, K, 128)) return fail(nullptr, B200T5_ECUDA, "%s", g_err);
+  // result arrays [M, T] with T = step + 1 columns (+ 1 when forced: a further label keeps the row going)
+  const int n_tiles = (V + 127) / 128, T = step + 1, out_ld = T + 1, Wd = (V + 31) / 32;
+  DevBuf pval, pidx, psum, fval, ftok, fids, lp, lg, st, unf, out, len, xn, ext;
+  ProcBufs pb;
+  const size_t mt = static_cast<size_t>(M) * n_tiles * 4;
+  if (pval.alloc(mt) != cudaSuccess || pidx.alloc(mt) != cudaSuccess || psum.alloc(mt) != cudaSuccess ||
+      fval.alloc(static_cast<size_t>(M) * 4) != cudaSuccess || ftok.alloc(static_cast<size_t>(M) * 4) != cudaSuccess ||
+      fids.alloc(static_cast<size_t>(M) * T * 8) != cudaSuccess || lp.alloc(static_cast<size_t>(M) * T * 4) != cudaSuccess ||
+      lg.alloc(static_cast<size_t>(M) * T * 4) != cudaSuccess || st.alloc(sizeof(DecodeState)) != cudaSuccess ||
+      unf.alloc(static_cast<size_t>(M) * 4) != cudaSuccess || out.alloc(static_cast<size_t>(M) * out_ld * 8) != cudaSuccess ||
+      len.alloc(static_cast<size_t>(M) * 4) != cudaSuccess || xn.alloc(static_cast<size_t>(M) * K * sizeof(res_t)) != cudaSuccess ||
+      ext.alloc(static_cast<size_t>(M) * 4) != cudaSuccess ||
+      (ph.on && pb.alloc(M, S, Wd, std::min(Wd * 32, step + 2 + S + ph.cfg.n_bad), ph.bad_ids.size(), ph.bad_off.size()) != cudaSuccess))
+    return fail(nullptr, B200T5_ENOMEM, "test_lm_score: allocation failed");
+  b200t5_ctx dummy;
+  dummy.num_sms = sms;
+  decode_init_kernel<<<M, 128, 0, s>>>(st.as<DecodeState>(), unf.as<int>(), out.as<long long>(), len.as<int>(), out_ld, M, 0, 0,
+                                       static_cast<const act_t*>(W), xn.as<res_t>(), K);
+  set_state_kernel<<<1, 1, 0, s>>>(st.as<DecodeState>(), step);
+  cudaError_t e = cudaSuccess;
+  if (ph.on) {
+    e = cudaMemcpy2DAsync(out.p, static_cast<size_t>(out_ld) * 8, hist, static_cast<size_t>(step + 1) * 8,
+                          static_cast<size_t>(step + 1) * 8, M, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = pb.upload(ph, s);
+    if (e == cudaSuccess)
+      proc_reset_kernel<<<M, 128, 0, s>>>(pb.dev(), nullptr, reinterpret_cast<const long long*>(enc_ids), out.as<long long>(),
+                                          out_ld, nullptr, step + 1);
+  }
+  // the row's label of this step sits in column `step` of its [M, T] label rows; score_reset_kernel reads column 0
+  if (e == cudaSuccess && forced)
+    e = cudaMemcpy2DAsync(fids.as<long long>() + step, static_cast<size_t>(T) * 8, forced, 8, 8, M, cudaMemcpyDeviceToDevice, s);
+  if (e == cudaSuccess) {
+    score_reset_kernel<<<M, 128, 0, s>>>(lp.as<float>(), lg.as<float>(), static_cast<size_t>(M) * T, ftok.as<int>(), M, nullptr, nullptr,
+                                         forced ? fids.as<long long>() + step : nullptr, T);
+    e = cudaGetLastError();
+  }
+  const ProcDev pd = ph.on ? pb.dev() : ProcDev();
+  const EpiArgmax::Params ea{pval.as<float>(), pidx.as<int>(), n_tiles, &st.as<DecodeState>()->step, eos, min_new, 0};
+  const int* ft = forced ? ftok.as<int>() : nullptr;
+  if (e == cudaSuccess && ph.on) {
+    EpiScore<true>::Params ep{{ea, pd, nullptr, 0}, psum.as<float>(), fval.as<float>(), ft, vals, V};
+    e = run_gemm(&dummy, mk(ta, tb, M, V, K, G_SCOREPROC128, 1), &ep, s, false);
+  } else if (e == cudaSuccess) {
+    EpiScore<false>::Params ep{ea, psum.as<float>(), fval.as<float>(), ft, vals, V};
+    e = run_gemm(&dummy, mk(ta, tb, M, V, K, G_SCORE128, 1), &ep, s, false);
+  }
+  ScoreDev sd;
+  sd.psum = psum.as<float>();
+  sd.fval = fval.as<float>();
+  sd.ftok = ftok.as<int>();
+  sd.forced = forced ? fids.as<long long>() : nullptr;
+  sd.logprob = lp.as<float>();
+  sd.logit = lg.as<float>();
+  if (e == cudaSuccess)
+    e = launch_kernel(ph.on ? finalize_step_score_kernel<true> : finalize_step_score_kernel<false>, dim3(M), dim3(128), 0, s, false,
+                      pval.as<float>(), pidx.as<int>(), n_tiles, st.as<DecodeState>(), unf.as<int>(), out.as<long long>(), len.as<int>(),
+                      out_ld, static_cast<long long>(-1), static_cast<long long>(0), static_cast<const act_t*>(W), xn.as<res_t>(), K,
+                      ext.as<int>(), static_cast<int*>(nullptr), static_cast<const int*>(nullptr), T, pd, sd);
+  if (e == cudaSuccess)
+    e = cudaMemcpy2DAsync(tokens, 8, out.as<long long>() + step + 1, static_cast<size_t>(out_ld) * 8, 8, M, cudaMemcpyDeviceToDevice, s);
+  if (e == cudaSuccess) e = cudaMemcpy2DAsync(logprob, 4, lp.as<float>() + step, static_cast<size_t>(T) * 4, 4, M, cudaMemcpyDeviceToDevice, s);
+  if (e == cudaSuccess) e = cudaMemcpy2DAsync(logit, 4, lg.as<float>() + step, static_cast<size_t>(T) * 4, 4, M, cudaMemcpyDeviceToDevice, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_lm_score: %s", cudaGetErrorString(e));
   return B200T5_OK;
 }
 

@@ -291,13 +291,34 @@ __global__ void admit_slots_kernel(const int* __restrict__ slots, const int* __r
 // (unfinished == 0) write nothing and stay at position 0.
 // kProc (logits processors active): a row finishes on any of the call's EOS ids, and a row that goes on marks its
 // token as seen and computes the bans of its next step (logits_process.cuh).
-template <bool kProc>
-__global__ void finalize_step_kernel(const float* __restrict__ pval, const int* __restrict__ pidx, int n_tiles,
-                                     DecodeState* st, int* __restrict__ unfinished,
-                                     long long* __restrict__ out_ids, int* __restrict__ out_len, int out_ld,
-                                     long long eos_tok, long long pad_tok, const act_t* __restrict__ E,
-                                     res_t* __restrict__ x, int d, int* __restrict__ live_extent,
-                                     int* __restrict__ pos, const int* __restrict__ out_row, int max_new, ProcDev pd) {
+//
+// kScore (token log-probabilities, finalize_step_score_kernel): the epilogue also left psum[b][i] = sum of
+// expf(v - pval[b][i]) over tile i (gemm.cuh: EpiScore). They are merged in an order that depends on nothing but
+// n_tiles and the 128-thread CTA - thread k adds tiles k, k + 128, ... in ascending order, the warp's lanes are
+// folded by the xor tree, thread 0 adds the four warps in order:
+//   M = max_i m_i,  S = sum_i s_i * expf(m_i - M),  lse = M + logf(S)
+// so a row's numbers are bit-identical whichever row-chain, slot or batch it sits in. For an unfinished row at step t
+//   logit[row][t] = v_tok,  logprob[row][t] = v_tok - lse          (fp32 [rows, max_new]; untouched positions stay 0)
+// where v_tok = M for the arg-max token. Teacher forcing (sd.forced != nullptr, int64 [rows, max_new], -100 after a
+// row's last label): tok = forced[row][t] instead of the arg-max, v_tok = fval[b] (written by the tile holding that
+// column), and the row finishes after its last label, not on EOS; ftok[b] becomes the next step's forced column.
+struct ScoreDev {
+  const float* psum = nullptr;   // [B][n_tiles]
+  const float* fval = nullptr;   // [B]
+  int* ftok = nullptr;           // [B]
+  const long long* forced = nullptr;  // [rows][max_new]
+  float* logprob = nullptr;      // [rows][max_new]
+  float* logit = nullptr;        // [rows][max_new]
+};
+
+template <bool kProc, bool kScore>
+DEVINL void finalize_step_body(const float* __restrict__ pval, const int* __restrict__ pidx, int n_tiles,
+                               DecodeState* st, int* __restrict__ unfinished,
+                               long long* __restrict__ out_ids, int* __restrict__ out_len, int out_ld,
+                               long long eos_tok, long long pad_tok, const act_t* __restrict__ E,
+                               res_t* __restrict__ x, int d, int* __restrict__ live_extent,
+                               int* __restrict__ pos, const int* __restrict__ out_row, int max_new, const ProcDev& pd,
+                               const ScoreDev& sd) {
   pdl_launch_dependents();
   pdl_wait();
   const int b = blockIdx.x;
@@ -331,6 +352,20 @@ __global__ void finalize_step_kernel(const float* __restrict__ pval, const int* 
     s_i[warp] = bidx;
   }
   __syncthreads();
+  float ssum = 0.f;
+  if constexpr (kScore) {
+    __shared__ float s_s[32];
+    float mx = s_v[0];
+    for (int w = 1; w < nwarp; ++w) mx = fmaxf(mx, s_v[w]);
+    for (int i = threadIdx.x; i < n_tiles; i += blockDim.x)
+      ssum += sd.psum[static_cast<size_t>(b) * n_tiles + i] * expf(pval[static_cast<size_t>(b) * n_tiles + i] - mx);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) ssum += __shfl_xor_sync(0xffffffffu, ssum, o);
+    if (lane_id() == 0) s_s[warp] = ssum;
+    __syncthreads();
+    if (threadIdx.x == 0)
+      for (int w = 1; w < nwarp; ++w) ssum += s_s[w];
+  }
   if (threadIdx.x == 0) {
     for (int w = 1; w < nwarp; ++w) {
       if (s_v[w] > best || (s_v[w] == best && s_i[w] < bidx)) {
@@ -339,13 +374,31 @@ __global__ void finalize_step_kernel(const float* __restrict__ pval, const int* 
       }
     }
     const int unf = unfinished[b];
-    const long long tok = unf ? static_cast<long long>(bidx) : pad_tok;
     const int row = out_row != nullptr ? out_row[b] : b;
+    long long tok = unf ? static_cast<long long>(bidx) : pad_tok;
+    bool forced = false;
+    if constexpr (kScore) {
+      forced = sd.forced != nullptr;
+      if (unf) {
+        float v_tok = best;
+        if (forced) {
+          tok = sd.forced[static_cast<size_t>(row) * max_new + t];
+          v_tok = sd.fval[b];
+        }
+        sd.logprob[static_cast<size_t>(row) * max_new + t] = v_tok - (best + logf(ssum));
+        if (sd.logit != nullptr) sd.logit[static_cast<size_t>(row) * max_new + t] = v_tok;
+      }
+    }
     if (pos == nullptr || unf) out_ids[static_cast<size_t>(row) * out_ld + t + 1] = tok;
     bool fin = false;
     if (unf) {
       out_len[row] = t + 1;
-      fin = (kProc ? proc_is_eos(*pd.cfg, tok) : tok == eos_tok) || (pos != nullptr && t + 1 >= max_new);
+      if (forced) {
+        fin = t + 1 >= max_new || sd.forced[static_cast<size_t>(row) * max_new + t + 1] < 0;
+        sd.ftok[b] = fin ? -1 : static_cast<int>(sd.forced[static_cast<size_t>(row) * max_new + t + 1]);
+      } else {
+        fin = (kProc ? proc_is_eos(*pd.cfg, tok) : tok == eos_tok) || (pos != nullptr && t + 1 >= max_new);
+      }
       if (fin) {
         unfinished[b] = 0;
         live_extent[b] = 0;
@@ -366,6 +419,47 @@ __global__ void finalize_step_kernel(const float* __restrict__ pval, const int* 
   if constexpr (kProc) {
     // the row's decoder ids are now its result row up to column t + 1 (written above, visible after the barrier)
     if (s_go) proc_new_bans(pd, pd.row0 + b, out_ids + static_cast<size_t>(out_row != nullptr ? out_row[b] : b) * out_ld, t + 2, true);
+  }
+}
+
+template <bool kProc>
+__global__ void finalize_step_kernel(const float* __restrict__ pval, const int* __restrict__ pidx, int n_tiles,
+                                     DecodeState* st, int* __restrict__ unfinished,
+                                     long long* __restrict__ out_ids, int* __restrict__ out_len, int out_ld,
+                                     long long eos_tok, long long pad_tok, const act_t* __restrict__ E,
+                                     res_t* __restrict__ x, int d, int* __restrict__ live_extent,
+                                     int* __restrict__ pos, const int* __restrict__ out_row, int max_new, ProcDev pd) {
+  finalize_step_body<kProc, false>(pval, pidx, n_tiles, st, unfinished, out_ids, out_len, out_ld, eos_tok, pad_tok, E, x, d,
+                                   live_extent, pos, out_row, max_new, pd, ScoreDev());
+}
+
+template <bool kProc>
+__global__ void finalize_step_score_kernel(const float* __restrict__ pval, const int* __restrict__ pidx, int n_tiles,
+                                           DecodeState* st, int* __restrict__ unfinished,
+                                           long long* __restrict__ out_ids, int* __restrict__ out_len, int out_ld,
+                                           long long eos_tok, long long pad_tok, const act_t* __restrict__ E,
+                                           res_t* __restrict__ x, int d, int* __restrict__ live_extent,
+                                           int* __restrict__ pos, const int* __restrict__ out_row, int max_new, ProcDev pd,
+                                           ScoreDev sd) {
+  finalize_step_body<kProc, true>(pval, pidx, n_tiles, st, unfinished, out_ids, out_len, out_ld, eos_tok, pad_tok, E, x, d,
+                                  live_extent, pos, out_row, max_new, pd, sd);
+}
+
+// Start of a scored call, and of every row of it. With logprob != nullptr: zero the n result elements (positions a
+// row never reaches stay 0, so a row's sum is its log-likelihood). For i < n_set: slot slots[i] (nullptr: i) starts
+// row rows[i] (nullptr: i) and takes its first forced column, -1 without teacher forcing (idle slots, start of a pool).
+__global__ void score_reset_kernel(float* __restrict__ logprob, float* __restrict__ logit, size_t n, int* __restrict__ ftok,
+                                   int n_set, const int* __restrict__ slots, const int* __restrict__ rows,
+                                   const long long* __restrict__ forced, int forced_ld) {
+  const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x, nth = static_cast<size_t>(gridDim.x) * blockDim.x;
+  if (logprob != nullptr)
+    for (size_t i = tid; i < n; i += nth) {
+      logprob[i] = 0.f;
+      logit[i] = 0.f;
+    }
+  for (size_t i = tid; i < static_cast<size_t>(n_set); i += nth) {
+    const int row = rows != nullptr ? rows[i] : static_cast<int>(i);
+    ftok[slots != nullptr ? slots[i] : i] = forced != nullptr ? static_cast<int>(forced[static_cast<size_t>(row) * forced_ld]) : -1;
   }
 }
 

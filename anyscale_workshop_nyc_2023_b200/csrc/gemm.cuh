@@ -15,6 +15,8 @@
 // so each functor first rounds the fp32 accumulator to bf16 and only then fuses
 // the residual add / GeGLU / KV scatter / arg-max.
 #pragma once
+#include <type_traits>
+
 #include "logits_process.cuh"
 #include "ptx.cuh"
 
@@ -606,6 +608,11 @@ struct EpiArgmax {
     int step_stride = 0;  // 1 = slot pool: per-row positions
   };
   static DEVINL void prologue(const Params&, uint8_t*, int, int = 128) {}
+  // the score of column n (shared with EpiScore: the arg-max and the log-sum-exp see the same fp32 number)
+  static DEVINL float value(const Params& p, uint32_t acc, int n, int N, bool block_eos) {
+    const float v = act_round(__uint_as_float(acc));
+    return (n >= N || (block_eos && n == p.eos)) ? -INFINITY : v;
+  }
   // a row's arg-max is not split: the first of the `parts` threads of each row takes the whole row
   template <int BN>
   static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t*, int part, int) {
@@ -621,8 +628,7 @@ struct EpiArgmax {
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const int n = n0 + j;
-        float v = act_round(__uint_as_float(acc[j]));
-        if (n >= N || (block_eos && n == p.eos)) v = -INFINITY;
+        const float v = value(p, acc[j], n, N, block_eos);
         if (v > best) {  // ascending scan + strict '>' keeps the lowest index among equal maxima
           best = v;
           bidx = n;
@@ -650,16 +656,56 @@ struct EpiArgmaxProc {
     int ldv;
   };
   static DEVINL void prologue(const Params&, uint8_t*, int, int = 128) {}
+  // What a row needs of the call's configuration, and the bitmap words of one 32-column chunk of it
+  // (shared with EpiScore, as is `value`).
+  struct Row {
+    bool enc_pen, rep_pen, bad_add;
+    float en, ep, rn, rp;
+    size_t rw;
+    int t;
+  };
+  struct Words {
+    uint32_t ban, seen, enc;
+  };
+  static DEVINL Row row(const Params& p, int m, bool m_ok) {
+    const ProcCfg& cf = *p.pd.cfg;
+    Row r;
+    r.enc_pen = cf.enc_pen;
+    r.rep_pen = cf.rep_pen;
+    r.bad_add = cf.bad_add;
+    r.en = cf.enc_neg;
+    r.ep = cf.enc_pos;
+    r.rn = cf.rep_neg;
+    r.rp = cf.rep_pos;
+    r.rw = static_cast<size_t>(p.pd.row0 + m) * p.pd.W;
+    r.t = m_ok ? p.a.step[m * p.a.step_stride] : 1;
+    return r;
+  }
+  static DEVINL Words words(const Params& p, const Row& r, bool m_ok, int n0) {
+    const int W = p.pd.W, w = n0 >> 5;
+    Words o{0, 0, 0};
+    if (m_ok && w < W) {
+      o.ban = p.pd.banned[r.rw + w] | p.pd.stat[w];
+      if (r.t == 0) o.ban |= p.pd.stat[W + w];
+      if (r.t < p.a.min_new) o.ban |= p.pd.stat[2 * W + w];
+      if (r.rep_pen) o.seen = p.pd.seen[r.rw + w];
+      if (r.enc_pen) o.enc = p.pd.enc[r.rw + w];
+    }
+    return o;
+  }
+  static DEVINL float value(const Row& r, const Words& o, uint32_t acc, int j, int n, int N) {
+    float v = act_round(__uint_as_float(acc));
+    if ((o.enc >> j) & 1u) v = v < 0.f ? v * r.en : v * r.ep;
+    if ((o.seen >> j) & 1u) v = v < 0.f ? v * r.rn : v * r.rp;
+    if (r.bad_add) v = v + 0.f;
+    if (n >= N || ((o.ban >> j) & 1u)) v = -INFINITY;
+    return v;
+  }
   template <int BN>
   static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t*, int part, int) {
     static_assert(BN % 32 == 0, "one bitmap word per 32 columns");
     if (part != 0) return;
-    const ProcCfg& cf = *p.pd.cfg;
-    const int W = p.pd.W;
-    const size_t rw = static_cast<size_t>(p.pd.row0 + m) * W;
-    const int t = m_ok ? p.a.step[m * p.a.step_stride] : 1;
-    const bool enc_pen = cf.enc_pen, rep_pen = cf.rep_pen, bad_add = cf.bad_add;
-    const float en = cf.enc_neg, ep = cf.enc_pos, rn = cf.rep_neg, rp = cf.rep_pos;
+    const Row r = row(p, m, m_ok);
     float best = -INFINITY;
     int bidx = n_tile * BN;
 #pragma unroll 1
@@ -667,23 +713,11 @@ struct EpiArgmaxProc {
       uint32_t acc[32];
       acc_ld_32(taddr + c * 32, acc);
       const int n0 = n_tile * BN + c * 32;
-      const int w = n0 >> 5;
-      uint32_t ban = 0, seen = 0, enc = 0;
-      if (m_ok && w < W) {
-        ban = p.pd.banned[rw + w] | p.pd.stat[w];
-        if (t == 0) ban |= p.pd.stat[W + w];
-        if (t < p.a.min_new) ban |= p.pd.stat[2 * W + w];
-        if (rep_pen) seen = p.pd.seen[rw + w];
-        if (enc_pen) enc = p.pd.enc[rw + w];
-      }
+      const Words o = words(p, r, m_ok, n0);
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const int n = n0 + j;
-        float v = act_round(__uint_as_float(acc[j]));
-        if ((enc >> j) & 1u) v = v < 0.f ? v * en : v * ep;
-        if ((seen >> j) & 1u) v = v < 0.f ? v * rn : v * rp;
-        if (bad_add) v = v + 0.f;
-        if (n >= N || ((ban >> j) & 1u)) v = -INFINITY;
+        const float v = value(r, o, acc[j], j, n, N);
         if (p.vals != nullptr && m_ok && n < N) p.vals[static_cast<size_t>(m) * p.ldv + n] = v;
         if (v > best) {
           best = v;
@@ -694,6 +728,76 @@ struct EpiArgmaxProc {
     if (m_ok) {
       p.a.pval[static_cast<size_t>(m) * p.a.n_tiles + n_tile] = best;
       p.a.pidx[static_cast<size_t>(m) * p.a.n_tiles + n_tile] = bidx;
+    }
+  }
+};
+
+// ---- lm_head + arg-max + log-sum-exp partials (token log-probabilities): what EpiArgmax (kProc = false) or
+// EpiArgmaxProc (kProc = true) emits, from the same per-column values, plus per (row, tile)
+//   psum = sum_n expf(v_n - tile max)   (-inf columns add 0; an all -inf tile emits 0)
+// accumulated in ascending column order by the one thread that owns the row, so it does not depend on where the row
+// sits; finalize_step_score_kernel merges the tiles. The tile is read twice from the staged accumulators: once for
+// the maximum, once for the sum. When the step is teacher-forced, ftok[m] is the row's forced column (-1: none) and
+// the tile that contains it writes its value to fval[m].
+template <bool kProc>
+struct EpiScore {
+  using Base = typename std::conditional<kProc, EpiArgmaxProc, EpiArgmax>::type;
+  struct Params {
+    typename Base::Params b;
+    float* psum;      // [M, n_tiles]
+    float* fval;      // [M]
+    const int* ftok;  // [M], nullptr = the step is not teacher-forced
+    float* vals;      // test hook only, else nullptr: the processed values [M, ldv]
+    int ldv;
+  };
+  static DEVINL void prologue(const Params&, uint8_t*, int, int = 128) {}
+  static DEVINL const EpiArgmax::Params& arg(const Params& p) {
+    if constexpr (kProc) return p.b.a;
+    else return p.b;
+  }
+  template <int BN>
+  static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t*, int part, int) {
+    if (part != 0) return;
+    const EpiArgmax::Params& a = arg(p);
+    EpiArgmaxProc::Row r{};
+    bool block_eos = false;
+    if constexpr (kProc) r = EpiArgmaxProc::row(p.b, m, m_ok);
+    else block_eos = m_ok && a.step[m * a.step_stride] < a.min_new;
+    const int forced = (m_ok && p.ftok != nullptr) ? p.ftok[m] : -1;
+    float best = -INFINITY, sum = 0.f;
+    int bidx = n_tile * BN;
+#pragma unroll 1
+    for (int pass = 0; pass < 2; ++pass) {
+#pragma unroll 1
+      for (int c = 0; c < BN / 32; ++c) {
+        uint32_t acc[32];
+        acc_ld_32(taddr + c * 32, acc);
+        const int n0 = n_tile * BN + c * 32;
+        EpiArgmaxProc::Words o{0, 0, 0};
+        if constexpr (kProc) o = EpiArgmaxProc::words(p.b, r, m_ok, n0);
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const int n = n0 + j;
+          float v;
+          if constexpr (kProc) v = EpiArgmaxProc::value(r, o, acc[j], j, n, N);
+          else v = EpiArgmax::value(a, acc[j], n, N, block_eos);
+          if (pass == 0) {
+            if (v > best) {
+              best = v;
+              bidx = n;
+            }
+            if (n == forced) p.fval[m] = v;
+            if (p.vals != nullptr && m_ok && n < N) p.vals[static_cast<size_t>(m) * p.ldv + n] = v;
+          } else if (v != -INFINITY) {
+            sum += expf(v - best);
+          }
+        }
+      }
+    }
+    if (m_ok) {
+      a.pval[static_cast<size_t>(m) * a.n_tiles + n_tile] = best;
+      a.pidx[static_cast<size_t>(m) * a.n_tiles + n_tile] = bidx;
+      p.psum[static_cast<size_t>(m) * a.n_tiles + n_tile] = sum;
     }
   }
 };

@@ -144,6 +144,61 @@ def logits_processor_args(kw: Dict[str, Any], eos_ids, default_eos: int, vocab_s
     return _LogitsArgs(p, arrays, eos_list) if active else None
 
 
+class TokenScores:
+    """What `generate(..., output_scores=True)` returns as `.scores`: per generated position, the chosen token's
+    processed score (`token_logits`) and its log-softmax (`token_logprobs`), fp32 [B, T'], 0 after a row's EOS.
+    NOT transformers' tuple of T' tensors [B, vocab]: the fused lm_head epilogue never writes the vocabulary-wide
+    scores. `compute_transition_scores` accepts it in place of that tuple."""
+
+    def __init__(self, token_logprobs, token_logits):
+        self.token_logprobs = token_logprobs
+        self.token_logits = token_logits
+
+    def __len__(self):
+        return int(self.token_logprobs.shape[1])
+
+
+class GenerateOutput:
+    """`generate(..., return_dict_in_generate=True)`: `.sequences` is the tensor a plain call returns, `.scores` a
+    TokenScores (None without output_scores=True), `.token_logprobs` a shortcut to scores.token_logprobs."""
+
+    def __init__(self, sequences, scores: Optional[TokenScores] = None):
+        self.sequences = sequences
+        self.scores = scores
+        self.token_logprobs = None if scores is None else scores.token_logprobs
+
+    def __getitem__(self, key):
+        return getattr(self, key)
+
+
+def generate_output_flags(kw: Dict[str, Any]):
+    """(return_dict_in_generate, output_scores) of a generate call. The outputs the CUDA path cannot give raise
+    instead of being dropped."""
+    for k in ("output_logits", "output_attentions", "output_hidden_states"):
+        if kw.get(k):
+            raise NotImplementedError(f"generate({k}=True) is not supported by the CUDA path")
+    return bool(kw.get("return_dict_in_generate")), bool(kw.get("output_scores"))
+
+
+def score_labels(labels, vocab_size: int) -> np.ndarray:
+    """Validate `labels` of score() as int64 [B, L]: ids in [0, vocab_size) or -100, every row with at least one
+    label, -100 only after a row's last label (teacher forcing stops there)."""
+    if labels is None:
+        raise ValueError("labels is required")
+    lab = np.ascontiguousarray(labels.detach().cpu().numpy() if isinstance(labels, torch.Tensor) else labels)
+    if lab.ndim != 2 or lab.shape[1] < 1 or lab.dtype.kind not in "iu":
+        raise ValueError(f"labels must be integers [batch, length >= 1], got {lab.dtype} {lab.shape}")
+    lab = lab.astype(np.int64)
+    ignored = lab == -100
+    if ((lab < 0) & ~ignored).any() or (lab >= vocab_size).any():
+        raise ValueError(f"labels contain ids outside [0, {vocab_size}) other than -100")
+    if ignored[:, 0].any():
+        raise ValueError("every row of labels needs at least one label")
+    if (ignored[:, :-1] & ~ignored[:, 1:]).any():
+        raise ValueError("labels: -100 may only follow a row's last label")
+    return lab
+
+
 def _chk(model, rc: int, handle=None) -> None:
     _lib.check(rc, handle, model._lib)
 
@@ -339,7 +394,11 @@ class B200T5ForConditionalGeneration:
         change greedy decoding are accepted and ignored, as HF itself does (generation/utils.py:583).
         transformers' greedy logits processors are applied on the GPU: repetition_penalty,
         encoder_repetition_penalty, no_repeat_ngram_size, encoder_no_repeat_ngram_size, bad_words_ids,
-        suppress_tokens, begin_suppress_tokens, and eos_token_id given as a list."""
+        suppress_tokens, begin_suppress_tokens, and eos_token_id given as a list.
+        return_dict_in_generate=True returns a GenerateOutput (`.sequences` = that tensor); with output_scores=True its
+        `.scores` / `.token_logprobs` carry each generated token's processed score and log-probability, computed in
+        the lm_head epilogue (see TokenScores, compute_transition_scores). output_logits / output_attentions /
+        output_hidden_states raise NotImplementedError."""
         if input_ids is None:
             input_ids = unused.pop("inputs", None)
         if input_ids is None:
@@ -353,12 +412,21 @@ class B200T5ForConditionalGeneration:
         for k in ("logits_processor", "stopping_criteria", "forced_bos_token_id", "decoder_input_ids", "encoder_outputs"):
             if unused.get(k) is not None:  # (may be tensors: no truth-value tests)
                 raise NotImplementedError(f"generate({k}=...) is not supported by the CUDA path")
+        as_dict, want_scores = generate_output_flags(unused)
         gp = self._gen_params(max_new_tokens, max_length, min_new_tokens, min_length, eos_token_id, pad_token_id,
                               decoder_start_token_id, poll_interval)
         lp = self._logits_args(unused, eos_token_id)
         host = torch.as_tensor(input_ids)
         if host.dim() != 2:
             raise ValueError(f"input_ids must be [batch, seq], got {tuple(host.shape)}")
+        if as_dict:
+            if not want_scores:  # the unchanged greedy call, wrapped
+                return GenerateOutput(self.generate(input_ids=input_ids, attention_mask=attention_mask, max_new_tokens=gp.max_new_tokens,
+                                                    min_new_tokens=gp.min_new_tokens, eos_token_id=eos_token_id, pad_token_id=pad_token_id,
+                                                    decoder_start_token_id=decoder_start_token_id, poll_interval=poll_interval,
+                                                    **{k: unused[k] for k in LOGITS_PROCESSOR_KWARGS if k in unused}))
+            seq, _, logp, logit = self._run_scored(host, attention_mask, gp, lp, None)
+            return GenerateOutput(seq, TokenScores(logp, logit))
         if self.takes_host_batches(host.shape[0], host.shape[1]) and host.device.type == "cpu":
             # more rows than one pool of decode slots, still in host memory: the slot pool admits prompts from host
             # buffers as slots free up, so nothing is copied to the device (and back) up front
@@ -390,6 +458,70 @@ class B200T5ForConditionalGeneration:
             pad = gp.pad_token_id if gp.pad_token_id >= 0 else self.generation_config.pad_token_id
             return torch.cat([torch.nn.functional.pad(o, (0, width - o.shape[1]), value=pad) for o in outs], dim=0)
         return self._generate_static(ids, mask, gp, lp)
+
+    def compute_transition_scores(self, sequences, scores, beam_indices=None, normalize_logits: bool = False):
+        """transformers' GenerationMixin.compute_transition_scores for the `.scores` of this model's generate: the
+        chosen tokens' log-probabilities (normalize_logits=True) or processed scores (False), fp32 [B, T']. One
+        deviation: positions after a row's EOS are 0 (transformers reports the score of the pad token it fed)."""
+        if not isinstance(scores, TokenScores):
+            raise TypeError("scores must be the `.scores` of this model's generate(..., output_scores=True)")
+        if beam_indices is not None:
+            raise NotImplementedError("beam search is not implemented")
+        return scores.token_logprobs if normalize_logits else scores.token_logits
+
+    @torch.no_grad()
+    def score(self, input_ids, attention_mask=None, labels=None):
+        """Teacher-forced log-likelihood of given targets, `T5ForConditionalGeneration(input_ids, attention_mask,
+        labels=labels)` without the logits: labels int64 [B, L], -100 after a row's last label. Returns
+        `.token_logprobs` fp32 [B, L] = log p(label | prompt, earlier labels) (0 at ignored positions), `.lengths` (labels
+        per row) and `.loss` = -sum / count over all labels, transformers' mean cross-entropy. More rows than
+        `pool_size` go through the slot pool; each (prompt, target) pair is a row."""
+        lab = score_labels(labels, self.config.vocab_size)
+        gp = _lib.GenParams(max_new_tokens=lab.shape[1], min_new_tokens=0, eos_token_id=-1, pad_token_id=-1,
+                            decoder_start_token_id=-1, poll_interval=8)
+        host = torch.as_tensor(input_ids)
+        if host.dim() != 2 or host.shape[0] != lab.shape[0]:
+            raise ValueError(f"input_ids must be [batch, seq] with one row per row of labels, got {tuple(host.shape)}")
+        _, lens, logp, _ = self._run_scored(host, attention_mask, gp, None, lab)
+        count = int((lab != -100).sum())
+        return SimpleNamespace(token_logprobs=logp, lengths=lens, loss=-(logp.double().sum() / count).float())
+
+    def _run_scored(self, host: torch.Tensor, attention_mask, gp, lp, labels: Optional[np.ndarray]):
+        """generate's routing (static batch, slot pool, static chunks) for a scored call: (sequences [B, 1+T'],
+        lengths [B], token_logprobs [B, T'], token_logits [B, T']) on the device. With `labels` the call is
+        teacher-forced and T' = labels.shape[1]."""
+        ids = host.to(device=self._device, dtype=torch.long).contiguous()
+        B, S = ids.shape
+        if ids.numel():
+            lo, hi = torch.aminmax(ids)
+            if bool(((lo < 0) | (hi >= self.config.vocab_size)).item()):
+                raise IndexError("input_ids contain token ids outside [0, vocab_size)")
+        if attention_mask is not None:
+            mask = torch.as_tensor(attention_mask).to(device=self._device, dtype=torch.long).contiguous()
+            if mask.shape != ids.shape:
+                raise ValueError("attention_mask shape must match input_ids")
+        else:
+            mask = self._infer_attention_mask(ids, gp, lp)
+        T = gp.max_new_tokens
+        if B > self.pool_size and self.takes_host_batches(B, S):
+            out, lens, logp, logit = self.generate_stream(ids.cpu().numpy(), None if mask is None else mask.cpu().numpy(),
+                                                          _gen_params=gp, _logits=lp, _labels=labels, output_scores=True)
+            out, lens, logp, logit = (torch.from_numpy(np.ascontiguousarray(a)).to(self._device) for a in (out, lens, logp, logit))
+        else:
+            parts = [self._generate_static(ids[lo:lo + self.pool_size], None if mask is None else mask[lo:lo + self.pool_size], gp, lp,
+                                           score=True, labels=None if labels is None else labels[lo:lo + self.pool_size])
+                     for lo in range(0, B, self.pool_size)]
+            out, lens, logp, logit = (torch.cat([p[i] for p in parts], dim=0) for i in range(4))
+        steps = T if labels is not None else int(lens.max().item())
+        return out[:, : steps + 1], lens, logp[:, :steps], logit[:, :steps]
+
+    def _score_io(self, logp, logit, labels):
+        """b200t5_score_io over two result arrays and optional labels (torch tensors or numpy arrays, all on the side
+        the entry point expects); returns the struct and what must stay alive with it."""
+        ptr = (lambda a: C.c_void_p(a.data_ptr())) if isinstance(logp, torch.Tensor) else (lambda a: a.ctypes.data_as(C.c_void_p))
+        io = _lib.ScoreIO(token_logprobs=ptr(logp), token_logits=ptr(logit), forced_ids=None if labels is None else ptr(labels),
+                          forced_len=0 if labels is None else int(labels.shape[1]))
+        return io, (logp, logit, labels)
 
     def takes_host_batches(self, B: int, S: int) -> bool:
         """True when a [B, S] batch would go through the slot pool, whose entry point takes HOST buffers: a caller that
@@ -426,7 +558,7 @@ class B200T5ForConditionalGeneration:
             return None
         return (~is_pad).to(torch.long).contiguous()
 
-    def _generate_static(self, ids: torch.Tensor, mask: Optional[torch.Tensor], gp, lp=None) -> torch.Tensor:
+    def _generate_static(self, ids: torch.Tensor, mask: Optional[torch.Tensor], gp, lp=None, score: bool = False, labels=None):
         B, S = ids.shape
         ids = ids.contiguous()
         mask = None if mask is None else mask.contiguous()
@@ -436,6 +568,17 @@ class B200T5ForConditionalGeneration:
             lens = torch.empty((B,), dtype=torch.int32, device=self._device)
             stream = torch.cuda.current_stream(self._device)
             with self._gpu_lock:
+                if score:  # full-width results: (ids [B, T+1], lengths, token_logprobs [B, T], token_logits [B, T])
+                    logp = torch.empty((B, T), dtype=torch.float32, device=self._device)
+                    logit = torch.empty((B, T), dtype=torch.float32, device=self._device)
+                    forced = None if labels is None else torch.from_numpy(np.ascontiguousarray(labels)).to(self._device)
+                    io, _keep = self._score_io(logp, logit, forced)
+                    _chk(self, self._lib.b200t5_generate_scored(self._h, _ptr(ids), _ptr(mask), B, S, C.byref(gp),
+                                                                None if lp is None else lp.ref(), _ptr(out), _ptr(lens), C.byref(io),
+                                                                C.c_void_p(stream.cuda_stream)), self._h)
+                    self.last_lengths = lens
+                    torch.cuda.current_stream(self._device).synchronize()
+                    return out, lens, logp, logit
                 if lp is None:
                     rc = self._lib.b200t5_generate(self._h, _ptr(ids), _ptr(mask), B, S, C.byref(gp), _ptr(out), _ptr(lens),
                                                    C.c_void_p(stream.cuda_stream))
@@ -456,7 +599,8 @@ class B200T5ForConditionalGeneration:
     def generate_host(self, input_ids: np.ndarray, attention_mask: Optional[np.ndarray] = None, **kw):
         """numpy in / numpy out through b200t5_generate_host (the foreign-host entry point):
         H2D copy, generation, D2H copy and synchronisation all happen inside the library. Takes the logits
-        processor kwargs `generate` takes (through b200t5_generate_host_ex)."""
+        processor kwargs `generate` takes (through b200t5_generate_host_ex). With output_scores=True it returns
+        (ids, lengths, token_logprobs, token_logits), the last two fp32 [B, T'] (b200t5_generate_host_scored)."""
         gp = self._gen_params(kw.get("max_new_tokens"), kw.get("max_length"), kw.get("min_new_tokens"),
                               kw.get("min_length"), kw.get("eos_token_id"), kw.get("pad_token_id"),
                               kw.get("decoder_start_token_id"), kw.get("poll_interval", 8))
@@ -466,8 +610,18 @@ class B200T5ForConditionalGeneration:
         mask = self._infer_mask_np(ids, gp, lp) if attention_mask is None else np.ascontiguousarray(attention_mask, dtype=np.int64)
         out = np.empty((B, gp.max_new_tokens + 1), dtype=np.int64)
         lens = np.empty((B,), dtype=np.int32)
+        want_scores = generate_output_flags(kw)[1]
         with self._gpu_lock:
             mp = None if mask is None else mask.ctypes.data_as(C.c_void_p)
+            if want_scores:  # -> (ids, lengths, token_logprobs, token_logits), numpy
+                logp = np.empty((B, gp.max_new_tokens), dtype=np.float32)
+                logit = np.empty((B, gp.max_new_tokens), dtype=np.float32)
+                io, _keep = self._score_io(logp, logit, None)
+                _chk(self, self._lib.b200t5_generate_host_scored(self._h, ids.ctypes.data_as(C.c_void_p), mp, B, S, C.byref(gp),
+                                                                 None if lp is None else lp.ref(), out.ctypes.data_as(C.c_void_p),
+                                                                 lens.ctypes.data_as(C.c_void_p), C.byref(io)), self._h)
+                steps = int(lens.max())
+                return out[:, : steps + 1], lens, logp[:, :steps], logit[:, :steps]
             if lp is None:
                 rc = self._lib.b200t5_generate_host(self._h, ids.ctypes.data_as(C.c_void_p), mp, B, S, C.byref(gp),
                                                     out.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p))
@@ -478,12 +632,14 @@ class B200T5ForConditionalGeneration:
         return out[:, : int(lens.max()) + 1], lens
 
     def generate_stream(self, input_ids: np.ndarray, attention_mask: Optional[np.ndarray] = None, *, pool: Optional[int] = None,
-                        admit_min: int = 0, _gen_params=None, _logits=None, **kw):
+                        admit_min: int = 0, _gen_params=None, _logits=None, _labels=None, **kw):
         """N prompts through a pool of decode slots (b200t5_generate_stream): a slot whose row has finished is
         refilled with the next prompt, so short answers do not wait for the slowest row of a fixed batch as they do
         when BatchPredictor hands `generate` one batch at a time (NB:908-913 -> JOB/predictor.py:102). Returns
         (int64 [N, 1+T'], int32 lengths [N]) with the rows in input order; every row equals what `generate` returns
-        for that prompt. Takes the logits processor kwargs `generate` takes (through b200t5_generate_stream_ex)."""
+        for that prompt. Takes the logits processor kwargs `generate` takes (through b200t5_generate_stream_ex). With
+        output_scores=True it returns (ids, lengths, token_logprobs, token_logits), the last two fp32 [N, T']
+        (b200t5_generate_stream_scored)."""
         gp = _gen_params or self._gen_params(kw.get("max_new_tokens"), kw.get("max_length"), kw.get("min_new_tokens"),
                                              kw.get("min_length"), kw.get("eos_token_id"), kw.get("pad_token_id"),
                                              kw.get("decoder_start_token_id"), kw.get("poll_interval", 8))
@@ -499,8 +655,20 @@ class B200T5ForConditionalGeneration:
             raise ValueError("attention_mask shape must match input_ids")
         out = np.empty((N, gp.max_new_tokens + 1), dtype=np.int64)
         lens = np.empty((N,), dtype=np.int32)
+        want_scores = generate_output_flags(kw)[1]
         with self._gpu_lock:
             mp = None if mask is None else mask.ctypes.data_as(C.c_void_p)
+            if want_scores:
+                logp = np.empty((N, gp.max_new_tokens), dtype=np.float32)
+                logit = np.empty((N, gp.max_new_tokens), dtype=np.float32)
+                io, _keep = self._score_io(logp, logit, None if _labels is None else np.ascontiguousarray(_labels, dtype=np.int64))
+                _chk(self, self._lib.b200t5_generate_stream_scored(self._h, ids.ctypes.data_as(C.c_void_p), mp, N, S, C.byref(gp),
+                                                                   None if lp is None else lp.ref(), int(pool or self.pool_slots),
+                                                                   int(admit_min), out.ctypes.data_as(C.c_void_p),
+                                                                   lens.ctypes.data_as(C.c_void_p), C.byref(io)), self._h)
+                self.last_lengths = torch.from_numpy(lens)
+                steps = int(lens.max())
+                return out[:, : steps + 1], lens, logp[:, :steps], logit[:, :steps]
             if lp is None:
                 rc = self._lib.b200t5_generate_stream(self._h, ids.ctypes.data_as(C.c_void_p), mp, N, S, C.byref(gp),
                                                       int(pool or self.pool_slots), int(admit_min),

@@ -109,6 +109,26 @@ typedef struct b200t5_logits_params {
                                       * the decoder ids */
 } b200t5_logits_params;
 
+/* Token log-probabilities of a call (the *_scored entry points). At every step the lm_head epilogue keeps, beside the
+ * arg-max, the log-sum-exp of the step's processed fp32 scores (the act-rounded logits after the logits processors and
+ * the EOS mask), so for the token t a row takes at step s
+ *   token_logits[row][s]   = score[t]                                  (what the arg-max compared)
+ *   token_logprobs[row][s] = score[t] - max - log(sum exp(score - max))  = log_softmax(score)[t]
+ * without the [rows, vocab] scores ever reaching memory. Positions a row does not reach (after its EOS) hold 0, so the
+ * sum of a row of token_logprobs is the log-likelihood of its sequence. Both arrays are fp32 [rows, max_new_tokens].
+ * forced_ids (teacher forcing): instead of the arg-max, row r takes forced_ids[r][s] at step s, until its last label -
+ * the position before the first -100 or forced_len - and not until an EOS; out_ids then echoes the labels and
+ * token_logprobs are log p(label | prompt, earlier labels), what a cross-entropy loss sums. Every row needs at least
+ * one label, labels lie in [0, vocab_size), -100 may only trail, 1 <= forced_len <= max_new_tokens, and logits
+ * processors cannot be combined with forced_ids: B200T5_EINVAL otherwise.
+ * The pointers are device pointers for b200t5_generate_scored and host pointers for the other two entry points. */
+typedef struct b200t5_score_io {
+  float* token_logprobs;      /* out, fp32 [rows, max_new_tokens]; 0 where the row has no token */
+  float* token_logits;        /* out, may be NULL: the processed score of the chosen token */
+  const int64_t* forced_ids;  /* in, may be NULL: [rows, forced_len], -100 after a row's last label */
+  int32_t forced_len;         /* <= max_new_tokens */
+} b200t5_score_io;
+
 typedef struct b200t5_stats {
   float encoder_ms;       /* encoder + cross-KV projection of the last generate call (CUDA events) */
   float decode_ms;        /* decode loop of the last generate call (CUDA events) */
@@ -170,6 +190,18 @@ int b200t5_generate_host_ex(b200t5_handle h, const int64_t* input_ids, const int
 int b200t5_generate_stream_ex(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int64_t N, int S,
                               const b200t5_gen_params* params, const b200t5_logits_params* logits, int pool,
                               int admit_min, int64_t* out_ids, int32_t* out_len);
+/* The three entry points above with token log-probabilities (`score` may be NULL: the call is exactly the one above,
+ * same graphs, same number of kernel launches). rows = B, or N for the slot pool. A row's numbers do not depend on the
+ * entry point, the batch or the slot it is decoded in: the three return bit-identical arrays for the same prompt. */
+int b200t5_generate_scored(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                           const b200t5_gen_params* params, const b200t5_logits_params* logits, int64_t* out_ids,
+                           int32_t* out_len, const b200t5_score_io* score, void* stream);
+int b200t5_generate_host_scored(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                                const b200t5_gen_params* params, const b200t5_logits_params* logits, int64_t* out_ids,
+                                int32_t* out_len, const b200t5_score_io* score);
+int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int64_t N, int S,
+                                  const b200t5_gen_params* params, const b200t5_logits_params* logits, int pool,
+                                  int admit_min, int64_t* out_ids, int32_t* out_len, const b200t5_score_io* score);
 int b200t5_get_stats(b200t5_handle h, b200t5_stats* out);
 
 /* ---- measurement hooks (bench.py) --------------------------------------------------- */
@@ -212,6 +244,14 @@ int b200t5_test_lm_argmax(int device, const void* x, const void* W, int M, int V
 int b200t5_test_lm_process(int device, const void* x, const void* W, int M, int V, int K, int step, int eos, int min_new,
                            const b200t5_logits_params* logits, const int64_t* hist, const int64_t* enc_ids, int S,
                            int64_t* tokens, float* vals, void* stream);
+/* One decode step of a scored call as the step graph runs it (csrc/gemm.cuh EpiScore -> finalize_step_score_kernel):
+ * arguments as b200t5_test_lm_process, where `logits`, hist and enc_ids may be NULL (no processors); forced int64 [M]
+ * (device, may be NULL) the tokens to take instead of the arg-max. tokens int64 [M], logprob and logit fp32 [M]
+ * (device): the token taken, its log-probability and its processed score; vals as in b200t5_test_lm_process.
+ * Test hook; both builds. */
+int b200t5_test_lm_score(int device, const void* x, const void* W, int M, int V, int K, int step, int eos, int min_new,
+                         const b200t5_logits_params* logits, const int64_t* hist, const int64_t* enc_ids, int S,
+                         const int64_t* forced, int64_t* tokens, float* logprob, float* logit, float* vals, void* stream);
 
 /* ---- parity hooks (used by tests/ only) --------------------------------------------- */
 /* Encoder last hidden state after the final RMSNorm, bf16 [B,S,d_model] (device). */
