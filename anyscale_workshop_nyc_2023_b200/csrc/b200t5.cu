@@ -179,7 +179,7 @@ struct DevBuf {
 };
 
 // Which epilogue/tile a GEMM uses.
-enum GemmKind { G_STORE256, G_RES256, G_GEGLU256, G_CROSSKV256, G_QKVDEC64, G_STORE32, G_RES32, G_GEGLU64, G_ARGMAX128, G_LOGITS128, G_ARGMAXPROC128, G_SCORE128, G_SCOREPROC128 };
+enum GemmKind { G_STORE256, G_RES256, G_GEGLU256, G_CROSSKV256, G_QKVDEC64, G_STORE32, G_RES32, G_GEGLU64, G_LOGITS128 };
 
 struct GemmOp {
   CUtensorMap tmA, tmB;
@@ -213,12 +213,10 @@ struct ProcHost {
 // Device state of the processors for `rows` rows (logits_process.cuh: ProcDev). The step graph bakes these
 // addresses: a reallocation means a new graph.
 // Host form of a call's scoring request (b200t5_score_io after validation). `forced`: the labels padded with -100 to
-// [rows, max_new_tokens], as the step kernels read them. lp / lg: device destinations of the two result arrays.
+// [rows, max_new_tokens], as the step kernels read them.
 struct ScoreHost {
   bool on = false;
   std::vector<long long> forced;
-  float* lp = nullptr;
-  float* lg = nullptr;
 };
 
 struct ProcBufs {
@@ -298,29 +296,34 @@ struct Plan {
   DevBuf self_kv;                       // [Ld][2][B][H][Tmax][64]
   DevBuf dec_bias;                      // float [H][Tmax]
   DevBuf pval, pidx;                    // [B][n_tiles]
-  DevBuf state, unfinished, out_ids, out_len, ids_dev, mask_dev;
+  DevBuf state, unfinished, ids_dev, mask_dev;
   // what the decode kernels attend to: copies of extent / key_ok in which a finished row's extent drops to 0
   // (retired: its K/V are no longer streamed). In slot-pool mode they describe the slots' CURRENT prompts while
   // extent / key_ok describe the prompts of the encoder pass being admitted.
   DevBuf live_extent, live_key_ok;
   DevBuf xs_stamps, xs_acc;  // in-situ profile of the cross-attention launches: [Ld * chains][2] stamps / {ns, launches}, then [Ld][2] {busy ns, layers}
-  // slot pool (b200t5_generate_stream): per-slot position and result row, admission lists, [N, Tmax+1] results
+  // slot pool (b200t5_generate_stream): per-slot position and result row, admission lists
   DevBuf pos, out_row, admit;
-  DevBuf stream_out, stream_len;
-  // logits processors (allocated by the first call that uses them); proc_on: this call's step runs EpiArgmaxProc
+  // A call's results, by row: ids [cap][Tmax+1] and lengths [cap]; for a scored call (allocated by the first one)
+  // log-probabilities and processed scores [cap][Tmax], and the labels [cap][Tmax] of a teacher-forced one. `batch`
+  // holds the static batch's B rows, `pool` the slot pool's N rows in input order (cap >= N: it only grows). The step
+  // graph bakes these addresses: a reallocation drops it.
+  struct Results {
+    DevBuf ids, len, lp, lg, forced;
+    size_t cap = 0;
+  };
+  Results batch, pool;
+  Results& res() { return stream_mode ? pool : batch; }
+  // logits processors (allocated by the first call that uses them); proc_on: this call's step runs EpiLmHead<true, *>
   ProcBufs proc;
   bool proc_on = false;
   int g_proc = -1;
   // token log-probabilities (allocated by the first call that asks for them); score_on: 0 = this call's step runs the
-  // plain arg-max kernels, 1 = EpiScore + finalize_step_score_kernel, 2 = those with teacher forcing. Part of the
+  // plain head, 1 = EpiLmHead<*, true> + finalize_step_kernel<*, true>, 2 = those with teacher forcing. Part of the
   // step graph's key, like proc_on.
   DevBuf psum, fval, ftok;              // [B][n_tiles], [B], [B]
-  DevBuf score_lp, score_lg, forced;    // [B][Tmax] results and labels of a static batch
-  DevBuf stream_lp, stream_lg, stream_forced;  // [stream_cap][Tmax]: the slot pool's
-  size_t score_stream_cap = 0;
   int score_on = 0;
   int g_score = -1;
-  size_t stream_cap = 0;   // rows stream_out / stream_len hold (the step graph bakes their addresses)
   bool stream_mode = false;
   int g_stream = -1;
   int g_xattn = -1;           // cross-attention kernel baked into the step graph (0 per-thread-load, 1 stream)
@@ -501,18 +504,34 @@ static cudaError_t run_gemm(b200t5_ctx* h, const GemmOp& g, const void* ep, cuda
       return launch_gemm<32, EpiResidual>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiResidual::Params*>(ep), h->num_sms, s, pdl);
     case G_GEGLU64:
       return launch_gemm<64, EpiGeglu>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiGeglu::Params*>(ep), h->num_sms, s, pdl);
-    case G_ARGMAX128:
-      return launch_gemm<128, EpiArgmax>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiArgmax::Params*>(ep), h->num_sms, s, pdl);
     case G_LOGITS128:
       return launch_gemm<128, EpiStoreF32>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiStoreF32::Params*>(ep), h->num_sms, s, pdl);
-    case G_ARGMAXPROC128:
-      return launch_gemm<128, EpiArgmaxProc>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiArgmaxProc::Params*>(ep), h->num_sms, s, pdl);
-    case G_SCORE128:
-      return launch_gemm<128, EpiScore<false>>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiScore<false>::Params*>(ep), h->num_sms, s, pdl);
-    case G_SCOREPROC128:
-      return launch_gemm<128, EpiScore<true>>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiScore<true>::Params*>(ep), h->num_sms, s, pdl);
   }
   return cudaErrorInvalidValue;
+}
+
+// The decode step's head, indexed [kProc][kScore]: the lm_head GEMM with its fused epilogue (gemm.cuh: EpiLmHead) and
+// the kernel that merges the epilogue's partials (elementwise.cuh: finalize_step_kernel).
+struct LmHead {
+  cudaError_t (*gemm)(const CUtensorMap&, const CUtensorMap&, int, int, int, int, const LmHeadParams&, int, cudaStream_t, bool, int);
+  void (*finalize)(FinalizeArgs);
+  cudaError_t (*prepare)();
+};
+template <bool kProc, bool kScore>
+constexpr LmHead lm_head_of() {
+  return {launch_gemm<128, EpiLmHead<kProc, kScore>>, finalize_step_kernel<kProc, kScore>, prepare_gemm<128, EpiLmHead<kProc, kScore>>};
+}
+static const LmHead kLmHeads[2][2] = {{lm_head_of<false, false>(), lm_head_of<false, true>()},
+                                      {lm_head_of<true, false>(), lm_head_of<true, true>()}};
+
+// the head of M rows x N columns: tmA holds the rows' normalised activations [M, K], tmB the lm_head weight [N, K]
+static cudaError_t run_lm_head(b200t5_ctx* h, bool proc, bool score, const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N,
+                               int K, const LmHeadParams& ep, const FinalizeArgs& fa, cudaStream_t s, bool pdl) {
+  const LmHead& lh = kLmHeads[proc][score];
+  h->launches += 2;
+  cudaError_t e = lh.gemm(tmA, tmB, M, N, K, 1, ep, h->num_sms, s, pdl, 0);
+  if (e == cudaSuccess) e = launch_kernel(lh.finalize, dim3(M), dim3(128), 0, s, pdl, fa);
+  return e;
 }
 
 // encoder GEMM, 128 x 256 tiles (gemm_2cta.cuh)
@@ -569,10 +588,12 @@ static cudaError_t init_kernel_attrs() {
 #define PREP(BN, EPI)                         \
   if ((e = prepare_gemm<BN, EPI>()) != cudaSuccess) return e;
   PREP(256, EpiStore) PREP(256, EpiResidual) PREP(256, EpiGeglu) PREP(256, EpiCrossKV) PREP(64, EpiQkvDecode)
-  PREP(32, EpiStore) PREP(32, EpiResidual) PREP(64, EpiGeglu) PREP(128, EpiArgmax) PREP(128, EpiStoreF32) PREP(128, EpiArgmaxProc)
-  PREP(128, EpiScore<false>) PREP(128, EpiScore<true>)
+  PREP(32, EpiStore) PREP(32, EpiResidual) PREP(64, EpiGeglu) PREP(128, EpiStoreF32)
   PREP(64, EpiStore) PREP(128, EpiStore)
 #undef PREP
+  for (const auto& row : kLmHeads)
+    for (const LmHead& lh : row)
+      if ((e = lh.prepare()) != cudaSuccess) return e;
   if ((e = prepare_gemm_2cta<EpiStore>()) != cudaSuccess) return e;
   if ((e = prepare_gemm_2cta<EpiResidual>()) != cudaSuccess) return e;
   if ((e = prepare_gemm_2cta<EpiGeglu>()) != cudaSuccess) return e;
@@ -1070,8 +1091,9 @@ static int build_plan(b200t5_ctx* h, int B, int S, int Tmax) {
   CU_OK(h, pl->pidx.alloc(static_cast<size_t>(B) * pl->n_vtiles * 4));
   CU_OK(h, pl->state.alloc(sizeof(DecodeState)));
   CU_OK(h, pl->unfinished.alloc(static_cast<size_t>(B) * 4));
-  CU_OK(h, pl->out_ids.alloc(static_cast<size_t>(B) * (Tmax + 1) * 8));
-  CU_OK(h, pl->out_len.alloc(static_cast<size_t>(B) * 4));
+  CU_OK(h, pl->batch.ids.alloc(static_cast<size_t>(B) * (Tmax + 1) * 8));
+  CU_OK(h, pl->batch.len.alloc(static_cast<size_t>(B) * 4));
+  pl->batch.cap = static_cast<size_t>(B);
   CU_OK(h, pl->ids_dev.alloc(M * 8));
   CU_OK(h, pl->mask_dev.alloc(M * 8));
   CU_OK(h, cudaMallocHost(&pl->h_ids, M * 8));
@@ -1381,58 +1403,39 @@ static int chain_head(b200t5_ctx* h, cudaStream_t s, const ChainView& v, float* 
   Plan& p = *h->plan;
   const int d = c.d, T = p.Tmax;
   const bool pdl = h->use_pdl;
-  DecodeState* st = p.state.as<DecodeState>();
   CU_OK(h, run_rmsnorm(h, v.dx, h->dec_final_ln.as<act_t>(), v.dxn, v.nb, d, c.eps, s, pdl));
   if (logits_out) {
     EpiStoreF32::Params ep{logits_out + static_cast<size_t>(v.b0) * ldl, ldl};
     CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, G_LOGITS128, 1), &ep, s, pdl));
-  } else {
-    float* pval = p.pval.as<float>() + static_cast<size_t>(v.b0) * p.n_vtiles;
-    int* pidx = p.pidx.as<int>() + static_cast<size_t>(v.b0) * p.n_vtiles;
-    const bool sm = p.stream_mode;
-    EpiArgmax::Params ep{pval, pidx, p.n_vtiles, sm ? p.pos.as<int>() + v.b0 : &st->step, static_cast<int>(eos), min_new, sm ? 1 : 0};
-    const ProcDev pd = p.proc_on ? p.proc.dev(v.b0) : ProcDev();
-    const int* ftok = p.score_on == 2 ? p.ftok.as<int>() + v.b0 : nullptr;
-    float* psum = p.psum.as<float>() + static_cast<size_t>(v.b0) * p.n_vtiles;
-    if (p.score_on && p.proc_on) {
-      EpiScore<true>::Params eps{{ep, pd, nullptr, 0}, psum, p.fval.as<float>() + v.b0, ftok, nullptr, 0};
-      CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, G_SCOREPROC128, 1), &eps, s, pdl));
-    } else if (p.score_on) {
-      EpiScore<false>::Params eps{ep, psum, p.fval.as<float>() + v.b0, ftok, nullptr, 0};
-      CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, G_SCORE128, 1), &eps, s, pdl));
-    } else if (p.proc_on) {
-      EpiArgmaxProc::Params epp{ep, pd, nullptr, 0};
-      CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, G_ARGMAXPROC128, 1), &epp, s, pdl));
-    } else {
-      CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, G_ARGMAX128, 1), &ep, s, pdl));
-    }
-    // static batch: rows b0.. of the plan's [B, T+1] result; slot pool: row out_row[slot] of the [N, T+1] result
-    long long* oid = sm ? p.stream_out.as<long long>() : p.out_ids.as<long long>() + static_cast<size_t>(v.b0) * (T + 1);
-    int* olen = sm ? p.stream_len.as<int>() : p.out_len.as<int>() + v.b0;
-    if (p.score_on) {
-      // the result rows are indexed like the ids: b0.. of [B, T] (static batch), out_row[slot] of [N, T] (slot pool)
-      ScoreDev sd;
-      sd.psum = psum;
-      sd.fval = p.fval.as<float>() + v.b0;
-      sd.ftok = p.ftok.as<int>() + v.b0;
-      const size_t r0 = sm ? 0 : static_cast<size_t>(v.b0) * T;
-      if (p.score_on == 2) sd.forced = (sm ? p.stream_forced : p.forced).as<long long>() + r0;
-      sd.logprob = (sm ? p.stream_lp : p.score_lp).as<float>() + r0;
-      sd.logit = (sm ? p.stream_lg : p.score_lg).as<float>() + r0;
-      CU_OK(h, launch_kernel(p.proc_on ? finalize_step_score_kernel<true> : finalize_step_score_kernel<false>, dim3(v.nb), dim3(128),
-                             0, s, pdl, pval, pidx, p.n_vtiles, st, p.unfinished.as<int>() + v.b0, oid, olen, T + 1, eos, pad,
-                             h->shared.as<act_t>(), v.dx, d, p.live_extent.as<int>() + v.b0,
-                             sm ? p.pos.as<int>() + v.b0 : static_cast<int*>(nullptr),
-                             sm ? p.out_row.as<int>() + v.b0 : static_cast<const int*>(nullptr), T, pd, sd));
-    } else {
-      CU_OK(h, launch_kernel(p.proc_on ? finalize_step_kernel<true> : finalize_step_kernel<false>, dim3(v.nb), dim3(128), 0, s,
-                             pdl, pval, pidx, p.n_vtiles, st, p.unfinished.as<int>() + v.b0, oid, olen, T + 1, eos, pad,
-                             h->shared.as<act_t>(), v.dx, d, p.live_extent.as<int>() + v.b0,
-                             sm ? p.pos.as<int>() + v.b0 : static_cast<int*>(nullptr),
-                             sm ? p.out_row.as<int>() + v.b0 : static_cast<const int*>(nullptr), T, pd));
-    }
-    h->launches++;
+    return B200T5_OK;
   }
+  const bool sm = p.stream_mode;
+  const Plan::Results& r = p.res();
+  // result rows: b0.. of the static batch's, out_row[slot] of the slot pool's
+  const size_t r0 = sm ? 0 : static_cast<size_t>(v.b0);
+  LmHeadParams ep{};
+  ep.pval = p.pval.as<float>() + static_cast<size_t>(v.b0) * p.n_vtiles;
+  ep.pidx = p.pidx.as<int>() + static_cast<size_t>(v.b0) * p.n_vtiles;
+  ep.n_tiles = p.n_vtiles;
+  ep.step = sm ? p.pos.as<int>() + v.b0 : &p.state.as<DecodeState>()->step;
+  ep.eos = static_cast<int>(eos);
+  ep.min_new = min_new;
+  ep.step_stride = sm ? 1 : 0;
+  if (p.proc_on) ep.pd = p.proc.dev(v.b0);
+  FinalizeArgs fa{ep.pval, ep.pidx, p.n_vtiles, p.state.as<DecodeState>(), p.unfinished.as<int>() + v.b0,
+                  r.ids.as<long long>() + r0 * (T + 1), r.len.as<int>() + r0, T + 1, eos, pad, h->shared.as<act_t>(), v.dx, d,
+                  p.live_extent.as<int>() + v.b0, sm ? p.pos.as<int>() + v.b0 : nullptr, sm ? p.out_row.as<int>() + v.b0 : nullptr,
+                  T, ep.pd, ScoreDev()};
+  if (p.score_on) {
+    ep.psum = p.psum.as<float>() + static_cast<size_t>(v.b0) * p.n_vtiles;
+    ep.fval = p.fval.as<float>() + v.b0;
+    fa.sd = {ep.psum, ep.fval, p.ftok.as<int>() + v.b0, nullptr, r.lp.as<float>() + r0 * T, r.lg.as<float>() + r0 * T};
+    if (p.score_on == 2) {
+      ep.ftok = fa.sd.ftok;
+      fa.sd.forced = r.forced.as<long long>() + r0 * T;
+    }
+  }
+  CU_OK(h, run_lm_head(h, p.proc_on, p.score_on != 0, v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, ep, fa, s, pdl));
   return B200T5_OK;
 }
 
@@ -1694,15 +1697,15 @@ static int parse_score(b200t5_ctx* h, const b200t5_score_io* sc, long long rows,
   return B200T5_OK;
 }
 
-// Make the plan's scoring buffers fit this call (`rows` result rows: the batch, or the slot pool's capacity) and queue
-// the labels on `s`. A new allocation drops the step graph, which bakes the addresses.
+// Make the scoring buffers of the call's results (p.res(): the batch, or the slot pool at its capacity) fit this call
+// and queue the labels on `s`. A new allocation drops the step graph, which bakes the addresses.
 static int setup_score(b200t5_ctx* h, const ScoreHost& sh, cudaStream_t s) {
   Plan& p = *h->plan;
   p.score_on = sh.on ? (sh.forced.empty() ? 1 : 2) : 0;
   if (!sh.on) return B200T5_OK;
-  const bool sm = p.stream_mode;
-  const size_t rows = sm ? p.stream_cap : static_cast<size_t>(p.B), n = rows * p.Tmax;
-  if (!p.psum.p || (sm ? p.score_stream_cap != rows : !p.score_lp.p)) {
+  Plan::Results& r = p.res();
+  const size_t n = r.cap * p.Tmax;
+  if (!p.psum.p || !r.forced.p || r.forced.bytes != n * 8) {
     CU_OK(h, cudaStreamSynchronize(s));
     if (!p.psum.p) {
       CU_OK(h, p.psum.alloc(static_cast<size_t>(p.B) * p.n_vtiles * 4));
@@ -1710,14 +1713,12 @@ static int setup_score(b200t5_ctx* h, const ScoreHost& sh, cudaStream_t s) {
       CU_OK(h, p.ftok.alloc(static_cast<size_t>(p.B) * 4));
       CU_OK(h, cudaMemset(p.fval.p, 0, p.fval.bytes));
     }
-    CU_OK(h, (sm ? p.stream_lp : p.score_lp).alloc(n * 4));
-    CU_OK(h, (sm ? p.stream_lg : p.score_lg).alloc(n * 4));
-    CU_OK(h, (sm ? p.stream_forced : p.forced).alloc(n * 8));
-    if (sm) p.score_stream_cap = rows;
+    CU_OK(h, r.lp.alloc(n * 4));
+    CU_OK(h, r.lg.alloc(n * 4));
+    CU_OK(h, r.forced.alloc(n * 8));
     p.g_score = -1;
   }
-  if (p.score_on == 2)
-    CU_OK(h, cudaMemcpyAsync((sm ? p.stream_forced : p.forced).p, sh.forced.data(), sh.forced.size() * 8, cudaMemcpyHostToDevice, s));
+  if (p.score_on == 2) CU_OK(h, cudaMemcpyAsync(r.forced.p, sh.forced.data(), sh.forced.size() * 8, cudaMemcpyHostToDevice, s));
   return B200T5_OK;
 }
 
@@ -1745,40 +1746,79 @@ static void fill_stats_model(b200t5_ctx* h, int steps) {
                       2.0 * c.Ld * 2.0 * c.d * c.I * sum_s;
 }
 
-static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* mask, int B, int S,
-                         const b200t5_gen_params* gp, const ProcHost& ph, const ScoreHost& sh, long long* out_ids, int* out_len,
-                         cudaStream_t s) {
+// A generate call's arguments after set_up_call: the special tokens and sizes every path resolves from them, the logits
+// processors and the scoring request.
+struct CallArgs {
+  long long eos = 0, pad = 0, start = 0;
+  int T = 0, min_new = 0;
+  ProcHost ph;
+  ScoreHost sh;
+};
+
+// Checks a call of B rows (the slot pool: B slots) for `rows` prompts and resolves what it asks for. `host`: the pointers
+// in `score` are host pointers.
+static int set_up_call(b200t5_ctx* h, int B, int S, long long rows, const b200t5_gen_params* gp, const void* input_ids,
+                       const void* out_ids, const void* out_len, const b200t5_logits_params* logits,
+                       const b200t5_score_io* score, bool host, CallArgs* a) {
+  TRY(validate(h, B, S, gp));
+  if (!gp || !input_ids || !out_ids || !out_len) return fail(h, B200T5_EINVAL, "null argument");
   const Cfg& c = h->c;
-  const long long eos = gp->eos_token_id >= 0 ? gp->eos_token_id : c.eos;
-  const long long pad = gp->pad_token_id >= 0 ? gp->pad_token_id : c.pad;
-  const long long start = gp->decoder_start_token_id >= 0 ? gp->decoder_start_token_id : c.start;
-  if (start >= c.V || pad >= c.V) return fail(h, B200T5_EINVAL, "special token id out of range");
-  const int T = gp->max_new_tokens;
-  const int min_new = gp->min_new_tokens > 0 ? gp->min_new_tokens : 0;
+  a->eos = gp->eos_token_id >= 0 ? gp->eos_token_id : c.eos;
+  a->pad = gp->pad_token_id >= 0 ? gp->pad_token_id : c.pad;
+  a->start = gp->decoder_start_token_id >= 0 ? gp->decoder_start_token_id : c.start;
+  a->T = gp->max_new_tokens;
+  a->min_new = gp->min_new_tokens > 0 ? gp->min_new_tokens : 0;
+  TRY(parse_logits_params(h, c.V, logits, a->eos, &a->ph));
+  CU_OK(h, cudaSetDevice(h->device));
+  TRY(parse_score(h, score, rows, a->T, host, a->ph.on, &a->sh));
+  if (a->start >= c.V || a->pad >= c.V) return fail(h, B200T5_EINVAL, "special token id out of range");
+  return B200T5_OK;
+}
+
+// Queues the copy of the first n rows of the call's results (p.res()) to ids / len and, for a scored call, to lp / lg
+// (lg may be NULL).
+static int copy_results(b200t5_ctx* h, size_t n, void* ids, void* len, void* lp, void* lg, cudaMemcpyKind kind, cudaStream_t s) {
+  Plan& p = *h->plan;
+  const Plan::Results& r = p.res();
+  const size_t T = static_cast<size_t>(p.Tmax);
+  CU_OK(h, cudaMemcpyAsync(ids, r.ids.p, n * (T + 1) * 8, kind, s));
+  CU_OK(h, cudaMemcpyAsync(len, r.len.p, n * 4, kind, s));
+  if (p.score_on) {
+    CU_OK(h, cudaMemcpyAsync(lp, r.lp.p, n * T * 4, kind, s));
+    if (lg) CU_OK(h, cudaMemcpyAsync(lg, r.lg.p, n * T * 4, kind, s));
+  }
+  return B200T5_OK;
+}
+
+// A static batch of B rows; its results stay in the plan's buffers (copy_results).
+static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* mask, int B, int S, const b200t5_gen_params* gp,
+                         const CallArgs& a, cudaStream_t s) {
+  const Cfg& c = h->c;
+  const int T = a.T;
   const int poll = gp->poll_interval > 0 ? gp->poll_interval : 8;
   TRY(ensure_plan(h, B, S, T));
   Plan& p = *h->plan;
   p.stream_mode = false;
-  TRY(setup_proc(h, ph, s));
-  TRY(setup_score(h, sh, s));
+  TRY(setup_proc(h, a.ph, s));
+  TRY(setup_score(h, a.sh, s));
   h->launches = 0;
   CU_OK(h, cudaEventRecord(h->ev[0], s));
   TRY(run_encoder(h, ids, mask, s));
   TRY(run_cross_kv(h, s));
   // (host-side capture, only when something baked into the graph changed; the GPU is busy with the encoder meanwhile)
-  TRY(ensure_graph(h, eos, pad, min_new, static_cast<double>(p.rows_valid) / (static_cast<double>(B) * S)));
+  TRY(ensure_graph(h, a.eos, a.pad, a.min_new, static_cast<double>(p.rows_valid) / (static_cast<double>(B) * S)));
   CU_OK(h, cudaMemcpyAsync(p.live_extent.p, p.extent.p, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToDevice, s));
   CU_OK(h, cudaMemcpyAsync(p.live_key_ok.p, p.key_ok.p, static_cast<size_t>(B) * S, cudaMemcpyDeviceToDevice, s));
-  decode_init_kernel<<<B, 128, 0, s>>>(p.state.as<DecodeState>(), p.unfinished.as<int>(), p.out_ids.as<long long>(),
-                                       p.out_len.as<int>(), T + 1, B, start, pad, h->shared.as<act_t>(), p.dx.as<res_t>(), c.d);
+  decode_init_kernel<<<B, 128, 0, s>>>(p.state.as<DecodeState>(), p.unfinished.as<int>(), p.batch.ids.as<long long>(),
+                                       p.batch.len.as<int>(), T + 1, B, a.start, a.pad, h->shared.as<act_t>(), p.dx.as<res_t>(), c.d);
   h->launches++;
   if (p.proc_on) {
-    proc_reset_kernel<<<B, 128, 0, s>>>(p.proc.dev(), nullptr, ids, p.out_ids.as<long long>(), T + 1, nullptr, 1);
+    proc_reset_kernel<<<B, 128, 0, s>>>(p.proc.dev(), nullptr, ids, p.batch.ids.as<long long>(), T + 1, nullptr, 1);
     h->launches++;
   }
   if (p.score_on) {
-    score_reset_kernel<<<B, 128, 0, s>>>(p.score_lp.as<float>(), p.score_lg.as<float>(), static_cast<size_t>(B) * T, p.ftok.as<int>(), B,
-                                         nullptr, nullptr, p.score_on == 2 ? p.forced.as<long long>() : nullptr, T);
+    score_reset_kernel<<<B, 128, 0, s>>>(p.batch.lp.as<float>(), p.batch.lg.as<float>(), static_cast<size_t>(B) * T, p.ftok.as<int>(),
+                                         B, nullptr, nullptr, p.score_on == 2 ? p.batch.forced.as<long long>() : nullptr, T);
     h->launches++;
   }
   CU_OK(h, cudaGetLastError());
@@ -1796,7 +1836,7 @@ static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* m
       h->launches += p.graph_nodes;
       ++steps;
     }
-    if ((t + 1) % poll == 0 && t + 1 < T && min_new < T) {
+    if ((t + 1) % poll == 0 && t + 1 < T && a.min_new < T) {
       // every row emitted EOS -> the remaining steps would only append pad tokens
       CU_OK(h, cudaMemcpyAsync(p.h_state, p.state.p, sizeof(DecodeState), cudaMemcpyDeviceToHost, s));
       CU_OK(h, cudaStreamSynchronize(s));
@@ -1804,37 +1844,21 @@ static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* m
     }
   }
   CU_OK(h, cudaEventRecord(h->ev[2], s));
-  CU_OK(h, cudaMemcpyAsync(out_ids, p.out_ids.p, static_cast<size_t>(B) * (T + 1) * 8, cudaMemcpyDeviceToDevice, s));
-  CU_OK(h, cudaMemcpyAsync(out_len, p.out_len.p, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToDevice, s));
-  if (p.score_on) {
-    CU_OK(h, cudaMemcpyAsync(sh.lp, p.score_lp.p, static_cast<size_t>(B) * T * 4, cudaMemcpyDeviceToDevice, s));
-    if (sh.lg) CU_OK(h, cudaMemcpyAsync(sh.lg, p.score_lg.p, static_cast<size_t>(B) * T * 4, cudaMemcpyDeviceToDevice, s));
-  }
   h->last_steps = steps;
   h->ev_valid = true;
   return B200T5_OK;
 }
 
-static long long call_eos(const b200t5_ctx* h, const b200t5_gen_params* gp) {
-  return gp->eos_token_id >= 0 ? gp->eos_token_id : h->c.eos;
-}
-
 extern "C" int b200t5_generate_scored(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
                                       const b200t5_gen_params* params, const b200t5_logits_params* logits, int64_t* out_ids,
                                       int32_t* out_len, const b200t5_score_io* score, void* stream) {
-  TRY(validate(h, B, S, params));
-  if (!params || !input_ids || !out_ids || !out_len) return fail(h, B200T5_EINVAL, "null argument");
-  ProcHost ph;
-  TRY(parse_logits_params(h, h->c.V, logits, call_eos(h, params), &ph));
-  CU_OK(h, cudaSetDevice(h->device));
-  ScoreHost sh;
-  TRY(parse_score(h, score, B, params->max_new_tokens, false, ph.on, &sh));
-  if (sh.on) {
-    sh.lp = score->token_logprobs;
-    sh.lg = score->token_logits;
-  }
-  return generate_impl(h, reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(attention_mask),
-                       B, S, params, ph, sh, reinterpret_cast<long long*>(out_ids), out_len, static_cast<cudaStream_t>(stream));
+  CallArgs a;
+  TRY(set_up_call(h, B, S, B, params, input_ids, out_ids, out_len, logits, score, false, &a));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  TRY(generate_impl(h, reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(attention_mask), B, S,
+                    params, a, s));
+  return copy_results(h, static_cast<size_t>(B), out_ids, out_len, a.sh.on ? score->token_logprobs : nullptr,
+                      a.sh.on ? score->token_logits : nullptr, cudaMemcpyDeviceToDevice, s);
 }
 
 extern "C" int b200t5_generate_ex(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
@@ -1862,14 +1886,9 @@ extern "C" int b200t5_generate_host_ex(b200t5_handle h, const int64_t* input_ids
 extern "C" int b200t5_generate_host_scored(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B,
                                            int S, const b200t5_gen_params* params, const b200t5_logits_params* logits,
                                            int64_t* out_ids, int32_t* out_len, const b200t5_score_io* score) {
-  TRY(validate(h, B, S, params));
-  if (!params || !input_ids || !out_ids || !out_len) return fail(h, B200T5_EINVAL, "null argument");
-  ProcHost ph;
-  TRY(parse_logits_params(h, h->c.V, logits, call_eos(h, params), &ph));
-  CU_OK(h, cudaSetDevice(h->device));
-  ScoreHost sh;
-  TRY(parse_score(h, score, B, params->max_new_tokens, true, ph.on, &sh));
-  TRY(ensure_plan(h, B, S, params->max_new_tokens));
+  CallArgs a;
+  TRY(set_up_call(h, B, S, B, params, input_ids, out_ids, out_len, logits, score, true, &a));
+  TRY(ensure_plan(h, B, S, a.T));
   Plan& p = *h->plan;
   cudaStream_t s = h->exec_stream;
   const size_t nb = static_cast<size_t>(B) * S * 8;
@@ -1879,31 +1898,12 @@ extern "C" int b200t5_generate_host_scored(b200t5_handle h, const int64_t* input
     memcpy(p.h_mask, attention_mask, nb);
     CU_OK(h, cudaMemcpyAsync(p.mask_dev.p, p.h_mask, nb, cudaMemcpyHostToDevice, s));
   }
-  // results land in the plan's own buffers; copy them out through pinned staging
-  DevBuf tmp_ids, tmp_len;
-  const int T = params->max_new_tokens;
-  CU_OK(h, tmp_ids.alloc(static_cast<size_t>(B) * (T + 1) * 8));
-  CU_OK(h, tmp_len.alloc(static_cast<size_t>(B) * 4));
-  DevBuf tmp_lp, tmp_lg;
-  const size_t score_bytes = static_cast<size_t>(B) * T * 4;
-  if (sh.on) {
-    CU_OK(h, tmp_lp.alloc(score_bytes));
-    sh.lp = tmp_lp.as<float>();
-    if (score->token_logits) {
-      CU_OK(h, tmp_lg.alloc(score_bytes));
-      sh.lg = tmp_lg.as<float>();
-    }
-  }
-  TRY(generate_impl(h, p.ids_dev.as<long long>(), attention_mask ? p.mask_dev.as<long long>() : nullptr, B, S, params,
-                    ph, sh, tmp_ids.as<long long>(), tmp_len.as<int>(), s));
-  if (sh.on) {
-    CU_OK(h, cudaMemcpyAsync(score->token_logprobs, tmp_lp.p, score_bytes, cudaMemcpyDeviceToHost, s));
-    if (sh.lg) CU_OK(h, cudaMemcpyAsync(score->token_logits, tmp_lg.p, score_bytes, cudaMemcpyDeviceToHost, s));
-  }
-  CU_OK(h, cudaMemcpyAsync(p.h_out, tmp_ids.p, static_cast<size_t>(B) * (T + 1) * 8, cudaMemcpyDeviceToHost, s));
-  CU_OK(h, cudaMemcpyAsync(p.h_len, tmp_len.p, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToHost, s));
+  TRY(generate_impl(h, p.ids_dev.as<long long>(), attention_mask ? p.mask_dev.as<long long>() : nullptr, B, S, params, a, s));
+  // ids and lengths through the pinned staging
+  TRY(copy_results(h, static_cast<size_t>(B), p.h_out, p.h_len, a.sh.on ? score->token_logprobs : nullptr,
+                   a.sh.on ? score->token_logits : nullptr, cudaMemcpyDeviceToHost, s));
   CU_OK(h, cudaStreamSynchronize(s));
-  memcpy(out_ids, p.h_out, static_cast<size_t>(B) * (T + 1) * 8);
+  memcpy(out_ids, p.h_out, static_cast<size_t>(B) * (a.T + 1) * 8);
   memcpy(out_len, p.h_len, static_cast<size_t>(B) * 4);
   return B200T5_OK;
 }
@@ -1932,43 +1932,33 @@ extern "C" int b200t5_generate_stream_ex(b200t5_handle h, const int64_t* input_i
 extern "C" int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int64_t N,
                                              int S, const b200t5_gen_params* gp, const b200t5_logits_params* logits, int pool,
                                              int admit_min, int64_t* out_ids, int32_t* out_len, const b200t5_score_io* score) {
-  if (!h) return fail(nullptr, B200T5_EINVAL, "null handle");
-  if (!gp || !input_ids || !out_ids || !out_len) return fail(h, B200T5_EINVAL, "null argument");
-  ProcHost ph;
-  TRY(parse_logits_params(h, h->c.V, logits, call_eos(h, gp), &ph));
   if (N < 1 || N > (1ll << 30)) return fail(h, B200T5_EINVAL, "bad prompt count N=%lld", static_cast<long long>(N));
   if (pool < 1) pool = 256;
   if (pool > N) pool = static_cast<int>(N);
-  TRY(validate(h, pool, S, gp));
-  ScoreHost sh;
-  TRY(parse_score(h, score, N, gp->max_new_tokens, true, ph.on, &sh));
-  CU_OK(h, cudaSetDevice(h->device));
+  CallArgs a;
+  TRY(set_up_call(h, pool, S, N, gp, input_ids, out_ids, out_len, logits, score, true, &a));
   const Cfg& c = h->c;
-  const long long eos = gp->eos_token_id >= 0 ? gp->eos_token_id : c.eos;
-  const long long pad = gp->pad_token_id >= 0 ? gp->pad_token_id : c.pad;
-  const long long start = gp->decoder_start_token_id >= 0 ? gp->decoder_start_token_id : c.start;
-  if (start >= c.V || pad >= c.V) return fail(h, B200T5_EINVAL, "special token id out of range");
-  const int T = gp->max_new_tokens;
-  const int min_new = gp->min_new_tokens > 0 ? gp->min_new_tokens : 0;
+  const int T = a.T;
   const int B = pool;
   if (admit_min < 1) admit_min = B >= 8 ? B / 8 : 1;
   const int poll = gp->poll_interval > 0 ? (gp->poll_interval > 64 ? 64 : gp->poll_interval) : kStepsPerGraph;
   TRY(ensure_plan(h, B, S, T));
   Plan& p = *h->plan;
   cudaStream_t s = h->exec_stream;
-  if (p.stream_cap < static_cast<size_t>(N)) {
+  Plan::Results& r = p.pool;
+  if (r.cap < static_cast<size_t>(N)) {
     // the step graph bakes the result addresses: a larger result buffer means a new graph
     CU_OK(h, cudaStreamSynchronize(s));
-    size_t cap = p.stream_cap ? p.stream_cap : 1024;
+    size_t cap = r.cap ? r.cap : 1024;
     while (cap < static_cast<size_t>(N)) cap *= 2;
-    CU_OK(h, p.stream_out.alloc(cap * (T + 1) * 8));
-    CU_OK(h, p.stream_len.alloc(cap * 4));
-    p.stream_cap = cap;
+    CU_OK(h, r.ids.alloc(cap * (T + 1) * 8));
+    CU_OK(h, r.len.alloc(cap * 4));
+    r.cap = cap;
     p.g_stream = -1;
   }
   p.stream_mode = true;
-  TRY(setup_proc(h, ph, s));
-  TRY(setup_score(h, sh, s));
+  TRY(setup_proc(h, a.ph, s));
+  TRY(setup_score(h, a.sh, s));
   double fill = 1.0;
   if (attention_mask) {  // fill of the first prompts (up to four pools' worth): picks the cross-attention kernel
     const long long rows = N < 4LL * B ? N : 4LL * B;
@@ -1976,18 +1966,18 @@ extern "C" int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* inp
     for (long long i = 0; i < rows * S; ++i) ones += attention_mask[i] != 0;
     fill = static_cast<double>(ones) / static_cast<double>(rows * S);
   }
-  TRY(ensure_graph(h, eos, pad, min_new, fill));
+  TRY(ensure_graph(h, a.eos, a.pad, a.min_new, fill));
   h->launches = 0;
   CU_OK(h, cudaEventRecord(h->ev[0], s));
   {
     const long long rows = N > B ? N : B;
     stream_init_kernel<<<static_cast<unsigned>(rows), 128, 0, s>>>(p.state.as<DecodeState>(), p.unfinished.as<int>(), p.pos.as<int>(),
-                                                                  p.live_extent.as<int>(), p.stream_out.as<long long>(),
-                                                                  p.stream_len.as<int>(), T + 1, static_cast<int>(N), B, start, pad,
+                                                                  p.live_extent.as<int>(), r.ids.as<long long>(),
+                                                                  r.len.as<int>(), T + 1, static_cast<int>(N), B, a.start, a.pad,
                                                                   h->shared.as<act_t>(), p.dx.as<res_t>(), c.d);
     h->launches++;
     if (p.score_on) {  // every result position 0, no slot forced until it is admitted
-      score_reset_kernel<<<1024, 128, 0, s>>>(p.stream_lp.as<float>(), p.stream_lg.as<float>(), static_cast<size_t>(N) * T,
+      score_reset_kernel<<<1024, 128, 0, s>>>(r.lp.as<float>(), r.lg.as<float>(), static_cast<size_t>(N) * T,
                                               p.ftok.as<int>(), B, nullptr, nullptr, nullptr, T);
       h->launches++;
     }
@@ -2013,17 +2003,17 @@ extern "C" int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* inp
   auto admit_now = [&](int k) -> int {
     admit_slots_kernel<<<k, 128, 0, s>>>(p.admit.as<int>() + B, p.admit.as<int>() + 2 * B, p.unfinished.as<int>(), p.pos.as<int>(),
                                          p.out_row.as<int>(), p.extent.as<int>(), p.live_extent.as<int>(),
-                                         p.key_ok.as<unsigned char>(), p.live_key_ok.as<unsigned char>(), S, start,
+                                         p.key_ok.as<unsigned char>(), p.live_key_ok.as<unsigned char>(), S, a.start,
                                          h->shared.as<act_t>(), p.dx.as<res_t>(), c.d);
     h->launches++;
     if (p.proc_on) {  // the admitted slots' processor state, from their prompts (still in ids_dev) and start token
       proc_reset_kernel<<<k, 128, 0, s>>>(p.proc.dev(), p.admit.as<int>() + B, p.ids_dev.as<long long>(),
-                                          p.stream_out.as<long long>(), T + 1, p.out_row.as<int>(), 1);
+                                          r.ids.as<long long>(), T + 1, p.out_row.as<int>(), 1);
       h->launches++;
     }
     if (p.score_on == 2) {  // the admitted slots' first labels
       score_reset_kernel<<<(k + 127) / 128, 128, 0, s>>>(nullptr, nullptr, 0, p.ftok.as<int>(), k, p.admit.as<int>() + B,
-                                                         p.admit.as<int>() + 2 * B, p.stream_forced.as<long long>(), T);
+                                                         p.admit.as<int>() + 2 * B, r.forced.as<long long>(), T);
       h->launches++;
     }
     CU_OK(h, cudaGetLastError());
@@ -2110,13 +2100,8 @@ extern "C" int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* inp
     }
   }
   CU_OK(h, cudaEventRecord(h->ev[2], s));
-  CU_OK(h, cudaMemcpyAsync(out_ids, p.stream_out.p, static_cast<size_t>(N) * (T + 1) * 8, cudaMemcpyDeviceToHost, s));
-  CU_OK(h, cudaMemcpyAsync(out_len, p.stream_len.p, static_cast<size_t>(N) * 4, cudaMemcpyDeviceToHost, s));
-  if (p.score_on) {
-    CU_OK(h, cudaMemcpyAsync(score->token_logprobs, p.stream_lp.p, static_cast<size_t>(N) * T * 4, cudaMemcpyDeviceToHost, s));
-    if (score->token_logits)
-      CU_OK(h, cudaMemcpyAsync(score->token_logits, p.stream_lg.p, static_cast<size_t>(N) * T * 4, cudaMemcpyDeviceToHost, s));
-  }
+  TRY(copy_results(h, static_cast<size_t>(N), out_ids, out_len, a.sh.on ? score->token_logprobs : nullptr,
+                   a.sh.on ? score->token_logits : nullptr, cudaMemcpyDeviceToHost, s));
   CU_OK(h, cudaStreamSynchronize(s));
   h->last_steps = steps;
   h->last_decode_bytes = 0;  // not modelled for a pool whose occupancy varies
@@ -2423,132 +2408,50 @@ extern "C" int b200t5_test_enc_gemm(int device, const void* A, const void* W, vo
 #endif
 }
 
-// lm_head + fused arg-max + greedy bookkeeping exactly as chain_head launches them (EpiArgmax partials per 128-column
-// tile, finalize_step_kernel's lowest-index reduction). W doubles as the embedding table of the gather.
-extern "C" int b200t5_test_lm_argmax(int device, const void* x, const void* W, int M, int V, int K, int step, int eos,
-                                     int min_new, int64_t* tokens, void* stream) {
+// lm_head + the decode step's head exactly as chain_head launches it, for M rows at position `step`: the head with
+// processors when `proc` or `logits` has an active processor (the row state built by proc_reset_kernel from the
+// decoder ids hist [M, step+1] and the prompts enc_ids [M, S]), scored when `score` (teacher-forced when `forced`
+// holds each row's label). W doubles as the embedding table of the gather. `vals`: the columns' values, not written
+// by the plain head.
+static int test_lm_head(const char* name, int device, const void* x, const void* W, int M, int V, int K, int step, int eos,
+                        int min_new, const b200t5_logits_params* logits, bool proc, const int64_t* hist, const int64_t* enc_ids,
+                        int S, bool score, const int64_t* forced, int64_t* tokens, float* logprob, float* logit, float* vals,
+                        void* stream) {
   const int sms = hook_device(device);
   if (sms < 0) return sms;
-  if (!x || !W || !tokens || M < 1 || V < 2 || K % 8 || step < 0) return fail(nullptr, B200T5_EINVAL, "test_lm_argmax: bad argument");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  CUtensorMap ta, tb;
-  if (!make_tmap(&ta, x, M, K, 128) || !make_tmap(&tb, W, V, K, 128)) return fail(nullptr, B200T5_ECUDA, "%s", g_err);
-  const int n_tiles = (V + 127) / 128, out_ld = step + 2;
-  DevBuf pval, pidx, st, unf, out, len, xn, ext;
-  if (pval.alloc(static_cast<size_t>(M) * n_tiles * 4) != cudaSuccess || pidx.alloc(static_cast<size_t>(M) * n_tiles * 4) != cudaSuccess ||
-      st.alloc(sizeof(DecodeState)) != cudaSuccess || unf.alloc(static_cast<size_t>(M) * 4) != cudaSuccess ||
-      out.alloc(static_cast<size_t>(M) * out_ld * 8) != cudaSuccess || len.alloc(static_cast<size_t>(M) * 4) != cudaSuccess ||
-      xn.alloc(static_cast<size_t>(M) * K * sizeof(res_t)) != cudaSuccess || ext.alloc(static_cast<size_t>(M) * 4) != cudaSuccess)
-    return fail(nullptr, B200T5_ENOMEM, "test_lm_argmax: allocation failed");
-  b200t5_ctx dummy;
-  dummy.num_sms = sms;
-  decode_init_kernel<<<M, 128, 0, s>>>(st.as<DecodeState>(), unf.as<int>(), out.as<long long>(), len.as<int>(), out_ld, M, 0, 0,
-                                       static_cast<const act_t*>(W), xn.as<res_t>(), K);
-  set_state_kernel<<<1, 1, 0, s>>>(st.as<DecodeState>(), step);
-  EpiArgmax::Params ep{pval.as<float>(), pidx.as<int>(), n_tiles, &st.as<DecodeState>()->step, eos, min_new, 0};
-  cudaError_t e = run_gemm(&dummy, mk(ta, tb, M, V, K, G_ARGMAX128, 1), &ep, s, false);
-  if (e == cudaSuccess)
-    e = launch_kernel(finalize_step_kernel<false>, dim3(M), dim3(128), 0, s, false, pval.as<float>(), pidx.as<int>(), n_tiles, st.as<DecodeState>(),
-                      unf.as<int>(), out.as<long long>(), len.as<int>(), out_ld, static_cast<long long>(-1), static_cast<long long>(0),
-                      static_cast<const act_t*>(W), xn.as<res_t>(), K, ext.as<int>(), static_cast<int*>(nullptr),
-                      static_cast<const int*>(nullptr), 1 << 30, ProcDev());
-  if (e == cudaSuccess)
-    e = cudaMemcpy2DAsync(tokens, 8, out.as<long long>() + step + 1, static_cast<size_t>(out_ld) * 8, 8, M, cudaMemcpyDeviceToDevice, s);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_lm_argmax: %s", cudaGetErrorString(e));
-  return B200T5_OK;
-}
-
-// lm_head + logits processors + arg-max exactly as chain_head launches them with processors on: the row state is
-// built by proc_reset_kernel from the given history and prompts, then EpiArgmaxProc and finalize_step_kernel<true>.
-extern "C" int b200t5_test_lm_process(int device, const void* x, const void* W, int M, int V, int K, int step, int eos,
-                                      int min_new, const b200t5_logits_params* logits, const int64_t* hist,
-                                      const int64_t* enc_ids, int S, int64_t* tokens, float* vals, void* stream) {
-  const int sms = hook_device(device);
-  if (sms < 0) return sms;
-  if (!x || !W || !tokens || !hist || !enc_ids || M < 1 || V < 2 || K % 8 || step < 0 || S < 1)
-    return fail(nullptr, B200T5_EINVAL, "test_lm_process: bad argument");
+  if (!x || !W || !tokens || M < 1 || V < 2 || K % 8 || step < 0 || (proc && (!hist || !enc_ids || S < 1)) ||
+      (score && (!logprob || !logit)))
+    return fail(nullptr, B200T5_EINVAL, "%s: bad argument", name);
   ProcHost ph;
   int rc = parse_logits_params(nullptr, V, logits, eos, &ph);
   if (rc != B200T5_OK) return rc;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  CUtensorMap ta, tb;
-  if (!make_tmap(&ta, x, M, K, 128) || !make_tmap(&tb, W, V, K, 128)) return fail(nullptr, B200T5_ECUDA, "%s", g_err);
-  const int n_tiles = (V + 127) / 128, out_ld = step + 2, Wd = (V + 31) / 32;
-  DevBuf pval, pidx, st, unf, out, len, xn, ext;
-  ProcBufs pb;
-  if (pval.alloc(static_cast<size_t>(M) * n_tiles * 4) != cudaSuccess || pidx.alloc(static_cast<size_t>(M) * n_tiles * 4) != cudaSuccess ||
-      st.alloc(sizeof(DecodeState)) != cudaSuccess || unf.alloc(static_cast<size_t>(M) * 4) != cudaSuccess ||
-      out.alloc(static_cast<size_t>(M) * out_ld * 8) != cudaSuccess || len.alloc(static_cast<size_t>(M) * 4) != cudaSuccess ||
-      xn.alloc(static_cast<size_t>(M) * K * sizeof(res_t)) != cudaSuccess || ext.alloc(static_cast<size_t>(M) * 4) != cudaSuccess ||
-      pb.alloc(M, S, Wd, std::min(Wd * 32, step + 2 + S + ph.cfg.n_bad), ph.bad_ids.size(), ph.bad_off.size()) != cudaSuccess)
-    return fail(nullptr, B200T5_ENOMEM, "test_lm_process: allocation failed");
-  b200t5_ctx dummy;
-  dummy.num_sms = sms;
-  decode_init_kernel<<<M, 128, 0, s>>>(st.as<DecodeState>(), unf.as<int>(), out.as<long long>(), len.as<int>(), out_ld, M, 0, 0,
-                                       static_cast<const act_t*>(W), xn.as<res_t>(), K);
-  cudaError_t e = cudaMemcpy2DAsync(out.p, static_cast<size_t>(out_ld) * 8, hist, static_cast<size_t>(step + 1) * 8,
-                                    static_cast<size_t>(step + 1) * 8, M, cudaMemcpyDeviceToDevice, s);
-  if (e == cudaSuccess) e = pb.upload(ph, s);
-  if (e == cudaSuccess) {
-    set_state_kernel<<<1, 1, 0, s>>>(st.as<DecodeState>(), step);
-    proc_reset_kernel<<<M, 128, 0, s>>>(pb.dev(), nullptr, reinterpret_cast<const long long*>(enc_ids), out.as<long long>(),
-                                        out_ld, nullptr, step + 1);
-    e = cudaGetLastError();
-  }
-  const ProcDev pd = pb.dev();
-  EpiArgmaxProc::Params ep{{pval.as<float>(), pidx.as<int>(), n_tiles, &st.as<DecodeState>()->step, eos, min_new, 0}, pd, vals, V};
-  if (e == cudaSuccess) e = run_gemm(&dummy, mk(ta, tb, M, V, K, G_ARGMAXPROC128, 1), &ep, s, false);
-  if (e == cudaSuccess)
-    e = launch_kernel(finalize_step_kernel<true>, dim3(M), dim3(128), 0, s, false, pval.as<float>(), pidx.as<int>(), n_tiles, st.as<DecodeState>(),
-                      unf.as<int>(), out.as<long long>(), len.as<int>(), out_ld, static_cast<long long>(-1), static_cast<long long>(0),
-                      static_cast<const act_t*>(W), xn.as<res_t>(), K, ext.as<int>(), static_cast<int*>(nullptr),
-                      static_cast<const int*>(nullptr), 1 << 30, pd);
-  if (e == cudaSuccess)
-    e = cudaMemcpy2DAsync(tokens, 8, out.as<long long>() + step + 1, static_cast<size_t>(out_ld) * 8, 8, M, cudaMemcpyDeviceToDevice, s);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_lm_process: %s", cudaGetErrorString(e));
-  return B200T5_OK;
-}
-
-// lm_head + arg-max + log-sum-exp partials + their merge as chain_head launches them for a scored call (EpiScore ->
-// finalize_step_score_kernel), with the row state of b200t5_test_lm_process when `logits` has an active processor.
-extern "C" int b200t5_test_lm_score(int device, const void* x, const void* W, int M, int V, int K, int step, int eos,
-                                    int min_new, const b200t5_logits_params* logits, const int64_t* hist,
-                                    const int64_t* enc_ids, int S, const int64_t* forced, int64_t* tokens, float* logprob,
-                                    float* logit, float* vals, void* stream) {
-  const int sms = hook_device(device);
-  if (sms < 0) return sms;
-  if (!x || !W || !tokens || !logprob || !logit || M < 1 || V < 2 || K % 8 || step < 0)
-    return fail(nullptr, B200T5_EINVAL, "test_lm_score: bad argument");
-  ProcHost ph;
-  int rc = parse_logits_params(nullptr, V, logits, eos, &ph);
-  if (rc != B200T5_OK) return rc;
-  if (ph.on && (!hist || !enc_ids || S < 1)) return fail(nullptr, B200T5_EINVAL, "test_lm_score: processors need hist and enc_ids");
+  proc = proc || ph.on;
+  if (proc && (!hist || !enc_ids || S < 1)) return fail(nullptr, B200T5_EINVAL, "%s: processors need hist and enc_ids", name);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CUtensorMap ta, tb;
   if (!make_tmap(&ta, x, M, K, 128) || !make_tmap(&tb, W, V, K, 128)) return fail(nullptr, B200T5_ECUDA, "%s", g_err);
   // result arrays [M, T] with T = step + 1 columns (+ 1 when forced: a further label keeps the row going)
   const int n_tiles = (V + 127) / 128, T = step + 1, out_ld = T + 1, Wd = (V + 31) / 32;
-  DevBuf pval, pidx, psum, fval, ftok, fids, lp, lg, st, unf, out, len, xn, ext;
+  const size_t mt = static_cast<size_t>(M) * n_tiles * 4, m4 = static_cast<size_t>(M) * 4;
+  DevBuf pval, pidx, st, unf, out, len, xn, ext, psum, fval, ftok, fids, lp, lg;
   ProcBufs pb;
-  const size_t mt = static_cast<size_t>(M) * n_tiles * 4;
-  if (pval.alloc(mt) != cudaSuccess || pidx.alloc(mt) != cudaSuccess || psum.alloc(mt) != cudaSuccess ||
-      fval.alloc(static_cast<size_t>(M) * 4) != cudaSuccess || ftok.alloc(static_cast<size_t>(M) * 4) != cudaSuccess ||
-      fids.alloc(static_cast<size_t>(M) * T * 8) != cudaSuccess || lp.alloc(static_cast<size_t>(M) * T * 4) != cudaSuccess ||
-      lg.alloc(static_cast<size_t>(M) * T * 4) != cudaSuccess || st.alloc(sizeof(DecodeState)) != cudaSuccess ||
-      unf.alloc(static_cast<size_t>(M) * 4) != cudaSuccess || out.alloc(static_cast<size_t>(M) * out_ld * 8) != cudaSuccess ||
-      len.alloc(static_cast<size_t>(M) * 4) != cudaSuccess || xn.alloc(static_cast<size_t>(M) * K * sizeof(res_t)) != cudaSuccess ||
-      ext.alloc(static_cast<size_t>(M) * 4) != cudaSuccess ||
-      (ph.on && pb.alloc(M, S, Wd, std::min(Wd * 32, step + 2 + S + ph.cfg.n_bad), ph.bad_ids.size(), ph.bad_off.size()) != cudaSuccess))
-    return fail(nullptr, B200T5_ENOMEM, "test_lm_score: allocation failed");
+  bool ok = pval.alloc(mt) == cudaSuccess && pidx.alloc(mt) == cudaSuccess && st.alloc(sizeof(DecodeState)) == cudaSuccess &&
+            unf.alloc(m4) == cudaSuccess && out.alloc(static_cast<size_t>(M) * out_ld * 8) == cudaSuccess && len.alloc(m4) == cudaSuccess &&
+            xn.alloc(static_cast<size_t>(M) * K * sizeof(res_t)) == cudaSuccess && ext.alloc(m4) == cudaSuccess;
+  if (ok && proc)
+    ok = pb.alloc(M, S, Wd, std::min(Wd * 32, step + 2 + S + ph.cfg.n_bad), ph.bad_ids.size(), ph.bad_off.size()) == cudaSuccess;
+  if (ok && score)
+    ok = psum.alloc(mt) == cudaSuccess && fval.alloc(m4) == cudaSuccess && ftok.alloc(m4) == cudaSuccess &&
+         lp.alloc(static_cast<size_t>(M) * T * 4) == cudaSuccess && lg.alloc(static_cast<size_t>(M) * T * 4) == cudaSuccess;
+  if (ok && score && forced) ok = fids.alloc(static_cast<size_t>(M) * T * 8) == cudaSuccess;
+  if (!ok) return fail(nullptr, B200T5_ENOMEM, "%s: allocation failed", name);
   b200t5_ctx dummy;
   dummy.num_sms = sms;
   decode_init_kernel<<<M, 128, 0, s>>>(st.as<DecodeState>(), unf.as<int>(), out.as<long long>(), len.as<int>(), out_ld, M, 0, 0,
                                        static_cast<const act_t*>(W), xn.as<res_t>(), K);
   set_state_kernel<<<1, 1, 0, s>>>(st.as<DecodeState>(), step);
   cudaError_t e = cudaSuccess;
-  if (ph.on) {
+  if (proc) {
     e = cudaMemcpy2DAsync(out.p, static_cast<size_t>(out_ld) * 8, hist, static_cast<size_t>(step + 1) * 8,
                           static_cast<size_t>(step + 1) * 8, M, cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess) e = pb.upload(ph, s);
@@ -2557,42 +2460,65 @@ extern "C" int b200t5_test_lm_score(int device, const void* x, const void* W, in
                                           out_ld, nullptr, step + 1);
   }
   // the row's label of this step sits in column `step` of its [M, T] label rows; score_reset_kernel reads column 0
-  if (e == cudaSuccess && forced)
+  if (e == cudaSuccess && score && forced)
     e = cudaMemcpy2DAsync(fids.as<long long>() + step, static_cast<size_t>(T) * 8, forced, 8, 8, M, cudaMemcpyDeviceToDevice, s);
-  if (e == cudaSuccess) {
+  if (e == cudaSuccess && score) {
     score_reset_kernel<<<M, 128, 0, s>>>(lp.as<float>(), lg.as<float>(), static_cast<size_t>(M) * T, ftok.as<int>(), M, nullptr, nullptr,
                                          forced ? fids.as<long long>() + step : nullptr, T);
     e = cudaGetLastError();
   }
-  const ProcDev pd = ph.on ? pb.dev() : ProcDev();
-  const EpiArgmax::Params ea{pval.as<float>(), pidx.as<int>(), n_tiles, &st.as<DecodeState>()->step, eos, min_new, 0};
-  const int* ft = forced ? ftok.as<int>() : nullptr;
-  if (e == cudaSuccess && ph.on) {
-    EpiScore<true>::Params ep{{ea, pd, nullptr, 0}, psum.as<float>(), fval.as<float>(), ft, vals, V};
-    e = run_gemm(&dummy, mk(ta, tb, M, V, K, G_SCOREPROC128, 1), &ep, s, false);
-  } else if (e == cudaSuccess) {
-    EpiScore<false>::Params ep{ea, psum.as<float>(), fval.as<float>(), ft, vals, V};
-    e = run_gemm(&dummy, mk(ta, tb, M, V, K, G_SCORE128, 1), &ep, s, false);
+  LmHeadParams ep{};
+  ep.pval = pval.as<float>();
+  ep.pidx = pidx.as<int>();
+  ep.n_tiles = n_tiles;
+  ep.step = &st.as<DecodeState>()->step;
+  ep.eos = eos;
+  ep.min_new = min_new;
+  if (proc) ep.pd = pb.dev();
+  ep.vals = vals;
+  ep.ldv = V;
+  FinalizeArgs fa{ep.pval, ep.pidx, n_tiles, st.as<DecodeState>(), unf.as<int>(), out.as<long long>(), len.as<int>(), out_ld, -1, 0,
+                  static_cast<const act_t*>(W), xn.as<res_t>(), K, ext.as<int>(), nullptr, nullptr, T, ep.pd, ScoreDev()};
+  if (score) {
+    ep.psum = psum.as<float>();
+    ep.fval = fval.as<float>();
+    ep.ftok = forced ? ftok.as<int>() : nullptr;
+    fa.sd = {ep.psum, ep.fval, ftok.as<int>(), forced ? fids.as<long long>() : nullptr, lp.as<float>(), lg.as<float>()};
   }
-  ScoreDev sd;
-  sd.psum = psum.as<float>();
-  sd.fval = fval.as<float>();
-  sd.ftok = ftok.as<int>();
-  sd.forced = forced ? fids.as<long long>() : nullptr;
-  sd.logprob = lp.as<float>();
-  sd.logit = lg.as<float>();
-  if (e == cudaSuccess)
-    e = launch_kernel(ph.on ? finalize_step_score_kernel<true> : finalize_step_score_kernel<false>, dim3(M), dim3(128), 0, s, false,
-                      pval.as<float>(), pidx.as<int>(), n_tiles, st.as<DecodeState>(), unf.as<int>(), out.as<long long>(), len.as<int>(),
-                      out_ld, static_cast<long long>(-1), static_cast<long long>(0), static_cast<const act_t*>(W), xn.as<res_t>(), K,
-                      ext.as<int>(), static_cast<int*>(nullptr), static_cast<const int*>(nullptr), T, pd, sd);
+  if (e == cudaSuccess) e = run_lm_head(&dummy, proc, score, ta, tb, M, V, K, ep, fa, s, false);
   if (e == cudaSuccess)
     e = cudaMemcpy2DAsync(tokens, 8, out.as<long long>() + step + 1, static_cast<size_t>(out_ld) * 8, 8, M, cudaMemcpyDeviceToDevice, s);
-  if (e == cudaSuccess) e = cudaMemcpy2DAsync(logprob, 4, lp.as<float>() + step, static_cast<size_t>(T) * 4, 4, M, cudaMemcpyDeviceToDevice, s);
-  if (e == cudaSuccess) e = cudaMemcpy2DAsync(logit, 4, lg.as<float>() + step, static_cast<size_t>(T) * 4, 4, M, cudaMemcpyDeviceToDevice, s);
+  if (e == cudaSuccess && score)
+    e = cudaMemcpy2DAsync(logprob, 4, lp.as<float>() + step, static_cast<size_t>(T) * 4, 4, M, cudaMemcpyDeviceToDevice, s);
+  if (e == cudaSuccess && score)
+    e = cudaMemcpy2DAsync(logit, 4, lg.as<float>() + step, static_cast<size_t>(T) * 4, 4, M, cudaMemcpyDeviceToDevice, s);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_lm_score: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "%s: %s", name, cudaGetErrorString(e));
   return B200T5_OK;
+}
+
+// the plain head: the lowest-index arg-max tie rule
+extern "C" int b200t5_test_lm_argmax(int device, const void* x, const void* W, int M, int V, int K, int step, int eos,
+                                     int min_new, int64_t* tokens, void* stream) {
+  return test_lm_head("test_lm_argmax", device, x, W, M, V, K, step, eos, min_new, nullptr, false, nullptr, nullptr, 0, false,
+                      nullptr, tokens, nullptr, nullptr, nullptr, stream);
+}
+
+// the head with processors, whatever `logits` holds
+extern "C" int b200t5_test_lm_process(int device, const void* x, const void* W, int M, int V, int K, int step, int eos,
+                                      int min_new, const b200t5_logits_params* logits, const int64_t* hist,
+                                      const int64_t* enc_ids, int S, int64_t* tokens, float* vals, void* stream) {
+  return test_lm_head("test_lm_process", device, x, W, M, V, K, step, eos, min_new, logits, true, hist, enc_ids, S, false,
+                      nullptr, tokens, nullptr, nullptr, vals, stream);
+}
+
+// the scored head, with processors when `logits` has an active one
+extern "C" int b200t5_test_lm_score(int device, const void* x, const void* W, int M, int V, int K, int step, int eos,
+                                    int min_new, const b200t5_logits_params* logits, const int64_t* hist,
+                                    const int64_t* enc_ids, int S, const int64_t* forced, int64_t* tokens, float* logprob,
+                                    float* logit, float* vals, void* stream) {
+  return test_lm_head("test_lm_score", device, x, W, M, V, K, step, eos, min_new, logits, false, hist, enc_ids, S, true, forced,
+                      tokens, logprob, logit, vals, stream);
 }
 
 extern "C" int b200t5_test_gemm_splitk(int device, const void* A, const void* W, void* C, int M, int N, int K, int bn,

@@ -292,10 +292,10 @@ __global__ void admit_slots_kernel(const int* __restrict__ slots, const int* __r
 // kProc (logits processors active): a row finishes on any of the call's EOS ids, and a row that goes on marks its
 // token as seen and computes the bans of its next step (logits_process.cuh).
 //
-// kScore (token log-probabilities, finalize_step_score_kernel): the epilogue also left psum[b][i] = sum of
-// expf(v - pval[b][i]) over tile i (gemm.cuh: EpiScore). They are merged in an order that depends on nothing but
-// n_tiles and the 128-thread CTA - thread k adds tiles k, k + 128, ... in ascending order, the warp's lanes are
-// folded by the xor tree, thread 0 adds the four warps in order:
+// kScore (token log-probabilities): the epilogue also left psum[b][i] = sum of expf(v - pval[b][i]) over tile i
+// (gemm.cuh: EpiLmHead). They are merged in an order that depends on nothing but n_tiles and the 128-thread CTA -
+// thread k adds tiles k, k + 128, ... in ascending order, the warp's lanes are folded by the xor tree, thread 0 adds the
+// four warps in order:
 //   M = max_i m_i,  S = sum_i s_i * expf(m_i - M),  lse = M + logf(S)
 // so a row's numbers are bit-identical whichever row-chain, slot or batch it sits in. For an unfinished row at step t
 //   logit[row][t] = v_tok,  logprob[row][t] = v_tok - lse          (fp32 [rows, max_new]; untouched positions stay 0)
@@ -311,23 +311,38 @@ struct ScoreDev {
   float* logit = nullptr;        // [rows][max_new]
 };
 
+struct FinalizeArgs {
+  const float* pval;  // [B][n_tiles]
+  const int* pidx;    // [B][n_tiles]
+  int n_tiles;
+  DecodeState* st;
+  int* unfinished;
+  long long* out_ids;  // [rows][out_ld]
+  int* out_len;        // [rows]
+  int out_ld;
+  long long eos_tok, pad_tok;
+  const act_t* E;  // embedding table
+  res_t* x;        // [B][d]: the next step's decoder input
+  int d;
+  int* live_extent;
+  int* pos;            // slot pool: per-slot positions, else nullptr
+  const int* out_row;  // slot pool: per-slot result rows, else nullptr
+  int max_new;
+  ProcDev pd;   // kProc
+  ScoreDev sd;  // kScore
+};
+
 template <bool kProc, bool kScore>
-DEVINL void finalize_step_body(const float* __restrict__ pval, const int* __restrict__ pidx, int n_tiles,
-                               DecodeState* st, int* __restrict__ unfinished,
-                               long long* __restrict__ out_ids, int* __restrict__ out_len, int out_ld,
-                               long long eos_tok, long long pad_tok, const act_t* __restrict__ E,
-                               res_t* __restrict__ x, int d, int* __restrict__ live_extent,
-                               int* __restrict__ pos, const int* __restrict__ out_row, int max_new, const ProcDev& pd,
-                               const ScoreDev& sd) {
+__global__ void finalize_step_kernel(const FinalizeArgs a) {
   pdl_launch_dependents();
   pdl_wait();
   const int b = blockIdx.x;
-  const int t = pos != nullptr ? pos[b] : st->step;
+  const int t = a.pos != nullptr ? a.pos[b] : a.st->step;
   float best = -INFINITY;
   int bidx = 0x7fffffff;
-  for (int i = threadIdx.x; i < n_tiles; i += blockDim.x) {
-    const float v = pval[static_cast<size_t>(b) * n_tiles + i];
-    const int ix = pidx[static_cast<size_t>(b) * n_tiles + i];
+  for (int i = threadIdx.x; i < a.n_tiles; i += blockDim.x) {
+    const float v = a.pval[static_cast<size_t>(b) * a.n_tiles + i];
+    const int ix = a.pidx[static_cast<size_t>(b) * a.n_tiles + i];
     if (v > best || (v == best && ix < bidx)) {
       best = v;
       bidx = ix;
@@ -357,8 +372,8 @@ DEVINL void finalize_step_body(const float* __restrict__ pval, const int* __rest
     __shared__ float s_s[32];
     float mx = s_v[0];
     for (int w = 1; w < nwarp; ++w) mx = fmaxf(mx, s_v[w]);
-    for (int i = threadIdx.x; i < n_tiles; i += blockDim.x)
-      ssum += sd.psum[static_cast<size_t>(b) * n_tiles + i] * expf(pval[static_cast<size_t>(b) * n_tiles + i] - mx);
+    for (int i = threadIdx.x; i < a.n_tiles; i += blockDim.x)
+      ssum += a.sd.psum[static_cast<size_t>(b) * a.n_tiles + i] * expf(a.pval[static_cast<size_t>(b) * a.n_tiles + i] - mx);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) ssum += __shfl_xor_sync(0xffffffffu, ssum, o);
     if (lane_id() == 0) s_s[warp] = ssum;
@@ -373,76 +388,53 @@ DEVINL void finalize_step_body(const float* __restrict__ pval, const int* __rest
         bidx = s_i[w];
       }
     }
-    const int unf = unfinished[b];
-    const int row = out_row != nullptr ? out_row[b] : b;
-    long long tok = unf ? static_cast<long long>(bidx) : pad_tok;
+    const int unf = a.unfinished[b];
+    const int row = a.out_row != nullptr ? a.out_row[b] : b;
+    long long tok = unf ? static_cast<long long>(bidx) : a.pad_tok;
     bool forced = false;
     if constexpr (kScore) {
-      forced = sd.forced != nullptr;
+      forced = a.sd.forced != nullptr;
       if (unf) {
         float v_tok = best;
         if (forced) {
-          tok = sd.forced[static_cast<size_t>(row) * max_new + t];
-          v_tok = sd.fval[b];
+          tok = a.sd.forced[static_cast<size_t>(row) * a.max_new + t];
+          v_tok = a.sd.fval[b];
         }
-        sd.logprob[static_cast<size_t>(row) * max_new + t] = v_tok - (best + logf(ssum));
-        if (sd.logit != nullptr) sd.logit[static_cast<size_t>(row) * max_new + t] = v_tok;
+        a.sd.logprob[static_cast<size_t>(row) * a.max_new + t] = v_tok - (best + logf(ssum));
+        if (a.sd.logit != nullptr) a.sd.logit[static_cast<size_t>(row) * a.max_new + t] = v_tok;
       }
     }
-    if (pos == nullptr || unf) out_ids[static_cast<size_t>(row) * out_ld + t + 1] = tok;
+    if (a.pos == nullptr || unf) a.out_ids[static_cast<size_t>(row) * a.out_ld + t + 1] = tok;
     bool fin = false;
     if (unf) {
-      out_len[row] = t + 1;
+      a.out_len[row] = t + 1;
       if (forced) {
-        fin = t + 1 >= max_new || sd.forced[static_cast<size_t>(row) * max_new + t + 1] < 0;
-        sd.ftok[b] = fin ? -1 : static_cast<int>(sd.forced[static_cast<size_t>(row) * max_new + t + 1]);
+        fin = t + 1 >= a.max_new || a.sd.forced[static_cast<size_t>(row) * a.max_new + t + 1] < 0;
+        a.sd.ftok[b] = fin ? -1 : static_cast<int>(a.sd.forced[static_cast<size_t>(row) * a.max_new + t + 1]);
       } else {
-        fin = (kProc ? proc_is_eos(*pd.cfg, tok) : tok == eos_tok) || (pos != nullptr && t + 1 >= max_new);
+        fin = (kProc ? proc_is_eos(*a.pd.cfg, tok) : tok == a.eos_tok) || (a.pos != nullptr && t + 1 >= a.max_new);
       }
       if (fin) {
-        unfinished[b] = 0;
-        live_extent[b] = 0;
-        atomicAdd(&st->finished_rows, 1);
+        a.unfinished[b] = 0;
+        a.live_extent[b] = 0;
+        atomicAdd(&a.st->finished_rows, 1);
       }
     }
-    if (pos != nullptr) pos[b] = (unf && !fin) ? t + 1 : 0;
-    s_tok = (pos != nullptr && fin) ? pad_tok : tok;
+    if (a.pos != nullptr) a.pos[b] = (unf && !fin) ? t + 1 : 0;
+    s_tok = (a.pos != nullptr && fin) ? a.pad_tok : tok;
     if constexpr (kProc) {
       s_go = unf && !fin;
-      if (unf && !fin && pd.cfg->rep_pen) bit_set(pd.seen + static_cast<size_t>(pd.row0 + b) * pd.W, static_cast<int>(tok));
+      if (unf && !fin && a.pd.cfg->rep_pen) bit_set(a.pd.seen + static_cast<size_t>(a.pd.row0 + b) * a.pd.W, static_cast<int>(tok));
     }
   }
   __syncthreads();
-  const uint4* src = reinterpret_cast<const uint4*>(E + static_cast<size_t>(s_tok) * d);
-  res_t* dst = x + static_cast<size_t>(b) * d;
-  for (int i = threadIdx.x; i < d / 8; i += blockDim.x) store_res8_from_act(dst + i * 8, src[i]);
+  const uint4* src = reinterpret_cast<const uint4*>(a.E + static_cast<size_t>(s_tok) * a.d);
+  res_t* dst = a.x + static_cast<size_t>(b) * a.d;
+  for (int i = threadIdx.x; i < a.d / 8; i += blockDim.x) store_res8_from_act(dst + i * 8, src[i]);
   if constexpr (kProc) {
     // the row's decoder ids are now its result row up to column t + 1 (written above, visible after the barrier)
-    if (s_go) proc_new_bans(pd, pd.row0 + b, out_ids + static_cast<size_t>(out_row != nullptr ? out_row[b] : b) * out_ld, t + 2, true);
+    if (s_go) proc_new_bans(a.pd, a.pd.row0 + b, a.out_ids + static_cast<size_t>(a.out_row != nullptr ? a.out_row[b] : b) * a.out_ld, t + 2, true);
   }
-}
-
-template <bool kProc>
-__global__ void finalize_step_kernel(const float* __restrict__ pval, const int* __restrict__ pidx, int n_tiles,
-                                     DecodeState* st, int* __restrict__ unfinished,
-                                     long long* __restrict__ out_ids, int* __restrict__ out_len, int out_ld,
-                                     long long eos_tok, long long pad_tok, const act_t* __restrict__ E,
-                                     res_t* __restrict__ x, int d, int* __restrict__ live_extent,
-                                     int* __restrict__ pos, const int* __restrict__ out_row, int max_new, ProcDev pd) {
-  finalize_step_body<kProc, false>(pval, pidx, n_tiles, st, unfinished, out_ids, out_len, out_ld, eos_tok, pad_tok, E, x, d,
-                                   live_extent, pos, out_row, max_new, pd, ScoreDev());
-}
-
-template <bool kProc>
-__global__ void finalize_step_score_kernel(const float* __restrict__ pval, const int* __restrict__ pidx, int n_tiles,
-                                           DecodeState* st, int* __restrict__ unfinished,
-                                           long long* __restrict__ out_ids, int* __restrict__ out_len, int out_ld,
-                                           long long eos_tok, long long pad_tok, const act_t* __restrict__ E,
-                                           res_t* __restrict__ x, int d, int* __restrict__ live_extent,
-                                           int* __restrict__ pos, const int* __restrict__ out_row, int max_new, ProcDev pd,
-                                           ScoreDev sd) {
-  finalize_step_body<kProc, true>(pval, pidx, n_tiles, st, unfinished, out_ids, out_len, out_ld, eos_tok, pad_tok, E, x, d,
-                                  live_extent, pos, out_row, max_new, pd, sd);
 }
 
 // Start of a scored call, and of every row of it. With logprob != nullptr: zero the n result elements (positions a

@@ -15,8 +15,6 @@
 // so each functor first rounds the fp32 accumulator to bf16 and only then fuses
 // the residual add / GeGLU / KV scatter / arg-max.
 #pragma once
-#include <type_traits>
-
 #include "logits_process.cuh"
 #include "ptx.cuh"
 
@@ -594,70 +592,45 @@ struct EpiQkvDecode {
   }
 };
 
-// ---- lm_head + greedy arg-max: logits never reach HBM. Each (row, n_tile) emits the
-// max bf16-rounded logit of its BN columns and the lowest column index attaining it
-// (torch.argmax first-index contract; generation/utils.py:2762,2793). EOS is masked
-// to -inf while step < min_new_tokens (generation/logits_process.py:225-233).
-struct EpiArgmax {
-  struct Params {
-    float* pval;  // [M, n_tiles]
-    int* pidx;    // [M, n_tiles]
-    int n_tiles;
-    const int* step;
-    int eos, min_new;
-    int step_stride = 0;  // 1 = slot pool: per-row positions
-  };
-  static DEVINL void prologue(const Params&, uint8_t*, int, int = 128) {}
-  // the score of column n (shared with EpiScore: the arg-max and the log-sum-exp see the same fp32 number)
-  static DEVINL float value(const Params& p, uint32_t acc, int n, int N, bool block_eos) {
-    const float v = act_round(__uint_as_float(acc));
-    return (n >= N || (block_eos && n == p.eos)) ? -INFINITY : v;
-  }
-  // a row's arg-max is not split: the first of the `parts` threads of each row takes the whole row
-  template <int BN>
-  static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t*, int part, int) {
-    if (part != 0) return;
-    float best = -INFINITY;
-    int bidx = n_tile * BN;  // all -inf (cannot happen with finite logits) -> first column, like torch
-    const bool block_eos = m_ok && p.step[m * p.step_stride] < p.min_new;
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      uint32_t acc[32];
-      acc_ld_32(taddr + c * 32, acc);
-      const int n0 = n_tile * BN + c * 32;
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int n = n0 + j;
-        const float v = value(p, acc[j], n, N, block_eos);
-        if (v > best) {  // ascending scan + strict '>' keeps the lowest index among equal maxima
-          best = v;
-          bidx = n;
-        }
-      }
-    }
-    if (m_ok) {
-      p.pval[static_cast<size_t>(m) * p.n_tiles + n_tile] = best;
-      p.pidx[static_cast<size_t>(m) * p.n_tiles + n_tile] = bidx;
-    }
-  }
+// ---- lm_head epilogue of the decode step: logits never reach HBM. Each (row, n_tile) emits the max of its BN column
+// values and the lowest column index attaining it (torch.argmax first-index contract; generation/utils.py:2762,2793);
+// finalize_step_kernel merges the tiles. A row is not split: the first of the `parts` threads of each row takes it all.
+//   kProc = false: a column's value is its logit rounded to act_t, EOS masked to -inf while step < min_new
+//     (generation/logits_process.py:225-233).
+//   kProc = true (logits_process.cuh): the logit after transformers' greedy processors. Each logit is rounded to act_t
+//     and widened to fp32 (HF's `.to(torch.float32)`), then in HF's order: encoder repetition penalty, repetition
+//     penalty (on the already penalised value), + 0 when bad words are active (HF adds a zero bias), and -inf where the
+//     row's next-step bans, the static mask, the begin-suppress mask (step 0) or the EOS mask (step < min_new) has the
+//     column's bit.
+//   kScore (token log-probabilities): also, per (row, tile),
+//     psum = sum_n expf(v_n - tile max)   (-inf columns add 0; an all -inf tile emits 0)
+//     accumulated in ascending column order by the one thread that owns the row, so it does not depend on where the
+//     row sits. The tile is read twice from the staged accumulators: once for the maximum, once for the sum. When the
+//     step is teacher-forced, ftok[m] is the row's forced column (-1: none) and the tile that contains it writes its
+//     value to fval[m].
+// The arg-max and the log-sum-exp see the same fp32 number per column.
+struct LmHeadParams {
+  float* pval;  // [M, n_tiles]
+  int* pidx;    // [M, n_tiles]
+  int n_tiles;
+  const int* step;
+  int eos, min_new;
+  int step_stride;  // 1 = slot pool: per-row positions
+  ProcDev pd;       // kProc
+  float* psum;      // kScore: [M, n_tiles]
+  float* fval;      // kScore: [M]
+  const int* ftok;  // kScore: [M], nullptr = the step is not teacher-forced
+  float* vals;      // test hook only, else nullptr: the processed values [M, ldv]
+  int ldv;
 };
 
-// ---- lm_head + logits processors + greedy arg-max (logits_process.cuh): the same (max, lowest index) partials as
-// EpiArgmax, from the logits after transformers' greedy processors. Each logit is rounded to act_t and widened to fp32
-// (HF's `.to(torch.float32)`), then in HF's order: encoder repetition penalty, repetition penalty (on the already
-// penalised value), + 0 when bad words are active (HF adds a zero bias), and -inf where the row's next-step bans, the
-// static mask, the begin-suppress mask (step 0) or the EOS mask (step < min_new) has the column's bit. `vals`
-// (test hook only, else nullptr) receives the processed values [M, ldv].
-struct EpiArgmaxProc {
-  struct Params {
-    EpiArgmax::Params a;
-    ProcDev pd;
-    float* vals;
-    int ldv;
-  };
+template <bool kProc, bool kScore>
+struct EpiLmHead {
+  using Params = LmHeadParams;
+  // The plain head never writes `vals` (its test hook reads only tokens): a per-column test would cost the hot path.
+  static constexpr bool kVals = kProc || kScore;
   static DEVINL void prologue(const Params&, uint8_t*, int, int = 128) {}
-  // What a row needs of the call's configuration, and the bitmap words of one 32-column chunk of it
-  // (shared with EpiScore, as is `value`).
+  // What a processed row needs of the call's configuration, and the bitmap words of one 32-column chunk of it
   struct Row {
     bool enc_pen, rep_pen, bad_add;
     float en, ep, rn, rp;
@@ -678,7 +651,7 @@ struct EpiArgmaxProc {
     r.rn = cf.rep_neg;
     r.rp = cf.rep_pos;
     r.rw = static_cast<size_t>(p.pd.row0 + m) * p.pd.W;
-    r.t = m_ok ? p.a.step[m * p.a.step_stride] : 1;
+    r.t = m_ok ? p.step[m * p.step_stride] : 1;
     return r;
   }
   static DEVINL Words words(const Params& p, const Row& r, bool m_ok, int n0) {
@@ -687,12 +660,18 @@ struct EpiArgmaxProc {
     if (m_ok && w < W) {
       o.ban = p.pd.banned[r.rw + w] | p.pd.stat[w];
       if (r.t == 0) o.ban |= p.pd.stat[W + w];
-      if (r.t < p.a.min_new) o.ban |= p.pd.stat[2 * W + w];
+      if (r.t < p.min_new) o.ban |= p.pd.stat[2 * W + w];
       if (r.rep_pen) o.seen = p.pd.seen[r.rw + w];
       if (r.enc_pen) o.enc = p.pd.enc[r.rw + w];
     }
     return o;
   }
+  // the value of column n without processors: EOS masked by index
+  static DEVINL float value(const Params& p, uint32_t acc, int n, int N, bool block_eos) {
+    const float v = act_round(__uint_as_float(acc));
+    return (n >= N || (block_eos && n == p.eos)) ? -INFINITY : v;
+  }
+  // ... and with processors: EOS masked by the bitmap
   static DEVINL float value(const Row& r, const Words& o, uint32_t acc, int j, int n, int N) {
     float v = act_round(__uint_as_float(acc));
     if ((o.enc >> j) & 1u) v = v < 0.f ? v * r.en : v * r.ep;
@@ -705,89 +684,38 @@ struct EpiArgmaxProc {
   static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t*, int part, int) {
     static_assert(BN % 32 == 0, "one bitmap word per 32 columns");
     if (part != 0) return;
-    const Row r = row(p, m, m_ok);
-    float best = -INFINITY;
-    int bidx = n_tile * BN;
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      uint32_t acc[32];
-      acc_ld_32(taddr + c * 32, acc);
-      const int n0 = n_tile * BN + c * 32;
-      const Words o = words(p, r, m_ok, n0);
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int n = n0 + j;
-        const float v = value(r, o, acc[j], j, n, N);
-        if (p.vals != nullptr && m_ok && n < N) p.vals[static_cast<size_t>(m) * p.ldv + n] = v;
-        if (v > best) {
-          best = v;
-          bidx = n;
-        }
-      }
-    }
-    if (m_ok) {
-      p.a.pval[static_cast<size_t>(m) * p.a.n_tiles + n_tile] = best;
-      p.a.pidx[static_cast<size_t>(m) * p.a.n_tiles + n_tile] = bidx;
-    }
-  }
-};
-
-// ---- lm_head + arg-max + log-sum-exp partials (token log-probabilities): what EpiArgmax (kProc = false) or
-// EpiArgmaxProc (kProc = true) emits, from the same per-column values, plus per (row, tile)
-//   psum = sum_n expf(v_n - tile max)   (-inf columns add 0; an all -inf tile emits 0)
-// accumulated in ascending column order by the one thread that owns the row, so it does not depend on where the row
-// sits; finalize_step_score_kernel merges the tiles. The tile is read twice from the staged accumulators: once for
-// the maximum, once for the sum. When the step is teacher-forced, ftok[m] is the row's forced column (-1: none) and
-// the tile that contains it writes its value to fval[m].
-template <bool kProc>
-struct EpiScore {
-  using Base = typename std::conditional<kProc, EpiArgmaxProc, EpiArgmax>::type;
-  struct Params {
-    typename Base::Params b;
-    float* psum;      // [M, n_tiles]
-    float* fval;      // [M]
-    const int* ftok;  // [M], nullptr = the step is not teacher-forced
-    float* vals;      // test hook only, else nullptr: the processed values [M, ldv]
-    int ldv;
-  };
-  static DEVINL void prologue(const Params&, uint8_t*, int, int = 128) {}
-  static DEVINL const EpiArgmax::Params& arg(const Params& p) {
-    if constexpr (kProc) return p.b.a;
-    else return p.b;
-  }
-  template <int BN>
-  static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t*, int part, int) {
-    if (part != 0) return;
-    const EpiArgmax::Params& a = arg(p);
-    EpiArgmaxProc::Row r{};
+    Row r{};
     bool block_eos = false;
-    if constexpr (kProc) r = EpiArgmaxProc::row(p.b, m, m_ok);
-    else block_eos = m_ok && a.step[m * a.step_stride] < a.min_new;
-    const int forced = (m_ok && p.ftok != nullptr) ? p.ftok[m] : -1;
+    if constexpr (kProc) r = row(p, m, m_ok);
+    else block_eos = m_ok && p.step[m * p.step_stride] < p.min_new;
+    int forced = -1;
+    if constexpr (kScore) forced = (m_ok && p.ftok != nullptr) ? p.ftok[m] : -1;
     float best = -INFINITY, sum = 0.f;
-    int bidx = n_tile * BN;
+    int bidx = n_tile * BN;  // all -inf (cannot happen with finite logits) -> first column, like torch
 #pragma unroll 1
-    for (int pass = 0; pass < 2; ++pass) {
+    for (int pass = 0; pass < (kScore ? 2 : 1); ++pass) {
 #pragma unroll 1
       for (int c = 0; c < BN / 32; ++c) {
         uint32_t acc[32];
         acc_ld_32(taddr + c * 32, acc);
         const int n0 = n_tile * BN + c * 32;
-        EpiArgmaxProc::Words o{0, 0, 0};
-        if constexpr (kProc) o = EpiArgmaxProc::words(p.b, r, m_ok, n0);
+        Words o{0, 0, 0};
+        if constexpr (kProc) o = words(p, r, m_ok, n0);
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
           const int n = n0 + j;
           float v;
-          if constexpr (kProc) v = EpiArgmaxProc::value(r, o, acc[j], j, n, N);
-          else v = EpiArgmax::value(a, acc[j], n, N, block_eos);
+          if constexpr (kProc) v = value(r, o, acc[j], j, n, N);
+          else v = value(p, acc[j], n, N, block_eos);
           if (pass == 0) {
-            if (v > best) {
+            if (v > best) {  // ascending scan + strict '>' keeps the lowest index among equal maxima
               best = v;
               bidx = n;
             }
-            if (n == forced) p.fval[m] = v;
-            if (p.vals != nullptr && m_ok && n < N) p.vals[static_cast<size_t>(m) * p.ldv + n] = v;
+            if constexpr (kScore)
+              if (n == forced) p.fval[m] = v;
+            if constexpr (kVals)
+              if (p.vals != nullptr && m_ok && n < N) p.vals[static_cast<size_t>(m) * p.ldv + n] = v;
           } else if (v != -INFINITY) {
             sum += expf(v - best);
           }
@@ -795,9 +723,9 @@ struct EpiScore {
       }
     }
     if (m_ok) {
-      a.pval[static_cast<size_t>(m) * a.n_tiles + n_tile] = best;
-      a.pidx[static_cast<size_t>(m) * a.n_tiles + n_tile] = bidx;
-      p.psum[static_cast<size_t>(m) * a.n_tiles + n_tile] = sum;
+      p.pval[static_cast<size_t>(m) * p.n_tiles + n_tile] = best;
+      p.pidx[static_cast<size_t>(m) * p.n_tiles + n_tile] = bidx;
+      if constexpr (kScore) p.psum[static_cast<size_t>(m) * p.n_tiles + n_tile] = sum;
     }
   }
 };

@@ -10,8 +10,8 @@
 //     EOS ids};
 //   - per row, the list of the tokens set in `banned` (so that the next update clears exactly those bits instead
 //     of the whole bitmap) and the prompt's ids as int32.
-// The fused lm_head epilogue (gemm.cuh: EpiArgmaxProc) applies them per 128-column tile; proc_new_bans runs at the
-// end of finalize_step_kernel<true>, one CTA per row, once the row's token is known.
+// The fused lm_head epilogue (gemm.cuh: EpiLmHead<true, *>) applies them per 128-column tile; proc_new_bans runs at the
+// end of finalize_step_kernel<true, *>, one CTA per row, once the row's token is known.
 #pragma once
 #include "ptx.cuh"
 

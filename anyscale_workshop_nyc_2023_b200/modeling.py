@@ -431,19 +431,8 @@ class B200T5ForConditionalGeneration:
             # more rows than one pool of decode slots, still in host memory: the slot pool admits prompts from host
             # buffers as slots free up, so nothing is copied to the device (and back) up front
             return self._generate_pool_from_host(host, attention_mask, gp, lp)
-        ids = host.to(device=self._device, dtype=torch.long).contiguous()
+        ids, mask = self._device_inputs(host, attention_mask, gp, lp)
         B, S = ids.shape
-        if ids.numel():
-            lo, hi = torch.aminmax(ids)  # one kernel, one synchronisation
-            if bool(((lo < 0) | (hi >= self.config.vocab_size)).item()):
-                raise IndexError("input_ids contain token ids outside [0, vocab_size)")
-        mask = None
-        if attention_mask is not None:
-            mask = torch.as_tensor(attention_mask).to(device=self._device, dtype=torch.long).contiguous()
-            if mask.shape != ids.shape:
-                raise ValueError("attention_mask shape must match input_ids")
-        else:
-            mask = self._infer_attention_mask(ids, gp, lp)
         if B > self.pool_size:
             if self.takes_host_batches(B, S):
                 # more rows than one pool of decode slots: continuous batching, same tokens row for row. The pool
@@ -490,18 +479,8 @@ class B200T5ForConditionalGeneration:
         """generate's routing (static batch, slot pool, static chunks) for a scored call: (sequences [B, 1+T'],
         lengths [B], token_logprobs [B, T'], token_logits [B, T']) on the device. With `labels` the call is
         teacher-forced and T' = labels.shape[1]."""
-        ids = host.to(device=self._device, dtype=torch.long).contiguous()
+        ids, mask = self._device_inputs(host, attention_mask, gp, lp)
         B, S = ids.shape
-        if ids.numel():
-            lo, hi = torch.aminmax(ids)
-            if bool(((lo < 0) | (hi >= self.config.vocab_size)).item()):
-                raise IndexError("input_ids contain token ids outside [0, vocab_size)")
-        if attention_mask is not None:
-            mask = torch.as_tensor(attention_mask).to(device=self._device, dtype=torch.long).contiguous()
-            if mask.shape != ids.shape:
-                raise ValueError("attention_mask shape must match input_ids")
-        else:
-            mask = self._infer_attention_mask(ids, gp, lp)
         T = gp.max_new_tokens
         if B > self.pool_size and self.takes_host_batches(B, S):
             out, lens, logp, logit = self.generate_stream(ids.cpu().numpy(), None if mask is None else mask.cpu().numpy(),
@@ -523,6 +502,32 @@ class B200T5ForConditionalGeneration:
                           forced_len=0 if labels is None else int(labels.shape[1]))
         return io, (logp, logit, labels)
 
+    def _check_inputs(self, ids, mask) -> None:
+        """input_ids (a torch tensor or a numpy array) within [0, vocab_size), and attention_mask (None: not given) of
+        the same shape."""
+        V = self.config.vocab_size
+        bad = False
+        if isinstance(ids, torch.Tensor):
+            if ids.numel():
+                lo, hi = torch.aminmax(ids)  # one kernel, one synchronisation
+                bad = bool(((lo < 0) | (hi >= V)).item())
+        elif ids.size:
+            bad = int(ids.min()) < 0 or int(ids.max()) >= V
+        if bad:
+            raise IndexError("input_ids contain token ids outside [0, vocab_size)")
+        if mask is not None and mask.shape != ids.shape:
+            raise ValueError("attention_mask shape must match input_ids")
+
+    def _device_inputs(self, host: torch.Tensor, attention_mask, gp, lp):
+        """input_ids and attention_mask as contiguous int64 tensors on the model's device, checked; without an
+        attention_mask the inferred one (None: attend everywhere)."""
+        ids = host.to(device=self._device, dtype=torch.long).contiguous()
+        mask = None
+        if attention_mask is not None:
+            mask = torch.as_tensor(attention_mask).to(device=self._device, dtype=torch.long).contiguous()
+        self._check_inputs(ids, mask)
+        return ids, (self._infer_attention_mask(ids, gp, lp) if mask is None else mask)
+
     def takes_host_batches(self, B: int, S: int) -> bool:
         """True when a [B, S] batch would go through the slot pool, whose entry point takes HOST buffers: a caller that
         still has the batch in host memory (predictor.py) hands it over as it is."""
@@ -530,13 +535,11 @@ class B200T5ForConditionalGeneration:
 
     def _generate_pool_from_host(self, ids: torch.Tensor, attention_mask, gp, lp=None) -> torch.Tensor:
         ids_np = np.ascontiguousarray(ids.numpy(), dtype=np.int64)
-        if ids_np.size and (int(ids_np.min()) < 0 or int(ids_np.max()) >= self.config.vocab_size):
-            raise IndexError("input_ids contain token ids outside [0, vocab_size)")
+        mask_np = None
         if attention_mask is not None:
             mask_np = np.ascontiguousarray(torch.as_tensor(attention_mask).cpu().numpy(), dtype=np.int64)
-            if mask_np.shape != ids_np.shape:
-                raise ValueError("attention_mask shape must match input_ids")
-        else:
+        self._check_inputs(ids_np, mask_np)
+        if mask_np is None:
             mask_np = self._infer_mask_np(ids_np, gp, lp)
         out_np, _ = self.generate_stream(ids_np, mask_np, _gen_params=gp, _logits=lp)
         return torch.from_numpy(out_np).to(self._device)
@@ -568,25 +571,20 @@ class B200T5ForConditionalGeneration:
             lens = torch.empty((B,), dtype=torch.int32, device=self._device)
             stream = torch.cuda.current_stream(self._device)
             with self._gpu_lock:
+                io = None
                 if score:  # full-width results: (ids [B, T+1], lengths, token_logprobs [B, T], token_logits [B, T])
                     logp = torch.empty((B, T), dtype=torch.float32, device=self._device)
                     logit = torch.empty((B, T), dtype=torch.float32, device=self._device)
                     forced = None if labels is None else torch.from_numpy(np.ascontiguousarray(labels)).to(self._device)
                     io, _keep = self._score_io(logp, logit, forced)
-                    _chk(self, self._lib.b200t5_generate_scored(self._h, _ptr(ids), _ptr(mask), B, S, C.byref(gp),
-                                                                None if lp is None else lp.ref(), _ptr(out), _ptr(lens), C.byref(io),
-                                                                C.c_void_p(stream.cuda_stream)), self._h)
-                    self.last_lengths = lens
+                _chk(self, self._lib.b200t5_generate_scored(self._h, _ptr(ids), _ptr(mask), B, S, C.byref(gp),
+                                                            None if lp is None else lp.ref(), _ptr(out), _ptr(lens),
+                                                            None if io is None else C.byref(io), C.c_void_p(stream.cuda_stream)),
+                     self._h)
+                self.last_lengths = lens
+                if score:
                     torch.cuda.current_stream(self._device).synchronize()
                     return out, lens, logp, logit
-                if lp is None:
-                    rc = self._lib.b200t5_generate(self._h, _ptr(ids), _ptr(mask), B, S, C.byref(gp), _ptr(out), _ptr(lens),
-                                                   C.c_void_p(stream.cuda_stream))
-                else:
-                    rc = self._lib.b200t5_generate_ex(self._h, _ptr(ids), _ptr(mask), B, S, C.byref(gp), lp.ref(), _ptr(out),
-                                                      _ptr(lens), C.c_void_p(stream.cuda_stream))
-                _chk(self, rc, self._h)
-                self.last_lengths = lens
                 steps = int(lens.max().item())  # synchronises; HF returns exactly the steps it ran
         return out[:, : steps + 1]
 
@@ -597,10 +595,10 @@ class B200T5ForConditionalGeneration:
         return np.ascontiguousarray(ids != pad, dtype=np.int64)
 
     def generate_host(self, input_ids: np.ndarray, attention_mask: Optional[np.ndarray] = None, **kw):
-        """numpy in / numpy out through b200t5_generate_host (the foreign-host entry point):
+        """numpy in / numpy out through b200t5_generate_host_scored (the foreign-host entry point):
         H2D copy, generation, D2H copy and synchronisation all happen inside the library. Takes the logits
-        processor kwargs `generate` takes (through b200t5_generate_host_ex). With output_scores=True it returns
-        (ids, lengths, token_logprobs, token_logits), the last two fp32 [B, T'] (b200t5_generate_host_scored)."""
+        processor kwargs `generate` takes. With output_scores=True it returns (ids, lengths, token_logprobs,
+        token_logits), the last two fp32 [B, T']."""
         gp = self._gen_params(kw.get("max_new_tokens"), kw.get("max_length"), kw.get("min_new_tokens"),
                               kw.get("min_length"), kw.get("eos_token_id"), kw.get("pad_token_id"),
                               kw.get("decoder_start_token_id"), kw.get("poll_interval", 8))
@@ -613,23 +611,19 @@ class B200T5ForConditionalGeneration:
         want_scores = generate_output_flags(kw)[1]
         with self._gpu_lock:
             mp = None if mask is None else mask.ctypes.data_as(C.c_void_p)
+            io = None
             if want_scores:  # -> (ids, lengths, token_logprobs, token_logits), numpy
                 logp = np.empty((B, gp.max_new_tokens), dtype=np.float32)
                 logit = np.empty((B, gp.max_new_tokens), dtype=np.float32)
                 io, _keep = self._score_io(logp, logit, None)
-                _chk(self, self._lib.b200t5_generate_host_scored(self._h, ids.ctypes.data_as(C.c_void_p), mp, B, S, C.byref(gp),
-                                                                 None if lp is None else lp.ref(), out.ctypes.data_as(C.c_void_p),
-                                                                 lens.ctypes.data_as(C.c_void_p), C.byref(io)), self._h)
-                steps = int(lens.max())
-                return out[:, : steps + 1], lens, logp[:, :steps], logit[:, :steps]
-            if lp is None:
-                rc = self._lib.b200t5_generate_host(self._h, ids.ctypes.data_as(C.c_void_p), mp, B, S, C.byref(gp),
-                                                    out.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p))
-            else:
-                rc = self._lib.b200t5_generate_host_ex(self._h, ids.ctypes.data_as(C.c_void_p), mp, B, S, C.byref(gp), lp.ref(),
-                                                       out.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p))
-            _chk(self, rc, self._h)
-        return out[:, : int(lens.max()) + 1], lens
+            _chk(self, self._lib.b200t5_generate_host_scored(self._h, ids.ctypes.data_as(C.c_void_p), mp, B, S, C.byref(gp),
+                                                             None if lp is None else lp.ref(), out.ctypes.data_as(C.c_void_p),
+                                                             lens.ctypes.data_as(C.c_void_p), None if io is None else C.byref(io)),
+                 self._h)
+        steps = int(lens.max())
+        if want_scores:
+            return out[:, : steps + 1], lens, logp[:, :steps], logit[:, :steps]
+        return out[:, : steps + 1], lens
 
     def generate_stream(self, input_ids: np.ndarray, attention_mask: Optional[np.ndarray] = None, *, pool: Optional[int] = None,
                         admit_min: int = 0, _gen_params=None, _logits=None, _labels=None, **kw):
@@ -637,9 +631,8 @@ class B200T5ForConditionalGeneration:
         refilled with the next prompt, so short answers do not wait for the slowest row of a fixed batch as they do
         when BatchPredictor hands `generate` one batch at a time (NB:908-913 -> JOB/predictor.py:102). Returns
         (int64 [N, 1+T'], int32 lengths [N]) with the rows in input order; every row equals what `generate` returns
-        for that prompt. Takes the logits processor kwargs `generate` takes (through b200t5_generate_stream_ex). With
-        output_scores=True it returns (ids, lengths, token_logprobs, token_logits), the last two fp32 [N, T']
-        (b200t5_generate_stream_scored)."""
+        for that prompt. Takes the logits processor kwargs `generate` takes. With output_scores=True it returns (ids,
+        lengths, token_logprobs, token_logits), the last two fp32 [N, T'] (b200t5_generate_stream_scored)."""
         gp = _gen_params or self._gen_params(kw.get("max_new_tokens"), kw.get("max_length"), kw.get("min_new_tokens"),
                                              kw.get("min_length"), kw.get("eos_token_id"), kw.get("pad_token_id"),
                                              kw.get("decoder_start_token_id"), kw.get("poll_interval", 8))
@@ -648,38 +641,30 @@ class B200T5ForConditionalGeneration:
         if ids.ndim != 2:
             raise ValueError(f"input_ids must be [batch, seq], got {ids.shape}")
         N, S = ids.shape
-        if ids.size and (int(ids.min()) < 0 or int(ids.max()) >= self.config.vocab_size):
-            raise IndexError("input_ids contain token ids outside [0, vocab_size)")
-        mask = self._infer_mask_np(ids, gp, lp) if attention_mask is None else np.ascontiguousarray(attention_mask, dtype=np.int64)
-        if mask is not None and mask.shape != ids.shape:
-            raise ValueError("attention_mask shape must match input_ids")
+        mask = None if attention_mask is None else np.ascontiguousarray(attention_mask, dtype=np.int64)
+        self._check_inputs(ids, mask)
+        if mask is None:
+            mask = self._infer_mask_np(ids, gp, lp)
         out = np.empty((N, gp.max_new_tokens + 1), dtype=np.int64)
         lens = np.empty((N,), dtype=np.int32)
         want_scores = generate_output_flags(kw)[1]
         with self._gpu_lock:
             mp = None if mask is None else mask.ctypes.data_as(C.c_void_p)
+            io = None
             if want_scores:
                 logp = np.empty((N, gp.max_new_tokens), dtype=np.float32)
                 logit = np.empty((N, gp.max_new_tokens), dtype=np.float32)
                 io, _keep = self._score_io(logp, logit, None if _labels is None else np.ascontiguousarray(_labels, dtype=np.int64))
-                _chk(self, self._lib.b200t5_generate_stream_scored(self._h, ids.ctypes.data_as(C.c_void_p), mp, N, S, C.byref(gp),
-                                                                   None if lp is None else lp.ref(), int(pool or self.pool_slots),
-                                                                   int(admit_min), out.ctypes.data_as(C.c_void_p),
-                                                                   lens.ctypes.data_as(C.c_void_p), C.byref(io)), self._h)
-                self.last_lengths = torch.from_numpy(lens)
-                steps = int(lens.max())
-                return out[:, : steps + 1], lens, logp[:, :steps], logit[:, :steps]
-            if lp is None:
-                rc = self._lib.b200t5_generate_stream(self._h, ids.ctypes.data_as(C.c_void_p), mp, N, S, C.byref(gp),
-                                                      int(pool or self.pool_slots), int(admit_min),
-                                                      out.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p))
-            else:
-                rc = self._lib.b200t5_generate_stream_ex(self._h, ids.ctypes.data_as(C.c_void_p), mp, N, S, C.byref(gp),
-                                                         lp.ref(), int(pool or self.pool_slots), int(admit_min),
-                                                         out.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p))
-            _chk(self, rc, self._h)
+            _chk(self, self._lib.b200t5_generate_stream_scored(self._h, ids.ctypes.data_as(C.c_void_p), mp, N, S, C.byref(gp),
+                                                               None if lp is None else lp.ref(), int(pool or self.pool_slots),
+                                                               int(admit_min), out.ctypes.data_as(C.c_void_p),
+                                                               lens.ctypes.data_as(C.c_void_p), None if io is None else C.byref(io)),
+                 self._h)
         self.last_lengths = torch.from_numpy(lens)
-        return out[:, : int(lens.max()) + 1], lens
+        steps = int(lens.max())
+        if want_scores:
+            return out[:, : steps + 1], lens, logp[:, :steps], logit[:, :steps]
+        return out[:, : steps + 1], lens
 
     def stats(self) -> Dict[str, float]:
         s = _lib.Stats()

@@ -230,21 +230,24 @@ int b200t5_set_option(b200t5_handle h, const char* name, int value);
  * step runs it. */
 int b200t5_get_xattn_profile(b200t5_handle h, double* avg_us_per_launch, int64_t* launches, double* bytes_per_launch,
                              double* busy_us_per_layer, double* bytes_per_layer);
-/* lm_head + fused greedy arg-max exactly as the decode step runs them (csrc/gemm.cuh EpiArgmax -> finalize_step_kernel):
+/* lm_head + fused greedy arg-max exactly as the decode step runs them (csrc/gemm.cuh EpiLmHead<false, false> ->
+ * finalize_step_kernel<false, false>):
  * x [M,K] and W [V,K] in the build's 2-byte type (device), `step` the decode position, EOS masked while
  * step < min_new. tokens: int64 [M] (device) = argmax_n act(x . W[n]) with torch.argmax's first-index tie rule
  * (transformers generation/utils.py:2762,2793; logits_process.py:225-233). Test hook. */
 int b200t5_test_lm_argmax(int device, const void* x, const void* W, int M, int V, int K, int step, int eos, int min_new,
                           int64_t* tokens, void* stream);
-/* One decode step of lm_head + logits processors + arg-max as the step graph runs them (csrc/gemm.cuh EpiArgmaxProc ->
- * finalize_step_kernel): x [M,K] and W [V,K] as in b200t5_test_lm_argmax; hist int64 [M, step+1] (device) the decoder
- * ids so far (start token first), enc_ids int64 [M,S] (device) the prompts; eos is the EOS id when `logits` lists none.
+/* One decode step of lm_head + logits processors + arg-max as the step graph runs them (csrc/gemm.cuh
+ * EpiLmHead<true, false> -> finalize_step_kernel<true, false>, whatever `logits` holds): x [M,K] and W [V,K] as in
+ * b200t5_test_lm_argmax; hist int64 [M, step+1] (device) the decoder ids so far (start token first), enc_ids int64
+ * [M,S] (device) the prompts; eos is the EOS id when `logits` lists none.
  * tokens: int64 [M] (device); vals: fp32 [M,V] (device, may be NULL) the processed logits the arg-max ran on. Test hook;
  * both builds. */
 int b200t5_test_lm_process(int device, const void* x, const void* W, int M, int V, int K, int step, int eos, int min_new,
                            const b200t5_logits_params* logits, const int64_t* hist, const int64_t* enc_ids, int S,
                            int64_t* tokens, float* vals, void* stream);
-/* One decode step of a scored call as the step graph runs it (csrc/gemm.cuh EpiScore -> finalize_step_score_kernel):
+/* One decode step of a scored call as the step graph runs it (csrc/gemm.cuh EpiLmHead<kProc, true> ->
+ * finalize_step_kernel<kProc, true>, kProc when `logits` has an active processor):
  * arguments as b200t5_test_lm_process, where `logits`, hist and enc_ids may be NULL (no processors); forced int64 [M]
  * (device, may be NULL) the tokens to take instead of the arg-max. tokens int64 [M], logprob and logit fp32 [M]
  * (device): the token taken, its log-probability and its processed score; vals as in b200t5_test_lm_process.

@@ -360,7 +360,7 @@ def _argmax_case(lib, x, W, step, eos, min_new):
 
 def test_fused_argmax_lowest_index_tie_rule(lib):
     """torch.argmax returns the FIRST index among equal maxima (transformers generation/utils.py:2762,2793). The fused
-    path reduces in three places: inside a 32-column chunk, across the chunks of a 128-column tile (EpiArgmax),
+    path reduces in three places: inside a 32-column chunk, across the chunks of a 128-column tile (EpiLmHead),
     across tiles and warps (finalize_step_kernel). Exact ties are constructed in all of them, including across the
     last, partial tile of V = 32128 = 251 * 128 and against the masked EOS column."""
     K, V, M = 64, 32128, 160

@@ -1,4 +1,4 @@
-"""Greedy logits processors on the CUDA path (csrc/logits_process.cuh, EpiArgmaxProc): the fused kernel against
+"""Greedy logits processors on the CUDA path (csrc/logits_process.cuh, EpiLmHead<true, *>): the fused kernel against
 transformers' processor classes run by torch on the same GPU, the model against the numpy oracle and against HF
 generate, properties that need no reference, and the invariances of the three entry points."""
 import ctypes as C

@@ -1,5 +1,5 @@
-"""Token log-probabilities on the CUDA path (csrc/gemm.cuh EpiScore, finalize_step_score_kernel): the fused kernels
-against torch.log_softmax on the same GPU, the model against the numpy oracle and against transformers, and the
+"""Token log-probabilities on the CUDA path (csrc/gemm.cuh EpiLmHead<*, true>, finalize_step_kernel<*, true>): the fused
+kernels against torch.log_softmax on the same GPU, the model against the numpy oracle and against transformers, and the
 properties that need no reference: scoring changes no token and no launch of a plain call, every entry point returns the
 same bits, and teacher-forced score() of a generation returns the generation's own numbers."""
 import ctypes as C

@@ -6,6 +6,7 @@ three runs of each, and the processor kernels' share of the decode time from tor
 """
 import argparse
 import json
+import re
 import statistics
 import sys
 from pathlib import Path
@@ -19,6 +20,12 @@ from anyscale_workshop_nyc_2023_b200.synth import SPECS, synthetic_token_batch  
 from anyscale_workshop_nyc_2023_b200.workload import checkpoint_dir  # noqa: E402
 
 PROC = dict(repetition_penalty=1.2, no_repeat_ngram_size=3)
+# kernel-name patterns (demangled or mangled template arguments <kProc, kScore>) -> label
+TAGS = (("proc_reset_kernel", "proc_reset_kernel"),
+        (r"EpiLmHead(<true, false>|ILb1ELb0E)", "lm_head (EpiLmHead<true, false>)"),
+        (r"EpiLmHead(<false, false>|ILb0ELb0E)", "lm_head (EpiLmHead<false, false>)"),
+        (r"finalize_step_kernel(<true, false>|ILb1ELb0E)", "finalize_step_kernel<true, false>"),
+        (r"finalize_step_kernel(<false, false>|ILb0ELb0E)", "finalize_step_kernel<false, false>"))
 
 
 def main():
@@ -52,8 +59,8 @@ def main():
             res[name].append(ms)
             launches[name] = nl
     toks = a.batch * a.new
-    # share of the call's GPU time: proc_reset_kernel, the EpiArgmaxProc lm_head and finalize_step_kernel<true> (which
-    # computes the bans), against the same kernels of the plain step
+    # share of the call's GPU time: proc_reset_kernel, the lm_head with processors and finalize_step_kernel<true, false>
+    # (which computes the bans), against the same kernels of the plain step
     share = {}
     for name, kw in settings.items():
         with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
@@ -62,12 +69,8 @@ def main():
         for ev in prof.key_averages():
             t = ev.device_time_total if hasattr(ev, "device_time_total") else ev.cuda_time_total
             total += t
-            for tag in ("proc_reset_kernel", "EpiArgmaxProc", "EpiArgmax", "finalize_step_kernel"):
-                if tag in ev.key:
-                    proc_fin = "<true>" in ev.key or "ILb1E" in ev.key
-                    key = "finalize_step_kernel<true>" if tag == "finalize_step_kernel" and proc_fin else tag
-                    if tag == "EpiArgmax" and "EpiArgmaxProc" in ev.key:
-                        continue
+            for pat, key in TAGS:
+                if re.search(pat, ev.key):
                     parts[key] = parts.get(key, 0.0) + t
                     break
         share[name] = {k: v / total for k, v in parts.items()}

@@ -8,6 +8,7 @@ the numbers.
 """
 import argparse
 import json
+import re
 import statistics
 import subprocess
 import sys
@@ -22,9 +23,11 @@ from anyscale_workshop_nyc_2023_b200.synth import SPECS, synthetic_token_batch  
 from anyscale_workshop_nyc_2023_b200.workload import checkpoint_dir  # noqa: E402
 
 SCORED = dict(return_dict_in_generate=True, output_scores=True)
-# kernel-name fragments -> label; the scoring kernels first (their names contain the plain ones')
-TAGS = (("EpiScore", "lm_head (EpiScore)"), ("EpiArgmax", "lm_head (EpiArgmax)"),
-        ("finalize_step_score_kernel", "finalize_step_score_kernel"), ("finalize_step_kernel", "finalize_step_kernel"),
+# kernel-name patterns (demangled or mangled template arguments <kProc, kScore>) -> label
+TAGS = ((r"EpiLmHead(<false, true>|ILb0ELb1E)", "lm_head (EpiLmHead<false, true>)"),
+        (r"EpiLmHead(<false, false>|ILb0ELb0E)", "lm_head (EpiLmHead<false, false>)"),
+        (r"finalize_step_kernel(<false, true>|ILb0ELb1E)", "finalize_step_kernel<false, true>"),
+        (r"finalize_step_kernel(<false, false>|ILb0ELb0E)", "finalize_step_kernel<false, false>"),
         ("score_reset_kernel", "score_reset_kernel"))
 
 
@@ -79,7 +82,7 @@ def main():
             t = ev.device_time_total if hasattr(ev, "device_time_total") else ev.cuda_time_total
             total += t
             for frag, label in TAGS:
-                if frag in ev.key:
+                if re.search(frag, ev.key):
                     parts[label] = parts.get(label, 0.0) + t
                     break
         share[name] = {"gpu_ms": total / 1e3, **{k: {"ms": v / 1e3, "share": v / total} for k, v in parts.items()}}

@@ -160,7 +160,7 @@ def main():
             model.generate_stream(ids, mask, pool=8, max_new_tokens=4)
             del model
     if section("logits_process"):
-        # EpiArgmaxProc + finalize_step_kernel<true> + proc_reset_kernel through the hook (a V that is no multiple of
+        # EpiLmHead<true, false> + finalize_step_kernel<true, false> + proc_reset_kernel through the hook (a V that is no multiple of
         # 32 or 128, bans at the vocabulary's end), then one small generate and one slot-pool run with every processor
         M, V, K, S, step = 20, 1000, 64, 30, 4
         xa, Wv = rnd(M, K), rnd(V, K)
