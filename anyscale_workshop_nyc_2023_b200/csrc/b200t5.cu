@@ -127,12 +127,12 @@ __global__ void split_tf32_kernel(const float* __restrict__ w, float* __restrict
   out[static_cast<size_t>(r) * 2 * Kp + Kp + k] = tf32_rn(v - hi);
 }
 #endif
-// mode 0: the engine's path (table lookup); 1/2: op-by-op arithmetic with pow_mode 1/0
+// mode 0: the GeGLU epilogue's function (gemm.cuh gelu_epilogue); 1/2: op-by-op arithmetic with pow_mode 1/0
 __global__ void geglu_elementwise_kernel(const act_t* gate, const act_t* up, act_t* out, long long n, int mode, GeluLut lut) {
   long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
   if (i >= n) return;
   const float x = act2float(gate[i]);
-  const float g = mode == 0 ? gelu_from_lut(x, lut.table, lut.lo, lut.hi) : gelu_new_act_exact(x, mode == 1 ? 1 : 0);
+  const float g = mode == 0 ? gelu_epilogue(x, lut.table, lut.lo, lut.hi) : gelu_new_act_exact(x, mode == 1 ? 1 : 0);
   out[i] = float2act(g * act2float(up[i]));
 }
 __global__ void build_gelu_table_kernel(uint16_t* full, int pow_mode) {
@@ -2309,11 +2309,27 @@ extern "C" int b200t5_decode_logits(b200t5_handle h, const int64_t* input_ids, c
   return sms;
 }
 
+// The GeGLU epilogue's gelu table, built with `pow_mode`; the fp16 build evaluates gelu_new directly and has none.
+static int hook_gelu_lut(int pow_mode, GeluLut* lut) {
+#if B200T5_F16
+  (void)pow_mode;
+  *lut = GeluLut{nullptr, 0, 0};
+  return B200T5_OK;
+#else
+  return ensure_gelu_lut(nullptr, pow_mode, lut);
+#endif
+}
+
+// C (res_t, in/out) += the product, as one residual phase of the stream: mode 1 after the first feed-forward block,
+// mode 5 in layer 0 (fp16 build: the stream is still fp16 there, so the sum is rounded; bf16 build: same as mode 1).
+static EpiResidual::Params hook_residual(void* C, int N, int mode) {
+  EpiResidual::Params ep{static_cast<res_t*>(C), static_cast<const res_t*>(C), N};
+  if (mode == 5) ep.round_out = 1;
+  return ep;
+}
+
 extern "C" int b200t5_test_gemm(int device, const void* A, const void* W, void* C, int M, int N, int K, int bn, int mode,
                                 int pow_mode, void* stream) {
-#if B200T5_F16
-  return fail(nullptr, B200T5_EINVAL, "the single-kernel test hooks exist in the bf16 build only (libb200t5.so)");
-#else
   const int sms = hook_device(device);
   if (sms < 0) return sms;
   if (K % 8) return fail(nullptr, B200T5_EINVAL, "K must be a multiple of 8");
@@ -2328,14 +2344,14 @@ extern "C" int b200t5_test_gemm(int device, const void* A, const void* W, void* 
     if (mode == 0) {
       EpiStore::Params ep{Cb, N};
       e = run_gemm_2cta<EpiStore>(&dummy, ta, tb, M, N, K, ep, s);
-    } else if (mode == 1) {
-      EpiResidual::Params ep{Cb, Cb, N};
+    } else if (mode == 1 || mode == 5) {
+      const EpiResidual::Params ep = hook_residual(C, N, mode);
       e = run_gemm_2cta<EpiResidual>(&dummy, ta, tb, M, N, K, ep, s);
     } else if (mode == 2) {
       GeluLut lut;
-      int lrc = ensure_gelu_lut(nullptr, pow_mode, &lut);
+      int lrc = hook_gelu_lut(pow_mode, &lut);
       if (lrc != B200T5_OK) return lrc;
-      EpiGeglu::Params ep{Cb, N / 2, lut};
+      EpiGeglu::Params ep{static_cast<ffh_t*>(C), N / 2, lut};
       e = run_gemm_2cta<EpiGeglu>(&dummy, ta, tb, M, N, K, ep, s);
     }
     if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_gemm(pair, mode=%d): %s", mode, cudaGetErrorString(e));
@@ -2347,15 +2363,15 @@ extern "C" int b200t5_test_gemm(int device, const void* A, const void* W, void* 
     else if (bn == 32) e = run_gemm(&dummy, mk(ta, tb, M, N, K, G_STORE32, 1), &ep, s);
     else if (bn == 64) e = launch_gemm<64, EpiStore>(ta, tb, M, N, K, 0, ep, sms, s);
     else if (bn == 128) e = launch_gemm<128, EpiStore>(ta, tb, M, N, K, 0, ep, sms, s);
-  } else if (mode == 1) {
-    EpiResidual::Params ep{Cb, Cb, N};
+  } else if (mode == 1 || mode == 5) {
+    const EpiResidual::Params ep = hook_residual(C, N, mode);
     if (bn == 256) e = run_gemm(&dummy, mk(ta, tb, M, N, K, G_RES256, 0), &ep, s);
     else if (bn == 32) e = run_gemm(&dummy, mk(ta, tb, M, N, K, G_RES32, 1), &ep, s);
   } else if (mode == 2) {
     GeluLut lut;
-    int lrc = ensure_gelu_lut(nullptr, pow_mode, &lut);
+    int lrc = hook_gelu_lut(pow_mode, &lut);
     if (lrc != B200T5_OK) return lrc;
-    EpiGeglu::Params ep{Cb, N / 2, lut};
+    EpiGeglu::Params ep{static_cast<ffh_t*>(C), N / 2, lut};
     if (bn == 256) e = run_gemm(&dummy, mk(ta, tb, M, N, K, G_GEGLU256, 0), &ep, s);
     else if (bn == 64) e = run_gemm(&dummy, mk(ta, tb, M, N, K, G_GEGLU64, 1), &ep, s);
   } else if (mode == 3) {
@@ -2364,15 +2380,11 @@ extern "C" int b200t5_test_gemm(int device, const void* A, const void* W, void* 
   }
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_gemm(bn=%d, mode=%d): %s", bn, mode, cudaGetErrorString(e));
   return B200T5_OK;
-#endif
 }
 
 extern "C" int b200t5_test_enc_gemm(int device, const void* A, const void* W, void* C, int M, int N, int K, int kernel,
                                     int mode, int pow_mode, const int* row_b, const int* row_s, int B, int H, int S,
                                     void* stream) {
-#if B200T5_F16
-  return fail(nullptr, B200T5_EINVAL, "the single-kernel test hooks exist in the bf16 build only (libb200t5.so)");
-#else
   const int sms = hook_device(device);
   if (sms < 0) return sms;
   if (K % 8) return fail(nullptr, B200T5_EINVAL, "K must be a multiple of 8");
@@ -2390,14 +2402,14 @@ extern "C" int b200t5_test_enc_gemm(int device, const void* A, const void* W, vo
   if (mode == 0) {
     EpiStore::Params ep{Cb, N};
     e = run_gemm_2cta<EpiStore>(&dummy, ta, tb, M, N, K, ep, s);
-  } else if (mode == 1) {
-    EpiResidual::Params ep{Cb, Cb, N};
+  } else if (mode == 1 || mode == 5) {
+    const EpiResidual::Params ep = hook_residual(C, N, mode);
     e = run_gemm_2cta<EpiResidual>(&dummy, ta, tb, M, N, K, ep, s);
   } else if (mode == 2) {
     GeluLut lut;
-    int lrc = ensure_gelu_lut(nullptr, pow_mode, &lut);
+    int lrc = hook_gelu_lut(pow_mode, &lut);
     if (lrc != B200T5_OK) return lrc;
-    EpiGeglu::Params ep{Cb, N / 2, lut};
+    EpiGeglu::Params ep{static_cast<ffh_t*>(C), N / 2, lut};
     e = run_gemm_2cta<EpiGeglu>(&dummy, ta, tb, M, N, K, ep, s);
   } else if (mode == 3) {
     EpiCrossKV::Params ep{Cb, B, H, S, row_b, row_s};
@@ -2405,7 +2417,6 @@ extern "C" int b200t5_test_enc_gemm(int device, const void* A, const void* W, vo
   }
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_enc_gemm(kernel=%d, mode=%d): %s", kernel, mode, cudaGetErrorString(e));
   return B200T5_OK;
-#endif
 }
 
 // lm_head + the decode step's head exactly as chain_head launches it, for M rows at position `step`: the head with
@@ -2523,9 +2534,6 @@ extern "C" int b200t5_test_lm_score(int device, const void* x, const void* W, in
 
 extern "C" int b200t5_test_gemm_splitk(int device, const void* A, const void* W, void* C, int M, int N, int K, int bn,
                                        int split, int mode, int pow_mode, void* aux, int Tmax, int step, void* stream) {
-#if B200T5_F16
-  return fail(nullptr, B200T5_EINVAL, "the single-kernel test hooks exist in the bf16 build only (libb200t5.so)");
-#else
   const int sms = hook_device(device);
   if (sms < 0) return sms;
   if (K % 8) return fail(nullptr, B200T5_EINVAL, "K must be a multiple of 8");
@@ -2543,14 +2551,14 @@ extern "C" int b200t5_test_gemm_splitk(int device, const void* A, const void* W,
   if (mode == 0) {
     EpiStore::Params ep{Cb, N};
     e = run_gemm_sk<EpiStore>(&dummy, ch, ta, tb, M, N, K, ep, s, false);
-  } else if (mode == 1) {
-    EpiResidual::Params ep{Cb, Cb, N};
+  } else if (mode == 1 || mode == 5) {
+    const EpiResidual::Params ep = hook_residual(C, N, mode);
     e = run_gemm_sk<EpiResidual>(&dummy, ch, ta, tb, M, N, K, ep, s, false);
   } else if (mode == 2) {
     GeluLut lut;
-    int lrc = ensure_gelu_lut(nullptr, pow_mode, &lut);
+    int lrc = hook_gelu_lut(pow_mode, &lut);
     if (lrc != B200T5_OK) return lrc;
-    EpiGeglu::Params ep{Cb, N / 2, lut};
+    EpiGeglu::Params ep{static_cast<ffh_t*>(C), N / 2, lut};
     e = run_gemm_sk<EpiGeglu>(&dummy, ch, ta, tb, M, N, K, ep, s, false);
   } else if (mode == 4) {
     if (!aux || N % 192 || Tmax <= step) return fail(nullptr, B200T5_EINVAL, "test_gemm_splitk: bad QKV arguments");
@@ -2562,7 +2570,6 @@ extern "C" int b200t5_test_gemm_splitk(int device, const void* A, const void* W,
   }
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_gemm_splitk(bn=%d, split=%d, mode=%d): %s", bn, split, mode, cudaGetErrorString(e));
   return B200T5_OK;
-#endif
 }
 
 // fp16 build only: the fp32-weight feed-forward output projection, R += A . W^T, through the tf32 two-pass product
@@ -2604,34 +2611,34 @@ extern "C" int b200t5_test_ffo(int device, const void* A, const void* W, void* R
 }
 
 extern "C" int b200t5_test_rmsnorm(int device, const void* x, const void* w, void* y, int M, int d, float eps, void* stream) {
-#if B200T5_F16
-  return fail(nullptr, B200T5_EINVAL, "the single-kernel test hooks exist in the bf16 build only (libb200t5.so)");
-#else
   const int sms = hook_device(device);
   if (sms < 0) return sms;
-  cudaError_t e = run_rmsnorm(nullptr, static_cast<const act_t*>(x), static_cast<const act_t*>(w), static_cast<act_t*>(y), M, d, eps, static_cast<cudaStream_t>(stream));
+  cudaError_t e = run_rmsnorm(nullptr, static_cast<const res_t*>(x), static_cast<const act_t*>(w), static_cast<act_t*>(y), M, d, eps, static_cast<cudaStream_t>(stream));
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "rmsnorm: %s", cudaGetErrorString(e));
   return B200T5_OK;
-#endif
 }
 
 extern "C" int b200t5_test_attn_decode(int device, int self, const void* q, const void* K, const void* V, void* ctx,
                                        int B, int H, int Tk, const int32_t* extent, const uint8_t* key_ok, int step,
                                        const float* dist_bias, void* stream) {
-#if B200T5_F16
-  return fail(nullptr, B200T5_EINVAL, "the single-kernel test hooks exist in the bf16 build only (libb200t5.so)");
-#else
   const int sms = hook_device(device);
   if (sms < 0) return sms;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (self == 1) {
+  if (self == 1 || self == 3) {
+    // the position: `step` for every row (static batch), or extent[b] for row b (slot pool, step_stride 1)
     DevBuf st;
     if (st.alloc(sizeof(DecodeState)) != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "alloc");
     set_state_kernel<<<1, 1, 0, s>>>(st.as<DecodeState>(), step);
-    self_attn_decode_warp_kernel<<<(B * H + kSelfWarpsPerCta - 1) / kSelfWarpsPerCta, kSelfWarpsPerCta * 32,
-                                   kSelfWarpsPerCta * Tk * sizeof(float), s>>>(
-        static_cast<const act_t*>(q), static_cast<const act_t*>(K), static_cast<const act_t*>(V), static_cast<act_t*>(ctx),
-        B * H, H, Tk, &st.as<DecodeState>()->step, dist_bias);
+    const int* pos = extent ? extent : &st.as<DecodeState>()->step;
+    const int stride = extent ? 1 : 0;
+    const act_t *qa = static_cast<const act_t*>(q), *Ka = static_cast<const act_t*>(K), *Va = static_cast<const act_t*>(V);
+    if (self == 3)
+      attn_decode_kernel<true><<<B * H, kAttnDecThreads, Tk * sizeof(float), s>>>(
+          qa, Ka, Va, static_cast<act_t*>(ctx), H, Tk, nullptr, nullptr, pos, dist_bias, XsStamps{nullptr, 0}, stride);
+    else
+      self_attn_decode_warp_kernel<<<(B * H + kSelfWarpsPerCta - 1) / kSelfWarpsPerCta, kSelfWarpsPerCta * 32,
+                                     kSelfWarpsPerCta * Tk * sizeof(float), s>>>(qa, Ka, Va, static_cast<act_t*>(ctx), B * H, H, Tk,
+                                                                                 pos, dist_bias, stride);
     cudaStreamSynchronize(s);
   } else if (self == 2) {  // the TMA stream kernel (attention_cross_stream.cuh); `step` = ring stages (0: 5)
     const int stages = step > 0 ? step : 5;
@@ -2651,15 +2658,11 @@ extern "C" int b200t5_test_attn_decode(int device, int self, const void* q, cons
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "attn_decode: %s", cudaGetErrorString(e));
   return B200T5_OK;
-#endif
 }
 
 extern "C" int b200t5_test_encoder_attn(int device, const void* qkv, void* ctx, const float* rel_bias,
                                         const uint8_t* key_ok, const int32_t* extent, int B, int S, int H, int impl,
                                         void* stream) {
-#if B200T5_F16
-  return fail(nullptr, B200T5_EINVAL, "the single-kernel test hooks exist in the bf16 build only (libb200t5.so)");
-#else
   const int sms = hook_device(device);
   if (sms < 0) return sms;
   // impl 1: the packed-row addressing the encoder uses (prompt b at rows cu[b] = b * S, only its extent computed)
@@ -2679,22 +2682,17 @@ extern "C" int b200t5_test_encoder_attn(int device, const void* qkv, void* ctx, 
   }
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "encoder_attn: %s", cudaGetErrorString(e));
   return B200T5_OK;
-#endif
 }
 
 extern "C" int b200t5_test_geglu(int device, const void* gate, const void* up, void* out, int64_t n, int pow_mode, void* stream) {
-#if B200T5_F16
-  return fail(nullptr, B200T5_EINVAL, "the single-kernel test hooks exist in the bf16 build only (libb200t5.so)");
-#else
   const int sms = hook_device(device);
   if (sms < 0) return sms;
   GeluLut lut;
-  int lrc = ensure_gelu_lut(nullptr, 0, &lut);
+  int lrc = hook_gelu_lut(0, &lut);
   if (lrc != B200T5_OK) return lrc;
   geglu_elementwise_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const act_t*>(gate), static_cast<const act_t*>(up), static_cast<act_t*>(out), n, pow_mode, lut);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "geglu: %s", cudaGetErrorString(e));
   return B200T5_OK;
-#endif
 }

@@ -267,21 +267,25 @@ int b200t5_decode_logits(b200t5_handle h, const int64_t* input_ids, const int64_
 /* T5Attention._relative_position_bucket for one offset (host-only, no GPU needed). */
 int b200t5_relative_bucket(int relative_position, int bidirectional, int num_buckets, int max_distance);
 
-/* Single-kernel hooks: all pointers are device pointers, bf16 unless noted. */
-/* C[M,N] = bf16(A[M,K] W[N,K]^T) via the wgmma GEMM; mode 0 plain, 1 += residual R (in C),
- * 2 GeGLU (W rows interleaved per bn/2, C is [M,N/2]), 3 fp32 output (C is float*). bn in {32,64,128,256};
- * bn = 512 selects the encoder configuration (128 x 256 tiles, weight in 128-row boxes, GeGLU interleave per 128), modes 0-2. */
+/* Single-kernel hooks, in both builds: all pointers are device pointers. A 2-byte tensor is the build's activation
+ * type (bf16 in libb200t5.so, fp16 in libb200t5_f16.so) unless noted. In the fp16 build the residual stream (the
+ * residual C / R of the GEMMs, the RMSNorm input x) is fp32, and so is the GeGLU output (holding fp16 values). */
+/* C[M,N] = act(A[M,K] W[N,K]^T) via the wgmma GEMM; mode 0 plain, 1 += residual R (in C), 5 += residual as in
+ * decoder / encoder layer 0 (fp16 build: C = fp16(R + fp16(acc)), where mode 1 is C = R + fp16(acc); bf16 build:
+ * same as 1), 2 GeGLU (W rows interleaved per bn/2, C is [M,N/2]), 3 fp32 output (C is float*). bn in {32,64,128,256};
+ * bn = 512 selects the encoder configuration (128 x 256 tiles, weight in 128-row boxes, GeGLU interleave per 128),
+ * modes 0, 1, 2, 5. pow_mode: the gelu table's (bf16 build; the fp16 build's epilogue has no table). */
 int b200t5_test_gemm(int device, const void* A, const void* W, void* C, int M, int N, int K, int bn, int mode,
                      int pow_mode, void* stream);
 /* The 128 x 256 encoder GEMM as the encoder launches it; kernel 0 = the kernel whose epilogue follows each main loop,
- * 1 = the epilogue-overlapped kernel (option "enc_gemm"). mode 0 plain, 1 += residual R (in C), 2 GeGLU (W rows
+ * 1 = the epilogue-overlapped kernel (option "enc_gemm"). mode 0 plain, 1 and 5 += residual R (in C), 2 GeGLU (W rows
  * interleaved per 128, C is [M,N/2]), 3 cross-attention K/V scatter: C is the arena [N/(H*64)][B][H][S][64] and row m
  * is position row_s[m] of prompt row_b[m] (both NULL: m = b*S + s, M = B*S). B, H, S are read in mode 3 only. */
 int b200t5_test_enc_gemm(int device, const void* A, const void* W, void* C, int M, int N, int K, int kernel, int mode,
                          int pow_mode, const int* row_b, const int* row_s, int B, int H, int S, void* stream);
 /* Same contract through the cluster split-K kernel the decode step uses (csrc/gemm_splitk.cuh):
  * bn in {64,128}; split in {1,2,4,8} CTAs per cluster along K (reduced automatically when K has
- * fewer 64-wide k-blocks); mode 0 plain, 1 += residual (in C), 2 GeGLU, 4 decoder QKV: C is the q
+ * fewer 64-wide k-blocks); mode 0 plain, 1 and 5 += residual (in C), 2 GeGLU, 4 decoder QKV: C is the q
  * buffer [M, N/3] and `aux` the self-KV cache [2][M][H][Tmax][64] whose row `step` is written. */
 int b200t5_test_gemm_splitk(int device, const void* A, const void* W, void* C, int M, int N, int K, int bn, int split,
                             int mode, int pow_mode, void* aux, int Tmax, int step, void* stream);
@@ -292,7 +296,9 @@ int b200t5_test_gemm_splitk(int device, const void* A, const void* W, void* C, i
 int b200t5_test_ffo(int device, const void* A, const void* W, void* R, int M, int N, int F, int kernel, int bn, int split,
                     void* stream);
 int b200t5_test_rmsnorm(int device, const void* x, const void* w, void* y, int M, int d, float eps, void* stream);
-/* self == 1: keys = step+1, dist_bias float [H][Tk]; self == 0: extent int32 [B], key_ok uint8 [B][Tk];
+/* Decoder self-attention: self == 3 the 4-warp-per-(row, head) kernel the decode step runs, self == 1 the one-warp
+ * variant (B200T5_SELF=warp); keys = t+1 with t = step, or, when extent is not NULL, t = extent[b] (int32 [B]: the
+ * slot pool's per-row positions); dist_bias float [H][Tk]. Cross-attention: self == 0: extent int32 [B], key_ok uint8 [B][Tk];
  * self == 2: as 0 through the TMA stream kernel (csrc/attention_cross_stream.cuh), `step` = ring stages (0: 5);
  * same rounding points as self == 0, the fp32 accumulations in the tensor core's order. */
 int b200t5_test_attn_decode(int device, int self, const void* q, const void* K, const void* V, void* ctx, int B,
@@ -302,8 +308,9 @@ int b200t5_test_attn_decode(int device, int self, const void* q, const void* K, 
  * cu[b] = b * S), where query rows >= extent[b] are not written. */
 int b200t5_test_encoder_attn(int device, const void* qkv, void* ctx, const float* rel_bias, const uint8_t* key_ok,
                              const int32_t* extent, int B, int S, int H, int impl, void* stream);
-/* out[i] = bf16(gelu_new(gate[i]) * up[i]). mode 0: the GeGLU epilogue's path (exhaustive gelu table);
- * mode 2: the op-by-op bf16 arithmetic the table is built from; mode 1: same with single-rounded pow. */
+/* out[i] = act(gelu_new(gate[i]) * up[i]). mode 0: exactly the GeGLU epilogue's function (bf16 build: the exhaustive
+ * gelu table; fp16 build: the op-by-op fp16 arithmetic with single-rounded pow); mode 2: the op-by-op arithmetic with
+ * double-rounded pow (x*x*x in act_t); mode 1: same with single-rounded pow. */
 int b200t5_test_geglu(int device, const void* gate, const void* up, void* out, int64_t n, int pow_mode,
                       void* stream);
 
