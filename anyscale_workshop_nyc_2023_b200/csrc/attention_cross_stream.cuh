@@ -99,15 +99,13 @@ DEVINL void xs_release_slot(uint64_t* bar, float last_acc) {
 __global__ void __maxnreg__(64)
 attn_cross_stream_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                          int k_row0, int v_row0,
-                         const act_t* __restrict__ kplane,  // = row k_row0 of tmK's tensor (L2 prefetch of whole slabs)
-                         const act_t* __restrict__ vplane,  // = row v_row0 of tmV's tensor
                          const act_t* __restrict__ q,    // [B, H*64]
                          act_t* __restrict__ ctx,        // [B, H*64]
                          int n_items,                    // B * H
                          int H, int Tk,
                          const int* __restrict__ extent,            // [B] keys to visit (0 = retired row)
                          const unsigned char* __restrict__ key_ok,  // [B][Tk] 1 = attended
-                         int stages, int late_pdl, int l2_prefetch, XsStamps stamps) {
+                         int stages, XsStamps stamps) {
   extern __shared__ uint8_t xs_raw[];
   uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(xs_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* s_mask = ring + static_cast<size_t>(stages) * kXsChunkBytes;          // [stages][64]
@@ -130,12 +128,11 @@ attn_cross_stream_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_c
     mbar_fence_init();
   }
   __syncthreads();
-  // late_pdl = 0: the dependent kernel (this chain's cross-attention output projection) may start its prologue at
-  // once, as everywhere else in the step. late_pdl = 1: its CTAs would only sit on their SMs (~140 KB of shared
-  // memory each) while this kernel streams, in the way of the OTHER chain's GEMMs: release them when this CTA
-  // starts its LAST item, so that the prologue overlaps the tail of the stream only.
-  if (!late_pdl) pdl_launch_dependents();
-  // everything above overlapped the previous kernel's tail; q / extent are that kernel's (or the previous step's) output
+  // The dependent kernel (this chain's cross-attention output projection) is released when this CTA starts its LAST
+  // item, not at once as everywhere else in the step: its CTAs would only sit on their SMs (~140 KB of shared memory
+  // each) while this kernel streams, in the way of the OTHER chain's GEMMs, so its prologue overlaps the tail of the
+  // stream only.
+  // Everything above overlapped the previous kernel's tail; q / extent are that kernel's (or the previous step's) output
   pdl_wait();
   unsigned long long t_start = 0;
   if (stamps.slots != nullptr && threadIdx.x == 0) t_start = global_timer_ns();
@@ -152,27 +149,12 @@ attn_cross_stream_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_c
       int stage = 0;
       uint32_t phase = 0;
       int n_next = first < n_items ? extent[first / H] : 0;
-      // The ring alone (2 CTAs x `stages` x 8 KB per SM, what fits next to a GEMM CTA) cannot cover the latency of
-      // DRAM under a saturating stream (~2.7 us: the per-thread-load kernel keeps ~114 KB per SM in flight): the
-      // HBM -> L2 leg is therefore driven one whole item ahead by L2 prefetches of the next item's K and V slabs (two
-      // instructions per item, no shared memory, no completion tracking), and the ring only has to cover an L2 hit.
-      auto prefetch_item = [&](int it, int n) {
-        if (l2_prefetch && n > 0) {
-          const uint64_t keep = l2_policy_evict_last();
-          prefetch_l2_bulk(kplane + static_cast<size_t>(it) * Tk * 64, static_cast<uint32_t>(n) * 128u, keep);
-          prefetch_l2_bulk(vplane + static_cast<size_t>(it) * Tk * 64, static_cast<uint32_t>(n) * 128u, keep);
-        }
-      };
-      if (first < n_items) prefetch_item(first, n_next);
       for (int it = first; it < n_items; it += stride) {
         const int b = it / H;
         const int n = n_next;
         // (the next item's extent is fetched a whole item ahead: the ring holds < 2 us of stream, an L2 round trip
         // under load is of that order)
-        if (it + stride < n_items) {
-          n_next = extent[(it + stride) / H];
-          prefetch_item(it + stride, n_next);
-        }
+        if (it + stride < n_items) n_next = extent[(it + stride) / H];
 #pragma unroll 1
         for (int kv = 0; kv < 2; ++kv) {
           const CUtensorMap* tm = kv ? &tmV : &tmK;
@@ -228,7 +210,7 @@ attn_cross_stream_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_c
       q_next = fetch_q(nxt);
       nn = extent[nxt / H];
     }
-    if (late_pdl && it == last_item) pdl_launch_dependents();
+    if (it == last_item) pdl_launch_dependents();
     xs_bar_sync();  // s_q visible (and the previous item's s_p / s_scores no longer read)
     // B operand of Q K^T: q in column 0, i.e. in the lanes of group 0
     uint32_t qb[8];
@@ -323,7 +305,7 @@ attn_cross_stream_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_c
       dst[8] = float2act(o[2]);
     }
   }
-  if (late_pdl && first >= n_items) pdl_launch_dependents();
+  if (first >= n_items) pdl_launch_dependents();  // no item
   if (stamps.slots != nullptr && threadIdx.x == 0) {
     atomicMin(&stamps.slots[2 * stamps.slot], t_start);
     atomicMax(&stamps.slots[2 * stamps.slot + 1], static_cast<unsigned long long>(global_timer_ns()));

@@ -190,125 +190,4 @@ attn_decode_kernel(const act_t* __restrict__ q,    // [B, H*64]
   }
 }
 
-// ---------------------------------------------------------------- self-attention, one warp per (b,h)
-// The decoder's own cache holds at most max_new_tokens (128) keys: a (b,h) problem is 16-32 KB,
-// so a whole CTA with block-wide barriers is mostly overhead. Here each warp owns one (b,h):
-// same arithmetic and rounding points as attn_decode_kernel<true>, only warp-level syncs.
-constexpr int kSelfWarpsPerCta = 4;
-
-// One (row, head) item handled by one warp; `sc` is this warp's score scratch (Tk floats of shared memory).
-// kNc: read K/V through the non-coherent path (stand-alone kernel: the cache rows were written by an earlier
-// kernel) or with plain loads (resident kernel: they may have been written by another CTA in the same launch).
-template <bool kNc>
-DEVINL void self_attn_warp_item(const act_t* __restrict__ q, const act_t* __restrict__ Kc,
-                                const act_t* __restrict__ Vc, act_t* __restrict__ ctx, int bh, int H, int Tk,
-                                int t, const float* __restrict__ dist_bias, float* sc) {
-  const int lane = threadIdx.x & 31;
-  const int h = bh % H;
-  const int ks = lane >> 3, dg = lane & 7;
-  const int nkeys = t + 1;
-  const size_t slab = static_cast<size_t>(bh) * Tk * 64;
-  const act_t* Kp = Kc + slab + dg * 8;
-  const act_t* Vp = Vc + slab + dg * 8;
-  auto load16 = [](const act_t* p) -> uint4 {
-    if constexpr (kNc) return ldg_nc_v4(p);
-    else return *reinterpret_cast<const uint4*>(p);
-  };
-  float qf[8];
-  {
-    const uint4 qv = *reinterpret_cast<const uint4*>(q + static_cast<size_t>(bh) * 64 + dg * 8);
-    qf[0] = act_lo(qv.x); qf[1] = act_hi(qv.x); qf[2] = act_lo(qv.y); qf[3] = act_hi(qv.y);
-    qf[4] = act_lo(qv.z); qf[5] = act_hi(qv.z); qf[6] = act_lo(qv.w); qf[7] = act_hi(qv.w);
-  }
-  constexpr int U = 4;
-  for (int jb = 0; jb < nkeys; jb += 4 * U) {
-    uint4 kv[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int j = jb + ks + 4 * u;
-      kv[u] = j < nkeys ? load16(Kp + static_cast<size_t>(j) * 64) : make_uint4(0, 0, 0, 0);
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int j = jb + ks + 4 * u;
-      float s = dot8(kv[u], qf);
-      s += __shfl_xor_sync(0xffffffffu, s, 1);
-      s += __shfl_xor_sync(0xffffffffu, s, 2);
-      s += __shfl_xor_sync(0xffffffffu, s, 4);
-      if (dg == 0 && j < nkeys) sc[j] = act_round(act_round(s) + dist_bias[h * Tk + (t - j)]);
-    }
-  }
-  __syncwarp();
-  float mx = -INFINITY;
-  for (int j = lane; j < nkeys; j += 32) mx = fmaxf(mx, sc[j]);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  float sum = 0.f;
-  for (int j = lane; j < nkeys; j += 32) {
-    const float e = expf(sc[j] - mx);
-    sc[j] = e;
-    sum += e;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  for (int j = lane; j < nkeys; j += 32) sc[j] = act_round(sc[j] / sum);
-  __syncwarp();
-  float acc[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) acc[e] = 0.f;
-  for (int jb = 0; jb < nkeys; jb += 4 * U) {
-    uint4 vv[U];
-    float p[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int j = jb + ks + 4 * u;
-      const bool ok = j < nkeys;
-      vv[u] = ok ? load16(Vp + static_cast<size_t>(j) * 64) : make_uint4(0, 0, 0, 0);
-      p[u] = ok ? sc[j] : 0.f;
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      acc[0] = fmaf(p[u], act_lo(vv[u].x), acc[0]);
-      acc[1] = fmaf(p[u], act_hi(vv[u].x), acc[1]);
-      acc[2] = fmaf(p[u], act_lo(vv[u].y), acc[2]);
-      acc[3] = fmaf(p[u], act_hi(vv[u].y), acc[3]);
-      acc[4] = fmaf(p[u], act_lo(vv[u].z), acc[4]);
-      acc[5] = fmaf(p[u], act_hi(vv[u].z), acc[5]);
-      acc[6] = fmaf(p[u], act_lo(vv[u].w), acc[6]);
-      acc[7] = fmaf(p[u], act_hi(vv[u].w), acc[7]);
-    }
-  }
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    acc[e] += __shfl_xor_sync(0xffffffffu, acc[e], 8);
-    acc[e] += __shfl_xor_sync(0xffffffffu, acc[e], 16);
-  }
-  if (ks == 0) {
-    uint4 o;
-    o.x = pack_act2(acc[0], acc[1]);
-    o.y = pack_act2(acc[2], acc[3]);
-    o.z = pack_act2(acc[4], acc[5]);
-    o.w = pack_act2(acc[6], acc[7]);
-    *reinterpret_cast<uint4*>(ctx + static_cast<size_t>(bh) * 64 + dg * 8) = o;
-  }
-  __syncwarp();
-}
-
-__global__ void __launch_bounds__(kSelfWarpsPerCta * 32)
-self_attn_decode_warp_kernel(const act_t* __restrict__ q,   // [B, H*64]
-                             const act_t* __restrict__ Kc,  // [B][H][Tk][64]
-                             const act_t* __restrict__ Vc,
-                             act_t* __restrict__ ctx,       // [B, H*64]
-                             int BH, int H, int Tk, const int* __restrict__ step,
-                             const float* __restrict__ dist_bias,    // [H][Tk]
-                             const int step_stride = 0) {            // 1 = slot pool: per-row positions
-  extern __shared__ float s_all[];  // kSelfWarpsPerCta * Tk floats
-  pdl_launch_dependents();
-  pdl_wait();
-  const int warp = threadIdx.x >> 5;
-  const int bh = blockIdx.x * kSelfWarpsPerCta + warp;
-  if (bh >= BH) return;
-  self_attn_warp_item<true>(q, Kc, Vc, ctx, bh, H, Tk, step[(bh / H) * step_stride], dist_bias, s_all + warp * Tk);
-}
-
 }  // namespace b200

@@ -178,20 +178,9 @@ struct DevBuf {
   }
 };
 
-// Which epilogue/tile a GEMM uses.
-enum GemmKind { G_STORE256, G_RES256, G_GEGLU256, G_CROSSKV256, G_QKVDEC64, G_STORE32, G_RES32, G_GEGLU64, G_LOGITS128 };
-
-struct GemmOp {
-  CUtensorMap tmA, tmB;
-  int M = 0, N = 0, K = 0;
-  GemmKind kind = G_STORE256;
-  int m_fastest = 0;
-};
-
 struct EncLayerW {
   DevBuf ln0, ln1, wqkv, wo, wi, wff_o;  // wi interleaved for BN=256
-  CUtensorMap tm_qkv, tm_o, tm_wi, tm_ffo;
-  CUtensorMap tm2_qkv, tm2_o, tm2_wi, tm2_ffo;  // box of 128 weight rows: each CTA of a pair stages half of a 256-wide tile
+  CUtensorMap tm_qkv, tm_o, tm_wi, tm_ffo;  // box of 128 weight rows: a 256-wide weight tile is loaded as two boxes
 };
 struct DecLayerW {
   DevBuf ln0, ln1, ln2, wqkv, wo, wcq, wco, wi, wff_o;  // wi interleaved per N-tile of the decode wi GEMM
@@ -385,7 +374,7 @@ struct b200t5_ctx {
   std::map<std::string, std::unique_ptr<DevBuf>> raw_f32;  // fp16 build: fp32 copies of the `wo` weights
   std::map<std::string, std::vector<int64_t>> raw_shape;
   DevBuf shared, lm_head, enc_final_ln, dec_final_ln, enc_relbias, dec_relbias, wcrosskv;
-  CUtensorMap tm_lm, tm_crosskv, tm2_crosskv;
+  CUtensorMap tm_lm, tm_crosskv;
   std::vector<float> enc_relbias_h, dec_relbias_h;  // [nb][H] as float
   std::vector<EncLayerW> enc;
   std::vector<DecLayerW> dec;
@@ -395,22 +384,16 @@ struct b200t5_ctx {
   bool admit_overlap = true;  // B200T5_ADMIT_OVERLAP=0: admission encoder passes on the decode stream (round-1 behaviour)
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
   bool ev_valid = false;
-  int pow_mode = 0;
   bool use_pdl = true;
   GeluLut gelu_lut{nullptr, 0, 0};
   // decode GEMMs: cluster split-K tiles (gemm_splitk.cuh). {BN, wanted split} per product;
-  // B200T5_SK=0 selects the persistent kernel instead, B200T5_SK="bn,s,bn,s,bn,s,bn,s" overrides
-  // (order: qkv, attention projections o/cq/co, wi, ffo).
+  // B200T5_SK="bn,s,bn,s,bn,s,bn,s" overrides (order: qkv, attention projections o/cq/co, wi, ffo).
   struct SkChoice {
     int bn, split;
   };
-  bool pack_rows = true;  // encoder on the valid rows only (variable-length packing); B200T5_PACK=0: all B*S rows as the reference does
-  bool use_2cta = true;   // encoder GEMMs on the 128 x 256 tile configuration (gemm_2cta.cuh); B200T5_2CTA=0 selects the G_*256 kernels
   // 128 x 256 encoder GEMMs through gemm_enc_ws_kernel (epilogue warps overlap the next tile's main loop) rather than
   // gemm_bf16_tn_kernel; bit-identical results. B200T5_ENC_GEMM, option "enc_gemm" 0|1.
   bool enc_gemm_ws = true;
-  bool self_block = true;  // decoder self-attention with a 4-warp CTA per (row, head): two memory round trips whatever t is
-                           // B200T5_SELF=warp selects one warp per (row, head)
   // Cross-attention of the decode step: the TMA-ring + mma.sync stream kernel (attention_cross_stream.cuh: small
   // footprint, shares the SMs with the other chain's GEMM CTAs; meant for batches whose prompts fill the window) or the
   // per-thread-load kernel (attention_decode.cuh: one short-lived CTA per (row, head), several per SM; meant for
@@ -419,13 +402,7 @@ struct b200t5_ctx {
   // "xattn" 0|1|2. The kernels differ only in the order of their fp32 accumulations (same tokens up to near-ties).
   int xattn_mode = 2;
   int xs_stages = 5;        // 8 KB ring stages per CTA (two CTAs per SM): B200T5_XS_STAGES
-  bool xs_late_pdl = true;  // release the dependent GEMM when a CTA starts its last item instead of at once: B200T5_XS_LATE_PDL
-  bool xs_l2_prefetch = false;   // drive HBM -> L2 one item ahead with bulk L2 prefetches (B200T5_XS_L2PF, "xattn_l2pf")
-  bool xattn_serialize = false;  // one cross-attention kernel at a time across the chains (B200T5_XS_SERIALIZE, "xattn_serialize")
-  std::vector<cudaEvent_t> xattn_ev;
   bool profile_xattn = false;  // b200t5_set_option("profile_xattn"): stamp every cross-attention launch inside the step graph
-  int small_prio = 0;  // B200T5_PRIO: launch priority of the latency-bound decode kernels (see launch_priority())
-  bool sk_on = true;
   int sk_stages64 = 0, sk_stages128 = 0;  // pipeline stages of the split-K tiles (0 = default 4 / 3): B200T5_SK_STAGES="a,b"
   SkChoice sk_qkv{64, 2}, sk_proj{64, 4}, sk_wi{128, 2}, sk_ffo{64, 4};  // split-K choices per product (tools/sweep_decode.py)
   int chains_override = 0;
@@ -485,31 +462,6 @@ extern "C" int b200t5_relative_bucket(int rel, int bidirectional, int num_bucket
 }
 
 // ================================================================== GEMM dispatch
-static cudaError_t run_gemm(b200t5_ctx* h, const GemmOp& g, const void* ep, cudaStream_t s, bool pdl = false) {
-  h->launches++;
-  switch (g.kind) {
-    case G_STORE256:
-      return launch_gemm<256, EpiStore>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiStore::Params*>(ep), h->num_sms, s, pdl);
-    case G_RES256:
-      return launch_gemm<256, EpiResidual>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiResidual::Params*>(ep), h->num_sms, s, pdl);
-    case G_GEGLU256:
-      return launch_gemm<256, EpiGeglu>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiGeglu::Params*>(ep), h->num_sms, s, pdl);
-    case G_CROSSKV256:
-      return launch_gemm<256, EpiCrossKV>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiCrossKV::Params*>(ep), h->num_sms, s, pdl);
-    case G_QKVDEC64:
-      return launch_gemm<64, EpiQkvDecode>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiQkvDecode::Params*>(ep), h->num_sms, s, pdl);
-    case G_STORE32:
-      return launch_gemm<32, EpiStore>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiStore::Params*>(ep), h->num_sms, s, pdl);
-    case G_RES32:
-      return launch_gemm<32, EpiResidual>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiResidual::Params*>(ep), h->num_sms, s, pdl);
-    case G_GEGLU64:
-      return launch_gemm<64, EpiGeglu>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiGeglu::Params*>(ep), h->num_sms, s, pdl);
-    case G_LOGITS128:
-      return launch_gemm<128, EpiStoreF32>(g.tmA, g.tmB, g.M, g.N, g.K, g.m_fastest, *static_cast<const EpiStoreF32::Params*>(ep), h->num_sms, s, pdl);
-  }
-  return cudaErrorInvalidValue;
-}
-
 // The decode step's head, indexed [kProc][kScore]: the lm_head GEMM with its fused epilogue (gemm.cuh: EpiLmHead) and
 // the kernel that merges the epilogue's partials (elementwise.cuh: finalize_step_kernel).
 struct LmHead {
@@ -585,12 +537,7 @@ static cudaError_t run_rmsnorm(b200t5_ctx* h, const res_t* x, const act_t* w, ac
 
 static cudaError_t init_kernel_attrs() {
   cudaError_t e;
-#define PREP(BN, EPI)                         \
-  if ((e = prepare_gemm<BN, EPI>()) != cudaSuccess) return e;
-  PREP(256, EpiStore) PREP(256, EpiResidual) PREP(256, EpiGeglu) PREP(256, EpiCrossKV) PREP(64, EpiQkvDecode)
-  PREP(32, EpiStore) PREP(32, EpiResidual) PREP(64, EpiGeglu) PREP(128, EpiStoreF32)
-  PREP(64, EpiStore) PREP(128, EpiStore)
-#undef PREP
+  if ((e = prepare_gemm<128, EpiStoreF32>()) != cudaSuccess) return e;
   for (const auto& row : kLmHeads)
     for (const LmHead& lh : row)
       if ((e = lh.prepare()) != cudaSuccess) return e;
@@ -610,9 +557,6 @@ static cudaError_t init_kernel_attrs() {
   if ((e = prepare_gemm_2cta<EpiResidual, B200T5_F16 != 0>()) != cudaSuccess) return e;
   if ((e = prepare_gemm_splitk<64, EpiResidual, B200T5_F16 != 0>()) != cudaSuccess) return e;
   if ((e = prepare_gemm_splitk<128, EpiResidual, B200T5_F16 != 0>()) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(self_attn_decode_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                kSelfWarpsPerCta * 4096 * 4)) != cudaSuccess)
-    return e;
   if ((e = cudaFuncSetAttribute(attn_cross_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 static_cast<int>(XsSmem::bytes(kXsMaxStages, 4096)))) != cudaSuccess)
     return e;
@@ -694,28 +638,17 @@ extern "C" int b200t5_create(const b200t5_config* cfg, int device, b200t5_handle
   h->num_sms = sms;
   h->enc.resize(h->c.Le);
   h->dec.resize(h->c.Ld);
-  const char* pm = getenv("B200T5_POW_MODE");
-  h->pow_mode = pm ? atoi(pm) : 0;
   const char* pdl_env = getenv("B200T5_PDL");
   h->use_pdl = pdl_env ? atoi(pdl_env) != 0 : true;
-  if (const char* pr_env = getenv("B200T5_PRIO")) h->small_prio = atoi(pr_env);
-  if (const char* pk_env = getenv("B200T5_PACK")) h->pack_rows = atoi(pk_env) != 0;
-  if (const char* tc_env = getenv("B200T5_2CTA")) h->use_2cta = atoi(tc_env) != 0;
   if (const char* eg_env = getenv("B200T5_ENC_GEMM")) h->enc_gemm_ws = atoi(eg_env) != 0;
-  if (const char* sf_env = getenv("B200T5_SELF")) h->self_block = strcmp(sf_env, "warp") != 0;
   if (const char* xa_env = getenv("B200T5_XATTN")) h->xattn_mode = strcmp(xa_env, "ldg") == 0 ? 0 : strcmp(xa_env, "stream") == 0 ? 1 : 2;
   if (const char* xs_env = getenv("B200T5_XS_STAGES")) {
     const int v = atoi(xs_env);
     if (v >= 2 && v <= kXsMaxStages) h->xs_stages = v;
   }
-  if (const char* lp_env = getenv("B200T5_XS_LATE_PDL")) h->xs_late_pdl = atoi(lp_env) != 0;
-  if (const char* se_env = getenv("B200T5_XS_SERIALIZE")) h->xattn_serialize = atoi(se_env) != 0;
-  if (const char* pf_env = getenv("B200T5_XS_L2PF")) h->xs_l2_prefetch = atoi(pf_env) != 0;
   if (const char* sk_env = getenv("B200T5_SK")) {
     int v[8];
-    const int n = sscanf(sk_env, "%d,%d,%d,%d,%d,%d,%d,%d", &v[0], &v[1], &v[2], &v[3], &v[4], &v[5], &v[6], &v[7]);
-    if (n == 1 && v[0] == 0) h->sk_on = false;
-    if (n == 8) {
+    if (sscanf(sk_env, "%d,%d,%d,%d,%d,%d,%d,%d", &v[0], &v[1], &v[2], &v[3], &v[4], &v[5], &v[6], &v[7]) == 8) {
       b200t5_ctx::SkChoice* dst[4] = {&h->sk_qkv, &h->sk_proj, &h->sk_wi, &h->sk_ffo};
       for (int i = 0; i < 4; ++i) {
         dst[i]->bn = v[2 * i] == 128 ? 128 : 64;
@@ -732,15 +665,6 @@ extern "C" int b200t5_create(const b200t5_config* cfg, int device, b200t5_handle
   }
   const char* ch_env = getenv("B200T5_CHAINS");
   h->chains_override = ch_env ? atoi(ch_env) : 0;
-#if B200T5_F16
-  // the fp16 build implements the default kernel set only (the measured-slower experiments and the fallbacks
-  // they replace assume the bf16 contract: 2-byte residual stream, table-driven gelu)
-  h->use_2cta = h->pack_rows = true;
-  if (!h->sk_on) {
-    delete h;
-    return fail(nullptr, B200T5_EINVAL, "B200T5_SK=0 is not available in the fp16 build");
-  }
-#endif
   if (const char* ao_env = getenv("B200T5_ADMIT_OVERLAP")) h->admit_overlap = atoi(ao_env) != 0;
   int prio_lo = 0, prio_hi = 0;
   cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);  // (lowest, highest)
@@ -761,7 +685,7 @@ extern "C" int b200t5_create(const b200t5_config* cfg, int device, b200t5_handle
   }
 #if !B200T5_F16  // (the fp16 build evaluates gelu_new directly; the table indexes bf16 bit patterns)
   {
-    int lrc = ensure_gelu_lut(nullptr, h->pow_mode, &h->gelu_lut);
+    int lrc = ensure_gelu_lut(nullptr, 0, &h->gelu_lut);
     if (lrc != B200T5_OK) {
       delete h;
       return lrc;
@@ -796,8 +720,6 @@ extern "C" int b200t5_destroy(b200t5_handle h) {
     if (h->chain_streams[i]) cudaStreamDestroy(h->chain_streams[i]);
   for (int i = 0; i <= kMaxChains; ++i)
     if (h->chain_ev[i]) cudaEventDestroy(h->chain_ev[i]);
-  for (cudaEvent_t e : h->xattn_ev)
-    if (e) cudaEventDestroy(e);
   for (int i = 0; i < 4; ++i)
     if (h->ev[i]) cudaEventDestroy(h->ev[i]);
   delete h;
@@ -984,14 +906,10 @@ extern "C" int b200t5_finalize(b200t5_handle h) {
     TRY(interleave_geglu(h, wi0, wi1, w.wi, F, d, 256, &wi_rows));
     if (!(p = take(h, key("layer.1.DenseReluDense.wo.weight"), d, F, &rc))) return rc;
     TRY(build_ffo(h, w.wff_o, key("layer.1.DenseReluDense.wo.weight"), p, d, F, &h->ffo_k));
-    TMAP(h, &w.tm_qkv, w.wqkv.p, 3 * I, d, 256);
-    TMAP(h, &w.tm_o, w.wo.p, d, I, 256);
-    TMAP(h, &w.tm_wi, w.wi.p, wi_rows, d, 256);
-    TMAP_FFO(h, &w.tm_ffo, w.wff_o.p, d, h->ffo_k, 256);
-    TMAP(h, &w.tm2_qkv, w.wqkv.p, 3 * I, d, 128);
-    TMAP(h, &w.tm2_o, w.wo.p, d, I, 128);
-    TMAP(h, &w.tm2_wi, w.wi.p, wi_rows, d, 128);
-    TMAP_FFO(h, &w.tm2_ffo, w.wff_o.p, d, h->ffo_k, 128);
+    TMAP(h, &w.tm_qkv, w.wqkv.p, 3 * I, d, k2ctaBox);
+    TMAP(h, &w.tm_o, w.wo.p, d, I, k2ctaBox);
+    TMAP(h, &w.tm_wi, w.wi.p, wi_rows, d, k2ctaBox);
+    TMAP_FFO(h, &w.tm_ffo, w.wff_o.p, d, h->ffo_k, k2ctaBox);
   }
 
   CU_OK(h, h->wcrosskv.alloc(static_cast<size_t>(c.Ld) * 2 * I * d * sizeof(act_t)));
@@ -1031,9 +949,8 @@ extern "C" int b200t5_finalize(b200t5_handle h) {
     const act_t* wi1 = wi0 ? take(h, key("layer.2.DenseReluDense.wi_1.weight"), F, d, &rc) : nullptr;
     if (!wi1) return rc;
     int wi_rows = 0;
-    // TMA box rows = the N-tile of the kernel that will read the weight (split-K or persistent)
-    const int bn_qkv = h->sk_on ? h->sk_qkv.bn : 64, bn_proj = h->sk_on ? h->sk_proj.bn : 32;
-    const int bn_wi = h->sk_on ? h->sk_wi.bn : 64, bn_ffo = h->sk_on ? h->sk_ffo.bn : 32;
+    // TMA box rows = the N-tile of the split-K kernel that will read the weight
+    const int bn_qkv = h->sk_qkv.bn, bn_proj = h->sk_proj.bn, bn_wi = h->sk_wi.bn, bn_ffo = h->sk_ffo.bn;
     TRY(interleave_geglu(h, wi0, wi1, w.wi, F, d, bn_wi, &wi_rows));
     w.wi_rows = wi_rows;
     if (!(p = take(h, key("layer.2.DenseReluDense.wo.weight"), d, F, &rc))) return rc;
@@ -1045,8 +962,7 @@ extern "C" int b200t5_finalize(b200t5_handle h) {
     TMAP(h, &w.tm_wi, w.wi.p, wi_rows, d, bn_wi);
     TMAP_FFO(h, &w.tm_ffo, w.wff_o.p, d, h->ffo_k, bn_ffo);
   }
-  TMAP(h, &h->tm_crosskv, h->wcrosskv.p, static_cast<uint64_t>(c.Ld) * 2 * I, d, 256);
-  TMAP(h, &h->tm2_crosskv, h->wcrosskv.p, static_cast<uint64_t>(c.Ld) * 2 * I, d, 128);
+  TMAP(h, &h->tm_crosskv, h->wcrosskv.p, static_cast<uint64_t>(c.Ld) * 2 * I, d, k2ctaBox);
 
   h->raw.clear();
   h->raw_f32.clear();
@@ -1165,18 +1081,6 @@ static int ensure_plan(b200t5_ctx* h, int B, int S, int Tmax) {
   return build_plan(h, B, S, Tmax);
 }
 
-static GemmOp mk(const CUtensorMap& a, const CUtensorMap& b, int M, int N, int K, GemmKind k, int m_fastest) {
-  GemmOp g;
-  g.tmA = a;
-  g.tmB = b;
-  g.M = M;
-  g.N = N;
-  g.K = K;
-  g.kind = k;
-  g.m_fastest = m_fastest;
-  return g;
-}
-
 // ================================================================== encoder
 static int run_encoder(b200t5_ctx* h, const long long* ids, const long long* mask, cudaStream_t s, const int* row_on = nullptr) {
   const Cfg& c = h->c;
@@ -1187,9 +1091,9 @@ static int run_encoder(b200t5_ctx* h, const long long* ids, const long long* mas
   h->launches++;
   // Variable-length packing: only rows below extent[b] are ever read downstream, so the encoder runs on those
   // (elementwise.cuh). The number of packed rows sizes the GEMM grids, hence one 4-byte read-back per call.
-  p.packed = h->pack_rows && S <= kEncPackMaxS;
+  p.packed = S <= kEncPackMaxS;
   if (row_on && !p.packed)
-    return fail(h, B200T5_EINVAL, "slot-pool admission needs the packed encoder path (S <= %d, B200T5_PACK at its default)", kEncPackMaxS);
+    return fail(h, B200T5_EINVAL, "slot-pool admission needs the packed encoder path (S <= %d)", kEncPackMaxS);
   const int* cu = nullptr;
   p.rows_valid = M;
   if (p.packed) {
@@ -1216,8 +1120,7 @@ static int run_encoder(b200t5_ctx* h, const long long* ids, const long long* mas
     CU_OK(h, run_rmsnorm(h, p.x.as<res_t>(), w.ln0.as<act_t>(), p.xn.as<act_t>(), M, d, c.eps, s));
     {
       EpiStore::Params ep{p.qkv.as<act_t>(), 3 * I};
-      if (h->use_2cta) CU_OK(h, run_gemm_2cta<EpiStore>(h, p.tm_xn, w.tm2_qkv, M, 3 * I, d, ep, s));
-      else CU_OK(h, run_gemm(h, mk(p.tm_xn, w.tm_qkv, M, 3 * I, d, G_STORE256, 0), &ep, s));
+      CU_OK(h, run_gemm_2cta<EpiStore>(h, p.tm_xn, w.tm_qkv, M, 3 * I, d, ep, s));
     }
     encoder_attn_kernel<<<dim3((S + kEncQ - 1) / kEncQ, B * H), kEncThreads, attn_smem, s>>>(
         p.qkv.as<act_t>(), p.ctx.as<act_t>(), p.enc_bias.as<float>(), p.key_ok.as<unsigned char>(), p.extent.as<int>(), cu, S, H);
@@ -1226,21 +1129,18 @@ static int run_encoder(b200t5_ctx* h, const long long* ids, const long long* mas
     {
       EpiResidual::Params ep{p.x.as<res_t>(), p.x.as<res_t>(), d};
       ep.round_out = l == 0;  // (fp16 build) the stream is still fp16 before the first feed-forward block
-      if (h->use_2cta) CU_OK(h, run_gemm_2cta<EpiResidual>(h, p.tm_ctx, w.tm2_o, M, d, I, ep, s));
-      else CU_OK(h, run_gemm(h, mk(p.tm_ctx, w.tm_o, M, d, I, G_RES256, 0), &ep, s));
+      CU_OK(h, run_gemm_2cta<EpiResidual>(h, p.tm_ctx, w.tm_o, M, d, I, ep, s));
     }
     CU_OK(h, run_rmsnorm(h, p.x.as<res_t>(), w.ln1.as<act_t>(), p.xn.as<act_t>(), M, d, c.eps, s));
     {
       EpiGeglu::Params ep{p.hff.as<ffh_t>(), F, h->gelu_lut};
-      if (h->use_2cta) CU_OK(h, run_gemm_2cta<EpiGeglu>(h, p.tm_xn, w.tm2_wi, M, wi_tiles * 256, d, ep, s));
-      else CU_OK(h, run_gemm(h, mk(p.tm_xn, w.tm_wi, M, wi_tiles * 256, d, G_GEGLU256, 0), &ep, s));
+      CU_OK(h, run_gemm_2cta<EpiGeglu>(h, p.tm_xn, w.tm_wi, M, wi_tiles * 256, d, ep, s));
     }
     {
       EpiResidual::Params ep{p.x.as<res_t>(), p.x.as<res_t>(), d};
       ep.round_acc = B200T5_F16 ? 0 : 1;  // fp16 build: `wo` is an fp32 Linear, its output is not rounded
       ep.round_out = B200T5_F16 ? 0 : 1;
-      if (h->use_2cta) CU_OK(h, run_ffo_2cta(h, p.tm_hff, w.tm2_ffo, M, d, ep, s));
-      else CU_OK(h, run_gemm(h, mk(p.tm_hff, w.tm_ffo, M, d, F, G_RES256, 0), &ep, s));
+      CU_OK(h, run_ffo_2cta(h, p.tm_hff, w.tm_ffo, M, d, ep, s));
     }
   }
   CU_OK(h, run_rmsnorm(h, p.x.as<res_t>(), h->enc_final_ln.as<act_t>(), p.xn.as<act_t>(), M, d, c.eps, s));
@@ -1256,8 +1156,7 @@ static int run_cross_kv(b200t5_ctx* h, cudaStream_t s) {
     ep.row_s = p.row_s.as<int>();
   }
   const int M = p.packed ? p.packed_rows : p.B * p.S;
-  if (h->use_2cta) CU_OK(h, run_gemm_2cta<EpiCrossKV>(h, p.tm_xn, h->tm2_crosskv, M, c.Ld * 2 * c.I, c.d, ep, s));
-  else CU_OK(h, run_gemm(h, mk(p.tm_xn, h->tm_crosskv, M, c.Ld * 2 * c.I, c.d, G_CROSSKV256, 0), &ep, s));
+  CU_OK(h, run_gemm_2cta<EpiCrossKV>(h, p.tm_xn, h->tm_crosskv, M, c.Ld * 2 * c.I, c.d, ep, s));
   return B200T5_OK;
 }
 
@@ -1302,29 +1201,22 @@ static int chain_layer_pre(b200t5_ctx* h, cudaStream_t s, const ChainView& v, in
   CU_OK(h, run_rmsnorm(h, v.dx, w.ln0.as<act_t>(), v.dxn, v.nb, d, c.eps, s, pdl));
   {
     EpiQkvDecode::Params ep{v.dq, skv, step, B, H, T, sstride};
-    if (h->sk_on) CU_OK(h, run_gemm_sk<EpiQkvDecode>(h, h->sk_qkv, v.ch->tm_dxn, w.tm_qkv, v.nb, 3 * I, d, ep, s, pdl));
-    else CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, w.tm_qkv, v.nb, 3 * I, d, G_QKVDEC64, 1), &ep, s, pdl));
+    CU_OK(h, run_gemm_sk<EpiQkvDecode>(h, h->sk_qkv, v.ch->tm_dxn, w.tm_qkv, v.nb, 3 * I, d, ep, s, pdl));
   }
-  if (h->self_block)  // 4 warps per (row, head): two memory round trips whatever t is
-    CU_OK(h, launch_kernel(attn_decode_kernel<true>, dim3(v.nb * H), dim3(kAttnDecThreads), T * sizeof(float), s, pdl, v.dq, skv,
-                           skv + static_cast<size_t>(B) * I * T, v.dctx, H, T, nullptr, nullptr, step, p.dec_bias.as<float>(),
-                           XsStamps{nullptr, 0}, sstride));
-  else
-    CU_OK(h, launch_kernel(self_attn_decode_warp_kernel, dim3((v.nb * H + kSelfWarpsPerCta - 1) / kSelfWarpsPerCta),
-                           dim3(kSelfWarpsPerCta * 32), kSelfWarpsPerCta * T * sizeof(float), s, pdl, v.dq, skv,
-                           skv + static_cast<size_t>(B) * I * T, v.dctx, v.nb * H, H, T, step, p.dec_bias.as<float>(), sstride));
+  // 4 warps per (row, head): two memory round trips whatever t is
+  CU_OK(h, launch_kernel(attn_decode_kernel<true>, dim3(v.nb * H), dim3(kAttnDecThreads), T * sizeof(float), s, pdl, v.dq, skv,
+                         skv + static_cast<size_t>(B) * I * T, v.dctx, H, T, nullptr, nullptr, step, p.dec_bias.as<float>(),
+                         XsStamps{nullptr, 0}, sstride));
   h->launches++;
   {
     EpiResidual::Params ep{v.dx, v.dx, d};
     ep.round_out = l == 0;  // (fp16 build) the stream is still fp16 before the first feed-forward block
-    if (h->sk_on) CU_OK(h, run_gemm_sk<EpiResidual>(h, h->sk_proj, v.ch->tm_dctx, w.tm_o, v.nb, d, I, ep, s, pdl));
-    else CU_OK(h, run_gemm(h, mk(v.ch->tm_dctx, w.tm_o, v.nb, d, I, G_RES32, 1), &ep, s, pdl));
+    CU_OK(h, run_gemm_sk<EpiResidual>(h, h->sk_proj, v.ch->tm_dctx, w.tm_o, v.nb, d, I, ep, s, pdl));
   }
   CU_OK(h, run_rmsnorm(h, v.dx, w.ln1.as<act_t>(), v.dxn, v.nb, d, c.eps, s, pdl));
   {
     EpiStore::Params ep{v.dq, I};
-    if (h->sk_on) CU_OK(h, run_gemm_sk<EpiStore>(h, h->sk_proj, v.ch->tm_dxn, w.tm_cq, v.nb, I, d, ep, s, pdl));
-    else CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, w.tm_cq, v.nb, I, d, G_STORE32, 1), &ep, s, pdl));
+    CU_OK(h, run_gemm_sk<EpiStore>(h, h->sk_proj, v.ch->tm_dxn, w.tm_cq, v.nb, I, d, ep, s, pdl));
   }
   return B200T5_OK;
 }
@@ -1340,11 +1232,9 @@ static cudaError_t launch_cross_attention(b200t5_ctx* h, cudaStream_t s, bool pd
   if (p.xattn_stream) {
     const int items = nb * c.H;
     const int k_row0 = ((l * 2) * B + b0) * c.H * S, v_row0 = ((l * 2 + 1) * B + b0) * c.H * S;
-    const act_t* arena = p.cross_kv.as<act_t>();
     return launch_kernel(attn_cross_stream_kernel, dim3(xs_grid(items, h->num_sms)), dim3(kXsThreads),
-                         XsSmem::bytes(h->xs_stages, S), s, pdl, p.tm_cross_kv, p.tm_cross_kv, k_row0, v_row0,
-                         arena + static_cast<size_t>(k_row0) * 64, arena + static_cast<size_t>(v_row0) * 64, q, ctx, items, c.H, S,
-                         ext, ok, h->xs_stages, h->xs_late_pdl ? 1 : 0, h->xs_l2_prefetch ? 1 : 0, st);
+                         XsSmem::bytes(h->xs_stages, S), s, pdl, p.tm_cross_kv, p.tm_cross_kv, k_row0, v_row0, q, ctx, items, c.H,
+                         S, ext, ok, h->xs_stages, st);
   }
   const act_t* kplane = p.cross_kv.as<act_t>() + l * (static_cast<size_t>(2) * B * I * S) + static_cast<size_t>(b0) * I * S;
   return launch_kernel(attn_decode_kernel<false>, dim3(nb * c.H), dim3(kAttnDecThreads), S * sizeof(float), s, pdl, q, kplane,
@@ -1352,15 +1242,10 @@ static cudaError_t launch_cross_attention(b200t5_ctx* h, cudaStream_t s, bool pd
 }
 
 // layer l, cross-attention over the encoder keys (the HBM-streaming kernel)
-static int chain_layer_cross(b200t5_ctx* h, cudaStream_t s, const ChainView& v, int l, int chain_index, bool pdl) {
+static int chain_layer_cross(b200t5_ctx* h, cudaStream_t s, const ChainView& v, int l, int chain_index) {
   Plan& p = *h->plan;
   const int S = p.S;
-  struct PrioGuard {
-    int saved;
-    PrioGuard() : saved(launch_priority()) { launch_priority() = 0; }
-    ~PrioGuard() { launch_priority() = saved; }
-  } guard;
-  CU_OK(h, launch_cross_attention(h, s, pdl, l, v.b0, v.nb, v.dq, v.dctx, p.live_extent.as<int>() + v.b0,
+  CU_OK(h, launch_cross_attention(h, s, h->use_pdl, l, v.b0, v.nb, v.dq, v.dctx, p.live_extent.as<int>() + v.b0,
                                   p.live_key_ok.as<unsigned char>() + static_cast<size_t>(v.b0) * S,
                                   h->profile_xattn ? l * p.n_chains + chain_index : -1));
   h->launches++;
@@ -1372,26 +1257,22 @@ static int chain_layer_post(b200t5_ctx* h, cudaStream_t s, const ChainView& v, i
   const Cfg& c = h->c;
   const int d = c.d, I = c.I, F = c.F;
   const bool pdl = h->use_pdl;
-  const int wi_tiles = (F + 31) / 32;
   DecLayerW& w = h->dec[l];
   {
     EpiResidual::Params ep{v.dx, v.dx, d};
     ep.round_out = l == 0;
-    if (h->sk_on) CU_OK(h, run_gemm_sk<EpiResidual>(h, h->sk_proj, v.ch->tm_dctx, w.tm_co, v.nb, d, I, ep, s, pdl));
-    else CU_OK(h, run_gemm(h, mk(v.ch->tm_dctx, w.tm_co, v.nb, d, I, G_RES32, 1), &ep, s, pdl));
+    CU_OK(h, run_gemm_sk<EpiResidual>(h, h->sk_proj, v.ch->tm_dctx, w.tm_co, v.nb, d, I, ep, s, pdl));
   }
   CU_OK(h, run_rmsnorm(h, v.dx, w.ln2.as<act_t>(), v.dxn, v.nb, d, c.eps, s, pdl));
   {
     EpiGeglu::Params ep{v.dh, F, h->gelu_lut};
-    if (h->sk_on) CU_OK(h, run_gemm_sk<EpiGeglu>(h, h->sk_wi, v.ch->tm_dxn, w.tm_wi, v.nb, w.wi_rows, d, ep, s, pdl));
-    else CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, w.tm_wi, v.nb, wi_tiles * 64, d, G_GEGLU64, 1), &ep, s, pdl));
+    CU_OK(h, run_gemm_sk<EpiGeglu>(h, h->sk_wi, v.ch->tm_dxn, w.tm_wi, v.nb, w.wi_rows, d, ep, s, pdl));
   }
   {
     EpiResidual::Params ep{v.dx, v.dx, d};
     ep.round_acc = B200T5_F16 ? 0 : 1;  // fp16 build: `wo` is an fp32 Linear, its output is not rounded
     ep.round_out = B200T5_F16 ? 0 : 1;
-    if (h->sk_on) CU_OK(h, run_ffo_sk(h, h->sk_ffo, v.ch->tm_dh, w.tm_ffo, v.nb, d, ep, s, pdl));
-    else CU_OK(h, run_gemm(h, mk(v.ch->tm_dh, w.tm_ffo, v.nb, d, F, G_RES32, 1), &ep, s, pdl));
+    CU_OK(h, run_ffo_sk(h, h->sk_ffo, v.ch->tm_dh, w.tm_ffo, v.nb, d, ep, s, pdl));
   }
   return B200T5_OK;
 }
@@ -1406,7 +1287,8 @@ static int chain_head(b200t5_ctx* h, cudaStream_t s, const ChainView& v, float* 
   CU_OK(h, run_rmsnorm(h, v.dx, h->dec_final_ln.as<act_t>(), v.dxn, v.nb, d, c.eps, s, pdl));
   if (logits_out) {
     EpiStoreF32::Params ep{logits_out + static_cast<size_t>(v.b0) * ldl, ldl};
-    CU_OK(h, run_gemm(h, mk(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, G_LOGITS128, 1), &ep, s, pdl));
+    h->launches++;
+    CU_OK(h, (launch_gemm<128, EpiStoreF32>(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, 1, ep, h->num_sms, s, pdl)));
     return B200T5_OK;
   }
   const bool sm = p.stream_mode;
@@ -1439,15 +1321,6 @@ static int chain_head(b200t5_ctx* h, cudaStream_t s, const ChainView& v, float* 
   return B200T5_OK;
 }
 
-static cudaEvent_t xattn_event(b200t5_ctx* h, size_t k) {
-  while (h->xattn_ev.size() <= k) {
-    cudaEvent_t e = nullptr;
-    cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
-    h->xattn_ev.push_back(e);
-  }
-  return h->xattn_ev[k];
-}
-
 // All chains of one step. `fork` (used while capturing the step graph) runs the chains on their own streams, so
 // that one chain's HBM-streaming cross-attention overlaps the other chain's latency-bound GEMM phases.
 static int run_decode_step(b200t5_ctx* h, cudaStream_t s, bool fork, float* logits_out, int ldl, long long eos,
@@ -1457,32 +1330,16 @@ static int run_decode_step(b200t5_ctx* h, cudaStream_t s, bool fork, float* logi
   const int nc = p.n_chains;
   ChainView v[kMaxChains];
   for (int i = 0; i < nc; ++i) v[i] = chain_view(h, p.chains[i]);
-  struct StepPrio {
-    StepPrio(int pr) { launch_priority() = pr; }
-    ~StepPrio() { launch_priority() = 0; }
-  } step_prio(h->small_prio);
   if (fork && nc > 1) {
     cudaStream_t cs[kMaxChains];
     cs[0] = s;
     for (int i = 1; i < nc; ++i) cs[i] = h->chain_streams[i];
     CU_OK(h, cudaEventRecord(h->chain_ev[0], s));
     for (int i = 1; i < nc; ++i) CU_OK(h, cudaStreamWaitEvent(cs[i], h->chain_ev[0], 0));
-    // Identical chains started together stay in lock-step: they all stream K/V at the same moment (sharing the
-    // HBM bandwidth) and all sit in their latency-bound GEMM phases at the same moment (HBM idle) - measured in
-    // round 2, two chains' 128-row cross-attention launches took 57 us each in situ against 41 us alone. With
-    // `xattn_serialize` ONE dependency is threaded through every cross-attention kernel in round-robin order
-    // (layer-major, chain-minor): at most one chain streams at a time, at full bandwidth, and the other chains'
-    // GEMM phases fill the gaps - a software pipeline across chains made of graph edges only.
-    size_t k = 0;
     for (int l = 0; l < c.Ld; ++l) {
       for (int i = 0; i < nc; ++i) {
         TRY(chain_layer_pre(h, cs[i], v[i], l));
-        const bool ser = h->xattn_serialize && k > 0;
-        if (ser) CU_OK(h, cudaStreamWaitEvent(cs[i], xattn_event(h, k - 1), 0));
-        // after an event wait the kernel has two predecessors: it is launched without the PDL attribute
-        TRY(chain_layer_cross(h, cs[i], v[i], l, i, h->use_pdl && !ser));
-        if (h->xattn_serialize) CU_OK(h, cudaEventRecord(xattn_event(h, k), cs[i]));
-        ++k;
+        TRY(chain_layer_cross(h, cs[i], v[i], l, i));
         TRY(chain_layer_post(h, cs[i], v[i], l));
       }
     }
@@ -1497,7 +1354,7 @@ static int run_decode_step(b200t5_ctx* h, cudaStream_t s, bool fork, float* logi
     for (int i = 0; i < nc; ++i) {
       for (int l = 0; l < c.Ld; ++l) {
         TRY(chain_layer_pre(h, s, v[i], l));
-        TRY(chain_layer_cross(h, s, v[i], l, i, h->use_pdl));
+        TRY(chain_layer_cross(h, s, v[i], l, i));
         TRY(chain_layer_post(h, s, v[i], l));
       }
       TRY(chain_head(h, s, v[i], logits_out, ldl, eos, pad, min_new));
@@ -2191,10 +2048,10 @@ extern "C" int b200t5_bench_cross_attn(b200t5_handle h, int reps, int rows_per_l
 // Runtime options (what the B200T5_* environment variables set at create time, changeable on a live handle so
 // that a sweep does not reload the model). Any change drops the execution plan: the next call re-captures the
 // step graph. Names: "chains" (row-chains per step, 0 = default), "xattn" (decode cross-attention: 0 = per-thread-load
-// kernel, 1 = TMA stream kernel, 2 = per call by prompt fill), "xattn_stages", "xattn_late_pdl", "xattn_serialize",
-// "xattn_l2pf", "pdl", "admit_overlap", "sk_stages64", "sk_stages128", "profile_xattn" (1 = every cross-attention launch
-// inside the step graph stamps %globaltimer; read with b200t5_get_xattn_profile; off in any timed region), "enc_gemm"
-// (128 x 256 encoder GEMMs: 1 = epilogue-overlapped kernel, 0 = the kernel whose epilogue follows each main loop).
+// kernel, 1 = TMA stream kernel, 2 = per call by prompt fill), "xattn_stages", "pdl", "admit_overlap", "sk_stages64",
+// "sk_stages128", "profile_xattn" (1 = every cross-attention launch inside the step graph stamps %globaltimer; read with
+// b200t5_get_xattn_profile; off in any timed region), "enc_gemm" (128 x 256 encoder GEMMs: 1 = epilogue-overlapped
+// kernel, 0 = the kernel whose epilogue follows each main loop).
 extern "C" int b200t5_set_option(b200t5_handle h, const char* name, int value) {
   if (!h || !name) return fail(h, B200T5_EINVAL, "null argument");
   const std::string n(name);
@@ -2203,10 +2060,7 @@ extern "C" int b200t5_set_option(b200t5_handle h, const char* name, int value) {
   else if (n == "xattn_stages") {
     if (value < 2 || value > kXsMaxStages) return fail(h, B200T5_EINVAL, "xattn_stages must be in [2, %d]", kXsMaxStages);
     h->xs_stages = value;
-  } else if (n == "xattn_late_pdl") h->xs_late_pdl = value != 0;
-  else if (n == "xattn_serialize") h->xattn_serialize = value != 0;
-  else if (n == "xattn_l2pf") h->xs_l2_prefetch = value != 0;
-  else if (n == "pdl") h->use_pdl = value != 0;
+  } else if (n == "pdl") h->use_pdl = value != 0;
   else if (n == "admit_overlap") h->admit_overlap = value != 0;
   else if (n == "sk_stages64") h->sk_stages64 = value;
   else if (n == "sk_stages128") h->sk_stages128 = value;
@@ -2334,49 +2188,30 @@ extern "C" int b200t5_test_gemm(int device, const void* A, const void* W, void* 
   if (sms < 0) return sms;
   if (K % 8) return fail(nullptr, B200T5_EINVAL, "K must be a multiple of 8");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // bn 512: the encoder configuration (128 x 256 tiles, weight loaded in 128-row boxes, gemm_2cta.cuh), modes 0/1/2/5;
+  // bn 128: the fp32 logits of b200t5_decode_logits, mode 3
+  if (!((bn == 512 && (mode == 0 || mode == 1 || mode == 2 || mode == 5)) || (bn == 128 && mode == 3)))
+    return fail(nullptr, B200T5_EINVAL, "test_gemm: bn=512 with mode 0/1/2/5, or bn=128 with mode 3");
   CUtensorMap ta, tb;
-  if (!make_tmap(&ta, A, M, K, 128) || !make_tmap(&tb, W, N, K, bn == 512 ? 128 : bn)) return fail(nullptr, B200T5_ECUDA, "%s", g_err);
+  if (!make_tmap(&ta, A, M, K, 128) || !make_tmap(&tb, W, N, K, 128)) return fail(nullptr, B200T5_ECUDA, "%s", g_err);
   b200t5_ctx dummy;
   dummy.num_sms = sms;
   cudaError_t e = cudaErrorInvalidValue;
-  act_t* Cb = static_cast<act_t*>(C);
-  if (bn == 512) {  // the encoder configuration: 128 x 256 tiles, weight loaded in 128-row boxes (gemm_2cta.cuh)
-    if (mode == 0) {
-      EpiStore::Params ep{Cb, N};
-      e = run_gemm_2cta<EpiStore>(&dummy, ta, tb, M, N, K, ep, s);
-    } else if (mode == 1 || mode == 5) {
-      const EpiResidual::Params ep = hook_residual(C, N, mode);
-      e = run_gemm_2cta<EpiResidual>(&dummy, ta, tb, M, N, K, ep, s);
-    } else if (mode == 2) {
-      GeluLut lut;
-      int lrc = hook_gelu_lut(pow_mode, &lut);
-      if (lrc != B200T5_OK) return lrc;
-      EpiGeglu::Params ep{static_cast<ffh_t*>(C), N / 2, lut};
-      e = run_gemm_2cta<EpiGeglu>(&dummy, ta, tb, M, N, K, ep, s);
-    }
-    if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_gemm(pair, mode=%d): %s", mode, cudaGetErrorString(e));
-    return B200T5_OK;
-  }
   if (mode == 0) {
-    EpiStore::Params ep{Cb, N};
-    if (bn == 256) e = run_gemm(&dummy, mk(ta, tb, M, N, K, G_STORE256, 0), &ep, s);
-    else if (bn == 32) e = run_gemm(&dummy, mk(ta, tb, M, N, K, G_STORE32, 1), &ep, s);
-    else if (bn == 64) e = launch_gemm<64, EpiStore>(ta, tb, M, N, K, 0, ep, sms, s);
-    else if (bn == 128) e = launch_gemm<128, EpiStore>(ta, tb, M, N, K, 0, ep, sms, s);
+    EpiStore::Params ep{static_cast<act_t*>(C), N};
+    e = run_gemm_2cta<EpiStore>(&dummy, ta, tb, M, N, K, ep, s);
   } else if (mode == 1 || mode == 5) {
     const EpiResidual::Params ep = hook_residual(C, N, mode);
-    if (bn == 256) e = run_gemm(&dummy, mk(ta, tb, M, N, K, G_RES256, 0), &ep, s);
-    else if (bn == 32) e = run_gemm(&dummy, mk(ta, tb, M, N, K, G_RES32, 1), &ep, s);
+    e = run_gemm_2cta<EpiResidual>(&dummy, ta, tb, M, N, K, ep, s);
   } else if (mode == 2) {
     GeluLut lut;
     int lrc = hook_gelu_lut(pow_mode, &lut);
     if (lrc != B200T5_OK) return lrc;
     EpiGeglu::Params ep{static_cast<ffh_t*>(C), N / 2, lut};
-    if (bn == 256) e = run_gemm(&dummy, mk(ta, tb, M, N, K, G_GEGLU256, 0), &ep, s);
-    else if (bn == 64) e = run_gemm(&dummy, mk(ta, tb, M, N, K, G_GEGLU64, 1), &ep, s);
-  } else if (mode == 3) {
+    e = run_gemm_2cta<EpiGeglu>(&dummy, ta, tb, M, N, K, ep, s);
+  } else {
     EpiStoreF32::Params ep{static_cast<float*>(C), N};
-    if (bn == 128) e = run_gemm(&dummy, mk(ta, tb, M, N, K, G_LOGITS128, 1), &ep, s);
+    e = launch_gemm<128, EpiStoreF32>(ta, tb, M, N, K, 1, ep, sms, s);
   }
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_gemm(bn=%d, mode=%d): %s", bn, mode, cudaGetErrorString(e));
   return B200T5_OK;
@@ -2624,7 +2459,8 @@ extern "C" int b200t5_test_attn_decode(int device, int self, const void* q, cons
   const int sms = hook_device(device);
   if (sms < 0) return sms;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (self == 1 || self == 3) {
+  if (self == 1) return fail(nullptr, B200T5_EINVAL, "attn_decode: self in {0, 2, 3}");
+  if (self == 3) {
     // the position: `step` for every row (static batch), or extent[b] for row b (slot pool, step_stride 1)
     DevBuf st;
     if (st.alloc(sizeof(DecodeState)) != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "alloc");
@@ -2632,13 +2468,8 @@ extern "C" int b200t5_test_attn_decode(int device, int self, const void* q, cons
     const int* pos = extent ? extent : &st.as<DecodeState>()->step;
     const int stride = extent ? 1 : 0;
     const act_t *qa = static_cast<const act_t*>(q), *Ka = static_cast<const act_t*>(K), *Va = static_cast<const act_t*>(V);
-    if (self == 3)
-      attn_decode_kernel<true><<<B * H, kAttnDecThreads, Tk * sizeof(float), s>>>(
-          qa, Ka, Va, static_cast<act_t*>(ctx), H, Tk, nullptr, nullptr, pos, dist_bias, XsStamps{nullptr, 0}, stride);
-    else
-      self_attn_decode_warp_kernel<<<(B * H + kSelfWarpsPerCta - 1) / kSelfWarpsPerCta, kSelfWarpsPerCta * 32,
-                                     kSelfWarpsPerCta * Tk * sizeof(float), s>>>(qa, Ka, Va, static_cast<act_t*>(ctx), B * H, H, Tk,
-                                                                                 pos, dist_bias, stride);
+    attn_decode_kernel<true><<<B * H, kAttnDecThreads, Tk * sizeof(float), s>>>(
+        qa, Ka, Va, static_cast<act_t*>(ctx), H, Tk, nullptr, nullptr, pos, dist_bias, XsStamps{nullptr, 0}, stride);
     cudaStreamSynchronize(s);
   } else if (self == 2) {  // the TMA stream kernel (attention_cross_stream.cuh); `step` = ring stages (0: 5)
     const int stages = step > 0 ? step : 5;
@@ -2648,8 +2479,7 @@ extern "C" int b200t5_test_attn_decode(int device, int self, const void* q, cons
     if (!make_tmap(&tk, K, static_cast<uint64_t>(items) * Tk, 64, kXsChunkKeys) || !make_tmap(&tv, V, static_cast<uint64_t>(items) * Tk, 64, kXsChunkKeys))
       return fail(nullptr, B200T5_ECUDA, "%s", g_err);
     attn_cross_stream_kernel<<<xs_grid(items, sms), kXsThreads, XsSmem::bytes(stages, Tk), s>>>(
-        tk, tv, 0, 0, static_cast<const act_t*>(K), static_cast<const act_t*>(V), static_cast<const act_t*>(q), static_cast<act_t*>(ctx), items, H,
-        Tk, extent, key_ok, stages, 1, 1, XsStamps{nullptr, 0});
+        tk, tv, 0, 0, static_cast<const act_t*>(q), static_cast<act_t*>(ctx), items, H, Tk, extent, key_ok, stages, XsStamps{nullptr, 0});
   } else {
     attn_decode_kernel<false><<<B * H, kAttnDecThreads, Tk * sizeof(float), s>>>(
         static_cast<const act_t*>(q), static_cast<const act_t*>(K), static_cast<const act_t*>(V), static_cast<act_t*>(ctx), H,

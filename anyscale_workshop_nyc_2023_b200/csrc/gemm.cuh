@@ -28,7 +28,7 @@ constexpr int kEpiSmemBytes = 8192;  // per-CTA scratch the epilogue functor may
 
 template <int BN>
 struct GemmCfg {
-  static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "BN");
+  static_assert(BN == 128 || BN == 256, "BN");
   static constexpr int kABytes = kBM * kBK * 2;
   static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
@@ -773,15 +773,6 @@ cudaError_t prepare_gemm() {
                               GemmCfg<BN>::kSmemBytes);
 }
 
-// Scheduling priority attached to every kernel launched through launch_kernel / launch_gemm_splitk
-// (0 = default). The decode step raises it for the short latency-bound kernels so that, when
-// row-chains run concurrently, their CTAs are placed ahead of the queued CTAs of another chain's
-// HBM-streaming cross-attention kernel instead of behind them.
-inline int& launch_priority() {
-  static thread_local int prio = 0;
-  return prio;
-}
-
 // Launch with (optionally) the programmatic-stream-serialization attribute (PDL).
 template <class... KArgs, class... Args>
 cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, bool pdl,
@@ -791,20 +782,11 @@ cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t 
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (pdl) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  if (launch_priority() != 0) {
-    attr[na].id = cudaLaunchAttributePriority;
-    attr[na].val.priority = launch_priority();
-    ++na;
-  }
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = na;
+  cfg.numAttrs = pdl ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 

@@ -1,6 +1,6 @@
 // Encoder GEMMs (M = packed prompt rows, tens of thousands):  D[M,N] = A[M,K] * W[N,K]^T  on 128 x 256 tiles.
 //
-// The encoder's tensor maps (tm2_*) have 128-row boxes for both operands; this configuration of the persistent
+// The encoder's tensor maps (EncLayerW::tm_*, tm_crosskv) have 128-row boxes for both operands; this configuration of the persistent
 // wgmma kernel (gemm.cuh) loads each 256-row weight tile as two such boxes. A 128 x 256 tile is the largest the
 // two consumer warpgroups hold in registers (128 fp32 accumulators per thread) and gives the best operand reuse
 // per byte of shared memory: per k-block 48 KB are staged for 128 x 256 x 64 MACs.

@@ -279,7 +279,7 @@ cudaError_t launch_gemm_splitk(const CUtensorMap& tmA, const CUtensorMap& tmB, i
   cfg.blockDim = dim3(kSkThreads);
   cfg.dynamicSmemBytes = Cfg::smem_bytes(stages, Epi::kPaired);
   cfg.stream = stream;
-  cudaLaunchAttribute attr[3];
+  cudaLaunchAttribute attr[2];
   int na = 0;
   attr[na].id = cudaLaunchAttributeClusterDimension;
   attr[na].val.clusterDim.x = split;
@@ -289,11 +289,6 @@ cudaError_t launch_gemm_splitk(const CUtensorMap& tmA, const CUtensorMap& tmB, i
   if (pdl) {
     attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  if (launch_priority() != 0) {
-    attr[na].id = cudaLaunchAttributePriority;
-    attr[na].val.priority = launch_priority();
     ++na;
   }
   cfg.attrs = attr;

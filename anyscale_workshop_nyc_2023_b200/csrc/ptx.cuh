@@ -386,21 +386,12 @@ DEVINL uint64_t l2_policy_evict_first() {
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
   return p;
 }
-DEVINL uint64_t l2_policy_evict_last() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
 DEVINL uint4 ldg_nc_v4_hint(const void* p, uint64_t policy) {
   uint4 r;
   asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0, %1, %2, %3}, [%4], %5;"
                : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
                : "l"(p), "l"(policy));
   return r;
-}
-// Bring [p, p + bytes) into L2 (no shared-memory destination); bytes % 16 == 0, p 16-byte aligned.
-DEVINL void prefetch_l2_bulk(const void* p, uint32_t bytes, uint64_t policy) {
-  asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(p), "r"(bytes), "l"(policy) : "memory");
 }
 
 }  // namespace b200

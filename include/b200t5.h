@@ -215,12 +215,11 @@ int b200t5_bench_cross_attn(b200t5_handle h, int reps, int rows_per_launch, floa
 /* Runtime options: what the B200T5_* environment variables set at create time, on a live handle (a sweep need not
  * reload the model). A change drops the execution plan; the next call re-captures the step graph. Names: "chains"
  * (row-chains per decode step, 0 = default), "xattn" (decode cross-attention: 0 = per-thread-load kernel, 1 = TMA stream kernel, 2 = per call by prompt fill),
- * "xattn_stages" (8 KB ring stages per CTA), "xattn_late_pdl", "xattn_serialize", "xattn_l2pf", "pdl", "admit_overlap",
- * "sk_stages64", "sk_stages128" (pipeline stages of
+ * "xattn_stages" (8 KB ring stages per CTA), "pdl", "admit_overlap", "sk_stages64", "sk_stages128" (pipeline stages of
  * the split-K decode GEMM tiles, 0 = default), "profile_xattn" (1 = every cross-attention launch inside the step graph
  * records %globaltimer stamps; never on in a timed region), "enc_gemm" (the 128 x 256 encoder GEMMs: 1 = default,
  * epilogue warps drain each tile while the next tile's MMAs run; 0 = the kernel whose epilogue follows each main loop;
- * bit-identical results; environment variable B200T5_ENC_GEMM at create time). */
+ * bit-identical results; environment variable B200T5_ENC_GEMM at create time). Any other name returns B200T5_EINVAL. */
 int b200t5_set_option(b200t5_handle h, const char* name, int value);
 /* With "profile_xattn" on: mean in-situ duration (first CTA start to last CTA end) of the cross-attention launches the
  * step graph made since the option was set, how many there were, and the algorithmic bytes of one such launch; and,
@@ -270,11 +269,12 @@ int b200t5_relative_bucket(int relative_position, int bidirectional, int num_buc
 /* Single-kernel hooks, in both builds: all pointers are device pointers. A 2-byte tensor is the build's activation
  * type (bf16 in libb200t5.so, fp16 in libb200t5_f16.so) unless noted. In the fp16 build the residual stream (the
  * residual C / R of the GEMMs, the RMSNorm input x) is fp32, and so is the GeGLU output (holding fp16 values). */
-/* C[M,N] = act(A[M,K] W[N,K]^T) via the wgmma GEMM; mode 0 plain, 1 += residual R (in C), 5 += residual as in
- * decoder / encoder layer 0 (fp16 build: C = fp16(R + fp16(acc)), where mode 1 is C = R + fp16(acc); bf16 build:
- * same as 1), 2 GeGLU (W rows interleaved per bn/2, C is [M,N/2]), 3 fp32 output (C is float*). bn in {32,64,128,256};
- * bn = 512 selects the encoder configuration (128 x 256 tiles, weight in 128-row boxes, GeGLU interleave per 128),
- * modes 0, 1, 2, 5. pow_mode: the gelu table's (bf16 build; the fp16 build's epilogue has no table). */
+/* C[M,N] = act(A[M,K] W[N,K]^T) via the wgmma GEMM in one of the configurations the library launches:
+ * bn = 512, the encoder configuration (128 x 256 tiles, weight in 128-row boxes) with mode 0 plain, 1 += residual R
+ * (in C), 5 += residual as in decoder / encoder layer 0 (fp16 build: C = fp16(R + fp16(acc)), where mode 1 is
+ * C = R + fp16(acc); bf16 build: same as 1), 2 GeGLU (W rows interleaved per 128, C is [M,N/2]); or bn = 128 with
+ * mode 3, the fp32 logits of b200t5_decode_logits (C is float*). Anything else returns B200T5_EINVAL. pow_mode: the
+ * gelu table's (bf16 build; the fp16 build's epilogue has no table). */
 int b200t5_test_gemm(int device, const void* A, const void* W, void* C, int M, int N, int K, int bn, int mode,
                      int pow_mode, void* stream);
 /* The 128 x 256 encoder GEMM as the encoder launches it; kernel 0 = the kernel whose epilogue follows each main loop,
@@ -296,11 +296,11 @@ int b200t5_test_gemm_splitk(int device, const void* A, const void* W, void* C, i
 int b200t5_test_ffo(int device, const void* A, const void* W, void* R, int M, int N, int F, int kernel, int bn, int split,
                     void* stream);
 int b200t5_test_rmsnorm(int device, const void* x, const void* w, void* y, int M, int d, float eps, void* stream);
-/* Decoder self-attention: self == 3 the 4-warp-per-(row, head) kernel the decode step runs, self == 1 the one-warp
- * variant (B200T5_SELF=warp); keys = t+1 with t = step, or, when extent is not NULL, t = extent[b] (int32 [B]: the
+/* Decoder self-attention: self == 3 the 4-warp-per-(row, head) kernel the decode step runs; keys = t+1 with t = step, or, when extent is not NULL, t = extent[b] (int32 [B]: the
  * slot pool's per-row positions); dist_bias float [H][Tk]. Cross-attention: self == 0: extent int32 [B], key_ok uint8 [B][Tk];
  * self == 2: as 0 through the TMA stream kernel (csrc/attention_cross_stream.cuh), `step` = ring stages (0: 5);
- * same rounding points as self == 0, the fp32 accumulations in the tensor core's order. */
+ * same rounding points as self == 0, the fp32 accumulations in the tensor core's order. self == 1 returns
+ * B200T5_EINVAL. */
 int b200t5_test_attn_decode(int device, int self, const void* q, const void* K, const void* V, void* ctx, int B,
                             int H, int Tk, const int32_t* extent, const uint8_t* key_ok, int step,
                             const float* dist_bias, void* stream);

@@ -100,7 +100,7 @@ def test_gelu_new_every_input_elementwise(lib, build):
 
 
 # (hook, bn / kernel, split): every GEMM that launches EpiGeglu, with the width over which it interleaves gate / up rows
-GEGLU_GEMMS = [("gemm", 64, 0), ("gemm", 256, 0), ("enc", 0, 0), ("enc", 1, 0), ("splitk", 64, 4), ("splitk", 128, 2)]
+GEGLU_GEMMS = [("enc", 0, 0), ("enc", 1, 0), ("splitk", 64, 4), ("splitk", 128, 2)]
 
 
 def geglu_half(hook, bn):
@@ -108,9 +108,7 @@ def geglu_half(hook, bn):
 
 
 def run_geglu_gemm(lib, hook, bn, split, A, Wi, out, M, F, K):
-    if hook == "gemm":
-        rc = lib.b200t5_test_gemm(DEV, P(A), P(Wi), P(out), M, 2 * F, K, bn, 2, 0, None)
-    elif hook == "enc":
+    if hook == "enc":
         rc = lib.b200t5_test_enc_gemm(DEV, P(A), P(Wi), P(out), M, 2 * F, K, bn, 2, 0, None, None, 0, 0, 0, None)
     else:
         rc = lib.b200t5_test_gemm_splitk(DEV, P(A), P(Wi), P(out), M, 2 * F, K, bn, split, 2, 0, None, 0, 0, None)
@@ -161,8 +159,7 @@ def overflow_case(dt):
     return A, W, M, N, K
 
 
-@pytest.mark.parametrize("hook,bn,split", [("gemm", 256, 0), ("gemm", 32, 0), ("gemm", 512, 0), ("enc", 0, 0), ("enc", 1, 0),
-                                           ("splitk", 64, 4)])
+@pytest.mark.parametrize("hook,bn,split", [("gemm", 512, 0), ("enc", 0, 0), ("enc", 1, 0), ("splitk", 64, 4)])
 def test_fp16_epilogues_overflow_to_inf_as_torch(hook, bn, split):
     """An fp16 Linear whose fp32 accumulator lies beyond 65504 gives +-inf in torch, and so must the store, the
     layer-0 residual (fp16 stream: the sum itself may overflow) and the GeGLU gate. (HF's T5Block then clamps inf
@@ -205,8 +202,6 @@ def test_fp16_epilogues_overflow_to_inf_as_torch(hook, bn, split):
         assert same(Cio, ref).all(), mode
         assert torch.isinf(Cio).any().item() == (mode == 5)
     # GeGLU: gate beyond the range -> gelu_new(+inf) = inf, gelu_new(-inf) = NaN (-inf * 0), as in torch
-    if hook == "gemm" and bn not in (64, 256, 512):
-        return
     F = N // 2
     half = 128 if hook == "enc" or bn == 512 else bn // 2
     W0, W1 = W[:F], torch.ones(F, K, device="cuda", dtype=dt) * 0.005
@@ -347,7 +342,7 @@ SELF_CASES = [  # B, H, Tmax: Tmax not a multiple of the kernels' 16-key stride
 ]
 
 
-@pytest.mark.parametrize("kernel", [3, 1])  # 3: attn_decode_kernel<true> (the decode step's default), 1: the one-warp variant
+@pytest.mark.parametrize("kernel", [3])  # attn_decode_kernel<true>, the kernel the decode step runs
 @pytest.mark.parametrize("B,H,T", SELF_CASES)
 @pytest.mark.parametrize("build", BUILDS)
 def test_self_attention_decode_positions(lib, build, kernel, B, H, T):

@@ -65,11 +65,9 @@ def ulp_close(a, b, ulps=1.0, build="bf16"):
 
 
 @pytest.mark.parametrize("M,N,K,bn,build", in_builds([
-    (128, 256, 64, 256), (128, 256, 128, 256), (256, 512, 768, 256), (300, 520, 264, 256),
-    (4096, 2304, 768, 256), (8, 2304, 768, 64), (256, 768, 768, 32), (256, 768, 2048, 32),
-    (256, 1000, 512, 128), (200, 136, 64, 64),
     # bn = 512: the encoder configuration (128 x 256 tiles, weight tile loaded as two 128-row TMA boxes)
     (256, 256, 64, 512), (512, 768, 768, 512), (4096, 2304, 768, 512), (300, 520, 264, 512), (1000, 1000, 2048, 512),
+    (128, 256, 64, 512), (128, 256, 128, 512), (256, 512, 768, 512),
 ]))
 def test_gemm_store(lib, M, N, K, bn, build):
     dt = DT[build]
@@ -118,8 +116,8 @@ def check_residual(Cio, y, ref, build, mode):
     assert exact > 0.99, exact
 
 
-@pytest.mark.parametrize("M,N,K,bn,build,mode", in_builds([(256, 768, 768, 32), (384, 512, 1024, 256), (130, 264, 128, 256),
-                                                           (4096, 768, 2048, 512), (130, 264, 128, 512)], modes=(1, 5)))
+@pytest.mark.parametrize("M,N,K,bn,build,mode", in_builds([(4096, 768, 2048, 512), (130, 264, 128, 512), (384, 512, 1024, 512)],
+                                                          modes=(1, 5)))
 def test_gemm_residual(lib, M, N, K, bn, build, mode):
     """mode 1: C = R + act(acc) (fp16 build: fp32 stream); mode 5: the layer-0 phase, C = act(R + act(acc))."""
     A, W, R, y, ref = residual_case(M, N, K, build, mode)
@@ -172,14 +170,14 @@ def test_geglu_exhaustive(lib):
     assert ((out.float() == ref2.float()) | (out.view(torch.int16) == ref2.view(torch.int16))).all()
 
 
-@pytest.mark.parametrize("M,F,K,bn,build", in_builds([(256, 2048, 768, 64), (512, 1024, 512, 256), (100, 160, 128, 64), (4096, 2048, 768, 512)]))
+@pytest.mark.parametrize("M,F,K,bn,build", in_builds([(4096, 2048, 768, 512), (512, 1024, 512, 512)]))
 def test_gemm_geglu(lib, M, F, K, bn, build):
     dt = DT[build]
     g = torch.Generator(device="cuda").manual_seed(5)
     A = (torch.randn(M, K, device="cuda", generator=g) * 0.5).to(dt)
     W0 = (torch.randn(F, K, device="cuda", generator=g) * 0.1).to(dt)
     W1 = (torch.randn(F, K, device="cuda", generator=g) * 0.1).to(dt)
-    tile = 256 if bn == 512 else bn  # the pair kernel's tile is 256 wide
+    tile = 256  # the encoder configuration's tile is 256 wide
     half = tile // 2
     ntiles = (F + half - 1) // half
     Wi = torch.zeros(ntiles * tile, K, device="cuda", dtype=dt)
@@ -211,6 +209,7 @@ SK_SHAPES = [
     (256, 768, 768, 64, 4), (256, 768, 2048, 64, 4), (256, 768, 2048, 64, 8), (256, 2304, 768, 128, 4),
     (64, 768, 768, 64, 4), (8, 512, 384, 64, 4), (8, 512, 384, 64, 8), (130, 1024, 2816, 64, 4),
     (256, 1000, 512, 128, 2), (200, 136, 64, 64, 4), (256, 768, 768, 64, 1), (100, 264, 1024, 128, 8),
+    (8, 2304, 768, 64, 2),
 ]
 
 
@@ -248,7 +247,8 @@ def test_gemm_splitk_residual(lib, M, N, K, bn, split, build, mode):
     check_residual(Cio, y, ref, build, mode)
 
 
-@pytest.mark.parametrize("M,F,K,bn,split,build", in_builds([(256, 2048, 768, 128, 2), (256, 2048, 768, 64, 4), (64, 1024, 512, 128, 4), (100, 2816, 1024, 64, 2)]))
+@pytest.mark.parametrize("M,F,K,bn,split,build", in_builds([(256, 2048, 768, 128, 2), (256, 2048, 768, 64, 4), (64, 1024, 512, 128, 4), (100, 2816, 1024, 64, 2),
+                                                             (100, 160, 128, 64, 2)]))
 def test_gemm_splitk_geglu(lib, M, F, K, bn, split, build):
     dt = DT[build]
     g = torch.Generator(device="cuda").manual_seed(5)
@@ -533,7 +533,7 @@ def test_self_attn_decode(lib, B, H, T, step, build):
     V = torch.randn(B, H, T, 64, device="cuda", generator=g).to(dt)
     dist_bias = torch.randn(H, T, device="cuda", generator=g).to(dt).float().contiguous()
     ctx = torch.empty(B, H * 64, device="cuda", dtype=dt)
-    _lib.check(lib.b200t5_test_attn_decode(DEV, 1, P(q), P(K), P(V), P(ctx), B, H, T, None, None, step, P(dist_bias), None), None, lib)
+    _lib.check(lib.b200t5_test_attn_decode(DEV, 3, P(q), P(K), P(V), P(ctx), B, H, T, None, None, step, P(dist_bias), None), None, lib)
     torch.cuda.synchronize()
     n = step + 1
     j = torch.arange(n, device="cuda")

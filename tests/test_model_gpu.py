@@ -220,7 +220,7 @@ def test_missing_attention_mask_is_inferred_from_pad_tokens_like_hf(models):
 
 def test_cross_attention_kernels_give_identical_tokens(models):
     """1, 2 and 3 row-chains and the knobs of the stream cross-attention kernel produce the same tokens (rows are independent
-    in every kernel, the ring depth and the PDL trigger do not touch the arithmetic); the two cross-attention kernels
+    in every kernel, the ring depth does not touch the arithmetic); the two cross-attention kernels
     differ only in the order of their fp32 accumulations, so they agree row for row up to the first near-tie step."""
     model, _ = models("mini", 2)
     spec = SPECS["mini"]
@@ -239,12 +239,11 @@ def test_cross_attention_kernels_give_identical_tokens(models):
         gated_b, _ = gated_prefix_match(stream.numpy(), base.numpy(), margins)
         print(f"stream kernel: vs oracle gated={gated:.2f} full={full:.2f}; vs per-thread-load kernel gated={gated_b:.2f} equal rows={gated_prefix_match(stream.numpy(), base.numpy(), margins)[1]:.2f}")
         assert gated == 1.0 and gated_b == 1.0
-        for name, value in (("chains", 1), ("chains", 3), ("xattn_stages", 2), ("xattn_late_pdl", 0), ("xattn_serialize", 1), ("xattn_l2pf", 1)):
+        for name, value in (("chains", 1), ("chains", 3), ("xattn_stages", 2)):
             model.set_option(name, value)
             assert torch.equal(model.generate(**kw).cpu(), stream), (name, value)
-        model.set_option("xattn_l2pf", 0)
     finally:
-        for name, value in (("xattn", 2), ("chains", 0), ("xattn_stages", 5), ("xattn_late_pdl", 1), ("xattn_serialize", 0)):
+        for name, value in (("xattn", 2), ("chains", 0), ("xattn_stages", 5)):
             model.set_option(name, value)
 
 

@@ -26,9 +26,9 @@ def static(n=256):
 
 
 ref = None
-CONFIGS = sys.argv[1].split(";") if len(sys.argv) > 1 else ("xattn=0", "xattn=1", "xattn=1,xattn_late_pdl=0", "xattn=1,chains=1", "xattn=1,pdl=0", "xattn=1,xattn_stages=2")
+CONFIGS = sys.argv[1].split(";") if len(sys.argv) > 1 else ("xattn=0", "xattn=1", "xattn=1,chains=1", "xattn=1,pdl=0", "xattn=1,xattn_stages=2")
 for opts in CONFIGS:
-    for k in ("xattn=0", "chains=0", "xattn_late_pdl=1", "pdl=1", "xattn_stages=5", "xattn_serialize=0", "sk_stages64=0", "sk_stages128=0", "xattn_l2pf=0"):
+    for k in ("xattn=0", "chains=0", "pdl=1", "xattn_stages=5", "sk_stages64=0", "sk_stages128=0"):
         a, b = k.split("=")
         m.set_option(a, int(b))
     for kv in opts.split(","):

@@ -19,9 +19,9 @@ from anyscale_workshop_nyc_2023_b200.modeling import B200T5ForConditionalGenerat
 from anyscale_workshop_nyc_2023_b200.synth import SPECS, synthetic_token_batch  # noqa: E402
 from anyscale_workshop_nyc_2023_b200.workload import checkpoint_dir  # noqa: E402
 
-DEFAULTS = {"chains": 0, "xattn": 2, "xattn_serialize": 0, "xattn_l2pf": 0, "xattn_stages": 5, "xattn_late_pdl": 1, "pdl": 1, "sk_stages64": 0, "sk_stages128": 0}
+DEFAULTS = {"chains": 0, "xattn": 2, "xattn_stages": 5, "pdl": 1, "sk_stages64": 0, "sk_stages128": 0}
 DEFAULT_CONFIGS = ("chains=1,xattn=0;chains=2,xattn=0;chains=1;chains=2;chains=3;chains=4;"
-                   "chains=2,xattn_late_pdl=0;chains=2,xattn_stages=4;chains=2,xattn_stages=6,sk_stages64=3,sk_stages128=2;"
+                   "chains=2,xattn_stages=4;chains=2,xattn_stages=6,sk_stages64=3,sk_stages128=2;"
                    "chains=2,xattn_stages=8,sk_stages64=2,sk_stages128=2;chains=3,xattn_stages=4;chains=2,sk_stages64=3")
 
 
