@@ -80,6 +80,25 @@ class ScoreIO(C.Structure):
     ]
 
 
+class BeamParams(C.Structure):
+    _fields_ = [
+        ("num_beams", C.c_int32),
+        ("num_return_sequences", C.c_int32),
+        ("length_penalty", C.c_double),
+        ("early_stopping", C.c_int32),
+    ]
+
+
+class BeamIO(C.Structure):
+    _fields_ = [
+        ("sequences", C.c_void_p),
+        ("lengths", C.c_void_p),
+        ("sequences_scores", C.c_void_p),
+        ("beam_indices", C.c_void_p),
+        ("token_logprobs", C.c_void_p),
+    ]
+
+
 class Stats(C.Structure):
     _fields_ = [
         ("encoder_ms", C.c_float),
@@ -116,6 +135,12 @@ SIGNATURES = {
                                          C.POINTER(ScoreIO)]),
     "b200t5_generate_stream_scored": (_i, [_vp, _i64p, _i64p, C.c_int64, _i, C.POINTER(GenParams), C.POINTER(LogitsParams), _i, _i,
                                            _i64p, _i32p, C.POINTER(ScoreIO)]),
+    "b200t5_generate_beam": (_i, [_vp, _i64p, _i64p, _i, _i, C.POINTER(GenParams), C.POINTER(BeamParams), C.POINTER(BeamIO), _vp]),
+    "b200t5_generate_host_beam": (_i, [_vp, _i64p, _i64p, _i, _i, C.POINTER(GenParams), C.POINTER(BeamParams), C.POINTER(BeamIO)]),
+    "b200t5_get_beam_stats": (_i, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_int32)]),
+    "b200t5_test_beam_step": (_i, [_i, _vp, _i, _i, _i, _i, _i, _i, _i, C.c_double, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                   _vp]),
+    "b200t5_test_beam_reorder": (_i, [_i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "b200t5_get_stats": (_i, [_vp, C.POINTER(Stats)]),
     "b200t5_bench_cross_attn": (_i, [_vp, _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_double), _vp]),
     "b200t5_set_option": (_i, [_vp, C.c_char_p, _i]),

@@ -24,6 +24,7 @@
 #include "attention_decode.cuh"
 #include "attention_cross_stream.cuh"
 #include "attention_encoder.cuh"
+#include "beam.cuh"
 #include "elementwise.cuh"
 #include "gemm.cuh"
 #include "gemm_splitk.cuh"
@@ -270,8 +271,19 @@ struct ProcBufs {
   }
 };
 
+// Beam-search state of a plan (beam.cuh), allocated by the first beam call. The step graph bakes these addresses.
+struct BeamBufs {
+  DevBuf logits, cand_lp, cand_tok, run_score, hist_par, hist_tok, hist_lp, fin, heur, parent, prm, len_scale, moved;
+  BeamDev dev(int rows) const {
+    return BeamDev{prm.as<BeamParams>(), len_scale.as<float>(), logits.as<float>(), nullptr, cand_lp.as<float>(), cand_tok.as<int>(),
+                   run_score.as<float>(), hist_par.as<int>(), hist_tok.as<int>(), hist_lp.as<float>(), fin.as<BeamFin>(), heur.as<int>(),
+                   parent.as<int>(), rows};
+  }
+};
+
 struct Plan {
   int B = 0, S = 0, Tmax = 0;
+  int group = 1;  // rows per prompt (num_beams): the row-chains split on prompt boundaries
   // encoder workspace
   DevBuf x, xn, qkv, ctx, hff;          // [B*S, d], [B*S, d], [B*S, 3I], [B*S, I], [B*S, F]
   DevBuf key_ok, extent, enc_bias;      // uint8 [B,S], int [B], float [H][2S-1]
@@ -315,6 +327,11 @@ struct Plan {
   int g_score = -1;
   bool stream_mode = false;
   int g_stream = -1;
+  // beam search: beam_k > 0 when this call's step runs the beam head (lm_head -> fp32 logits -> beam.cuh); part of the
+  // step graph's key. Every other value of a beam call lives in device memory.
+  BeamBufs beam;
+  int beam_k = 0;
+  int g_beam = -1;
   int g_xattn = -1;           // cross-attention kernel baked into the step graph (0 per-thread-load, 1 stream)
   bool xattn_stream = false;  // ... and the one launch_cross_attention issues now
   long long rows_valid = 0;   // valid prompt tokens of the last encoder pass (packed rows)
@@ -973,12 +990,13 @@ extern "C" int b200t5_finalize(b200t5_handle h) {
 
 
 // ================================================================== plans
-static int build_plan(b200t5_ctx* h, int B, int S, int Tmax) {
+static int build_plan(b200t5_ctx* h, int B, int S, int Tmax, int group) {
   const Cfg& c = h->c;
   std::unique_ptr<Plan> pl(new Plan());
   pl->B = B;
   pl->S = S;
   pl->Tmax = Tmax;
+  pl->group = group;
   const size_t M = static_cast<size_t>(B) * S;
   const int d = c.d, I = c.I, F = c.F, H = c.H;
   CU_OK(h, pl->x.alloc(M * d * sizeof(res_t)));
@@ -1059,12 +1077,13 @@ static int build_plan(b200t5_ctx* h, int B, int S, int Tmax) {
     int nc = B >= 512 ? 4 : (B >= 128 ? 2 : 1);
     if (h->chains_override > 0) nc = h->chains_override;
     if (nc > kMaxChains) nc = kMaxChains;
-    if (nc > B) nc = B;
+    const int groups = B / group;  // a chain holds whole prompts (beam search: `group` rows each)
+    if (nc > groups) nc = groups;
     pl->n_chains = nc;
     for (int i = 0; i < nc; ++i) {
       Plan::Chain& ch = pl->chains[i];
-      ch.b0 = static_cast<int>(static_cast<long long>(B) * i / nc);
-      ch.nb = static_cast<int>(static_cast<long long>(B) * (i + 1) / nc) - ch.b0;
+      ch.b0 = group * static_cast<int>(static_cast<long long>(groups) * i / nc);
+      ch.nb = group * static_cast<int>(static_cast<long long>(groups) * (i + 1) / nc) - ch.b0;
       TMAP(h, &ch.tm_dxn, pl->dxn.as<act_t>() + static_cast<size_t>(ch.b0) * d, ch.nb, d, 128);
       TMAP(h, &ch.tm_dctx, pl->dctx.as<act_t>() + static_cast<size_t>(ch.b0) * I, ch.nb, I, 128);
       TMAP_FFO(h, &ch.tm_dh, pl->dh.as<ffh_t>() + static_cast<size_t>(ch.b0) * F, ch.nb, F, 128);
@@ -1074,11 +1093,11 @@ static int build_plan(b200t5_ctx* h, int B, int S, int Tmax) {
   return B200T5_OK;
 }
 
-static int ensure_plan(b200t5_ctx* h, int B, int S, int Tmax) {
-  if (h->plan && h->plan->B == B && h->plan->S == S && h->plan->Tmax == Tmax) return B200T5_OK;
+static int ensure_plan(b200t5_ctx* h, int B, int S, int Tmax, int group = 1) {
+  if (h->plan && h->plan->B == B && h->plan->S == S && h->plan->Tmax == Tmax && h->plan->group == group) return B200T5_OK;
   CU_OK(h, cudaDeviceSynchronize());
   h->plan.reset();
-  return build_plan(h, B, S, Tmax);
+  return build_plan(h, B, S, Tmax, group);
 }
 
 // ================================================================== encoder
@@ -1321,6 +1340,24 @@ static int chain_head(b200t5_ctx* h, cudaStream_t s, const ChainView& v, float* 
   return B200T5_OK;
 }
 
+// The beam bookkeeping of one step, after every chain's lm_head (beam.cuh).
+static int run_beam_step(b200t5_ctx* h, cudaStream_t s) {
+  Plan& p = *h->plan;
+  const Cfg& c = h->c;
+  const int rows = p.B, prompts = p.B / p.beam_k;
+  const BeamDev bd = p.beam.dev(rows);
+  DecodeState* st = p.state.as<DecodeState>();
+  CU_OK(h, launch_kernel(beam_row_kernel, dim3(rows), dim3(kBeamRowThreads), 0, s, false, bd, c.V, static_cast<const DecodeState*>(st),
+                         static_cast<const int*>(p.unfinished.as<int>())));
+  CU_OK(h, launch_kernel(beam_select_kernel, dim3(prompts), dim3(32), 0, s, false, bd, c.V, st, p.unfinished.as<int>(),
+                         p.live_extent.as<int>(), static_cast<const act_t*>(h->shared.as<act_t>()), p.dx.as<res_t>(), c.d));
+  CU_OK(h, launch_kernel(beam_reorder_kernel, dim3(c.Ld * 2 * c.H, prompts), dim3(kBeamReorderThreads), 0, s, false,
+                         p.self_kv.as<act_t>(), bd, static_cast<const int*>(p.unfinished.as<int>()), static_cast<const DecodeState*>(st),
+                         c.H, p.Tmax, p.beam.moved.as<unsigned long long>()));
+  h->launches += 3;
+  return B200T5_OK;
+}
+
 // All chains of one step. `fork` (used while capturing the step graph) runs the chains on their own streams, so
 // that one chain's HBM-streaming cross-attention overlaps the other chain's latency-bound GEMM phases.
 static int run_decode_step(b200t5_ctx* h, cudaStream_t s, bool fork, float* logits_out, int ldl, long long eos,
@@ -1330,6 +1367,10 @@ static int run_decode_step(b200t5_ctx* h, cudaStream_t s, bool fork, float* logi
   const int nc = p.n_chains;
   ChainView v[kMaxChains];
   for (int i = 0; i < nc; ++i) v[i] = chain_view(h, p.chains[i]);
+  if (!logits_out && p.beam_k) {  // beam search: the lm_head stores the fp32 logits for beam_row_kernel
+    logits_out = p.beam.logits.as<float>();
+    ldl = c.V;
+  }
   if (fork && nc > 1) {
     cudaStream_t cs[kMaxChains];
     cs[0] = s;
@@ -1360,6 +1401,7 @@ static int run_decode_step(b200t5_ctx* h, cudaStream_t s, bool fork, float* logi
       TRY(chain_head(h, s, v[i], logits_out, ldl, eos, pad, min_new));
     }
   }
+  if (p.beam_k && logits_out == p.beam.logits.as<float>()) TRY(run_beam_step(h, s));
   // joins every chain; not PDL-launched so that it sees all of them complete
   CU_OK(h, launch_kernel(advance_step_kernel, dim3(1), dim3(32), 0, s, false, p.state.as<DecodeState>(),
                          h->profile_xattn ? p.xs_stamps.as<unsigned long long>() : static_cast<unsigned long long*>(nullptr),
@@ -1382,7 +1424,7 @@ static int ensure_graph(b200t5_ctx* h, long long eos, long long pad, int min_new
   const int want = pick_xattn(h, fill);
   p.xattn_stream = want != 0;
   if (p.gexec && p.g_eos == eos && p.g_pad == pad && p.g_min_new == min_new && p.g_stream == (p.stream_mode ? 1 : 0) && p.g_xattn == want &&
-      p.g_proc == (p.proc_on ? 1 : 0) && p.g_score == p.score_on)
+      p.g_proc == (p.proc_on ? 1 : 0) && p.g_score == p.score_on && p.g_beam == p.beam_k)
     return B200T5_OK;
   if (p.gexec) cudaGraphExecDestroy(p.gexec);
   if (p.graph) cudaGraphDestroy(p.graph);
@@ -1411,6 +1453,7 @@ static int ensure_graph(b200t5_ctx* h, long long eos, long long pad, int min_new
   p.g_xattn = want;
   p.g_proc = p.proc_on ? 1 : 0;
   p.g_score = p.score_on;
+  p.g_beam = p.beam_k;
   return B200T5_OK;
 }
 
@@ -1656,6 +1699,7 @@ static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* m
   TRY(ensure_plan(h, B, S, T));
   Plan& p = *h->plan;
   p.stream_mode = false;
+  p.beam_k = 0;
   TRY(setup_proc(h, a.ph, s));
   TRY(setup_score(h, a.sh, s));
   h->launches = 0;
@@ -1765,6 +1809,192 @@ extern "C" int b200t5_generate_host_scored(b200t5_handle h, const int64_t* input
   return B200T5_OK;
 }
 
+// ================================================================== beam search
+static int parse_beam(b200t5_ctx* h, const b200t5_beam_params* bp) {
+  if (!bp) return fail(h, B200T5_EINVAL, "null beam params");
+  if (bp->num_beams < 2 || bp->num_beams > kBeamMax) return fail(h, B200T5_EINVAL, "num_beams=%d outside [2, %d]", bp->num_beams, kBeamMax);
+  if (bp->num_return_sequences < 1 || bp->num_return_sequences > bp->num_beams)
+    return fail(h, B200T5_EINVAL, "num_return_sequences=%d outside [1, num_beams=%d]", bp->num_return_sequences, bp->num_beams);
+  if (bp->early_stopping < 0 || bp->early_stopping > 2) return fail(h, B200T5_EINVAL, "early_stopping=%d outside {0, 1, 2}", bp->early_stopping);
+  if (!std::isfinite(bp->length_penalty)) return fail(h, B200T5_EINVAL, "length_penalty is not finite");
+  return B200T5_OK;
+}
+
+// The plan's beam state and result staging, sized by the plan (B = prompts * k rows, Tmax): allocated once per plan.
+static int ensure_beam_bufs(b200t5_ctx* h, Plan& p) {
+  BeamBufs& b = p.beam;
+  if (b.prm.p) return B200T5_OK;
+  const size_t rows = static_cast<size_t>(p.B), T = static_cast<size_t>(p.Tmax), prompts = rows / p.group;
+  CU_OK(h, b.logits.alloc(rows * h->c.V * 4));
+  CU_OK(h, b.cand_lp.alloc(rows * kBeamCand * 4));
+  CU_OK(h, b.cand_tok.alloc(rows * kBeamCand * 4));
+  CU_OK(h, b.run_score.alloc(rows * 4));
+  CU_OK(h, b.hist_par.alloc(T * rows * 4));
+  CU_OK(h, b.hist_tok.alloc(T * rows * 4));
+  CU_OK(h, b.hist_lp.alloc(T * rows * 4));
+  CU_OK(h, b.fin.alloc(prompts * kBeamMax * sizeof(BeamFin)));
+  CU_OK(h, b.heur.alloc(prompts * 4));
+  CU_OK(h, b.parent.alloc(rows * 4));
+  CU_OK(h, b.len_scale.alloc(T * 4));
+  CU_OK(h, b.moved.alloc(8));
+  CU_OK(h, b.prm.alloc(sizeof(BeamParams)));
+  p.g_beam = -1;
+  return B200T5_OK;
+}
+
+// fp32(1 / (l ** length_penalty)) for l = 1..T, the reciprocal taken in double (oracle/beam.py: length_scale)
+static std::vector<float> beam_len_scale(double length_penalty, int T) {
+  std::vector<float> v(T);
+  for (int l = 1; l <= T; ++l) v[l - 1] = static_cast<float>(1.0 / pow(static_cast<double>(l), length_penalty));
+  return v;
+}
+
+// A static batch of B prompts as B * k decode rows; the results stay in the plan's beam state (beam_output_kernel).
+static int generate_beam_impl(b200t5_ctx* h, const long long* ids, const long long* mask, int Bp, int S, const b200t5_gen_params* gp,
+                              const b200t5_beam_params* bp, const CallArgs& a, cudaStream_t s) {
+  const Cfg& c = h->c;
+  const int T = a.T, k = bp->num_beams, rows = Bp * k;
+  const int poll = gp->poll_interval > 0 ? gp->poll_interval : 8;
+  if (rows > 65535) return fail(h, B200T5_EINVAL, "B * num_beams = %d rows is too many", rows);
+  TRY(ensure_plan(h, rows, S, T, k));
+  Plan& p = *h->plan;
+  p.stream_mode = false;
+  p.proc_on = false;
+  p.score_on = 0;
+  p.beam_k = k;
+  TRY(ensure_beam_bufs(h, p));
+  const BeamDev bd = p.beam.dev(rows);
+  const BeamParams prm{k, T, a.min_new, static_cast<int>(a.eos), bp->early_stopping, bp->early_stopping == 2 && bp->length_penalty > 0.0};
+  const std::vector<float> ls = beam_len_scale(bp->length_penalty, T);
+  CU_OK(h, cudaMemcpyAsync(p.beam.prm.p, &prm, sizeof(prm), cudaMemcpyHostToDevice, s));
+  CU_OK(h, cudaMemcpyAsync(p.beam.len_scale.p, ls.data(), ls.size() * 4, cudaMemcpyHostToDevice, s));
+  h->launches = 0;
+  CU_OK(h, cudaEventRecord(h->ev[0], s));
+  // The encoder runs on row b*k of each prompt only (the other rows have extent 0 in its pass, as in a slot-pool
+  // admission); beam_replicate_kernel then gives the prompt's other rows its cross-attention K/V. The unpacked encoder
+  // (S > kEncPackMaxS) takes no such row selection and runs every row.
+  const bool packed = S <= kEncPackMaxS;
+  const size_t rb = static_cast<size_t>(S) * 8;
+  for (int j = 0; j < (packed ? 1 : k); ++j) {
+    CU_OK(h, cudaMemcpy2DAsync(p.ids_dev.as<long long>() + static_cast<size_t>(j) * S, k * rb, ids, rb, rb, Bp, cudaMemcpyDeviceToDevice, s));
+    if (mask) CU_OK(h, cudaMemcpy2DAsync(p.mask_dev.as<long long>() + static_cast<size_t>(j) * S, k * rb, mask, rb, rb, Bp, cudaMemcpyDeviceToDevice, s));
+  }
+  const int* row_on = nullptr;
+  if (packed) {
+    for (int r = 0; r < rows; ++r) p.h_admit[r] = r % k == 0;
+    CU_OK(h, cudaMemcpyAsync(p.admit.p, p.h_admit, static_cast<size_t>(rows) * 4, cudaMemcpyHostToDevice, s));
+    row_on = p.admit.as<int>();
+  }
+  TRY(run_encoder(h, p.ids_dev.as<long long>(), mask ? p.mask_dev.as<long long>() : nullptr, s, row_on));
+  TRY(run_cross_kv(h, s));
+  if (packed) {
+    beam_replicate_kernel<<<dim3(c.Ld * 2 * c.H, rows), 256, 0, s>>>(p.cross_kv.as<act_t>(), p.extent.as<int>(), p.key_ok.as<unsigned char>(),
+                                                                     rows, k, c.H, S);
+    h->launches++;
+  }
+  const double valid = packed ? static_cast<double>(p.rows_valid) * k : static_cast<double>(p.rows_valid);
+  TRY(ensure_graph(h, a.eos, a.pad, 0, valid / (static_cast<double>(rows) * S)));
+  CU_OK(h, cudaMemcpyAsync(p.live_extent.p, p.extent.p, static_cast<size_t>(rows) * 4, cudaMemcpyDeviceToDevice, s));
+  CU_OK(h, cudaMemcpyAsync(p.live_key_ok.p, p.key_ok.p, static_cast<size_t>(rows) * S, cudaMemcpyDeviceToDevice, s));
+  decode_init_kernel<<<rows, 128, 0, s>>>(p.state.as<DecodeState>(), p.unfinished.as<int>(), p.batch.ids.as<long long>(),
+                                          p.batch.len.as<int>(), T + 1, rows, a.start, a.pad, h->shared.as<act_t>(), p.dx.as<res_t>(), c.d);
+  beam_init_kernel<<<(std::max(rows, Bp * kBeamMax) + 255) / 256, 256, 0, s>>>(bd, Bp, k);
+  h->launches += 2;
+  CU_OK(h, cudaMemsetAsync(p.beam.moved.p, 0, 8, s));
+  CU_OK(h, cudaGetLastError());
+  CU_OK(h, cudaEventRecord(h->ev[1], s));
+  int steps = 0;
+  for (int t = 0; t < T; ++t) {
+    if (t % kStepsPerGraph == 0 && t + kStepsPerGraph <= T && poll % kStepsPerGraph == 0) {
+      CU_OK(h, cudaGraphLaunch(p.gexec8, s));
+      h->launches += static_cast<int64_t>(p.graph_nodes) * kStepsPerGraph;
+      steps += kStepsPerGraph;
+      t += kStepsPerGraph - 1;
+    } else {
+      CU_OK(h, cudaGraphLaunch(p.gexec, s));
+      h->launches += p.graph_nodes;
+      ++steps;
+    }
+    if ((t + 1) % poll == 0 && t + 1 < T) {
+      // every prompt retired: its finished set can no longer change
+      CU_OK(h, cudaMemcpyAsync(p.h_state, p.state.p, sizeof(DecodeState), cudaMemcpyDeviceToHost, s));
+      CU_OK(h, cudaStreamSynchronize(s));
+      if (p.h_state->finished_rows >= rows) break;
+    }
+  }
+  CU_OK(h, cudaEventRecord(h->ev[2], s));
+  h->last_steps = steps;
+  h->ev_valid = true;
+  return B200T5_OK;
+}
+
+static int beam_output(b200t5_ctx* h, int Bp, const b200t5_beam_params* bp, long long start, long long pad, int64_t* seq, int32_t* len,
+                       float* sc, int64_t* bidx, float* lp, cudaStream_t s) {
+  Plan& p = *h->plan;
+  const int n = Bp * bp->num_return_sequences;
+  beam_output_kernel<<<(n + 127) / 128, 128, 0, s>>>(p.beam.dev(p.B), Bp, bp->num_return_sequences, reinterpret_cast<long long*>(seq), len, sc,
+                                                     reinterpret_cast<long long*>(bidx), lp, start, pad);
+  h->launches++;
+  CU_OK(h, cudaGetLastError());
+  return B200T5_OK;
+}
+
+extern "C" int b200t5_generate_beam(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                                    const b200t5_gen_params* params, const b200t5_beam_params* beam, const b200t5_beam_io* io,
+                                    void* stream) {
+  CallArgs a;
+  if (!io) return fail(h, B200T5_EINVAL, "null beam io");
+  TRY(set_up_call(h, B, S, B, params, input_ids, io->sequences, io->lengths, nullptr, nullptr, false, &a));
+  TRY(parse_beam(h, beam));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  TRY(generate_beam_impl(h, reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(attention_mask), B, S,
+                         params, beam, a, s));
+  return beam_output(h, B, beam, a.start, a.pad, io->sequences, io->lengths, io->sequences_scores, io->beam_indices, io->token_logprobs, s);
+}
+
+extern "C" int b200t5_generate_host_beam(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                                         const b200t5_gen_params* params, const b200t5_beam_params* beam, const b200t5_beam_io* io) {
+  CallArgs a;
+  if (!io) return fail(h, B200T5_EINVAL, "null beam io");
+  TRY(set_up_call(h, B, S, B, params, input_ids, io->sequences, io->lengths, nullptr, nullptr, true, &a));
+  TRY(parse_beam(h, beam));
+  cudaStream_t s = h->exec_stream;
+  const size_t nb = static_cast<size_t>(B) * S * 8;
+  const size_t n = static_cast<size_t>(B) * beam->num_return_sequences, T = static_cast<size_t>(a.T);
+  DevBuf in_ids, in_mask, o_seq, o_len, o_sc, o_bi, o_lp;
+  CU_OK(h, in_ids.alloc(nb));
+  CU_OK(h, cudaMemcpyAsync(in_ids.p, input_ids, nb, cudaMemcpyHostToDevice, s));
+  if (attention_mask) {
+    CU_OK(h, in_mask.alloc(nb));
+    CU_OK(h, cudaMemcpyAsync(in_mask.p, attention_mask, nb, cudaMemcpyHostToDevice, s));
+  }
+  CU_OK(h, o_seq.alloc(n * (T + 1) * 8));
+  CU_OK(h, o_len.alloc(n * 4));
+  CU_OK(h, o_sc.alloc(n * 4));
+  CU_OK(h, o_bi.alloc(n * T * 8));
+  CU_OK(h, o_lp.alloc(n * T * 4));
+  TRY(generate_beam_impl(h, in_ids.as<long long>(), attention_mask ? in_mask.as<long long>() : nullptr, B, S, params, beam, a, s));
+  TRY(beam_output(h, B, beam, a.start, a.pad, o_seq.as<int64_t>(), o_len.as<int32_t>(), o_sc.as<float>(), o_bi.as<int64_t>(),
+                  o_lp.as<float>(), s));
+  CU_OK(h, cudaMemcpyAsync(io->sequences, o_seq.p, o_seq.bytes, cudaMemcpyDeviceToHost, s));
+  CU_OK(h, cudaMemcpyAsync(io->lengths, o_len.p, o_len.bytes, cudaMemcpyDeviceToHost, s));
+  if (io->sequences_scores) CU_OK(h, cudaMemcpyAsync(io->sequences_scores, o_sc.p, o_sc.bytes, cudaMemcpyDeviceToHost, s));
+  if (io->beam_indices) CU_OK(h, cudaMemcpyAsync(io->beam_indices, o_bi.p, o_bi.bytes, cudaMemcpyDeviceToHost, s));
+  if (io->token_logprobs) CU_OK(h, cudaMemcpyAsync(io->token_logprobs, o_lp.p, o_lp.bytes, cudaMemcpyDeviceToHost, s));
+  CU_OK(h, cudaStreamSynchronize(s));
+  return B200T5_OK;
+}
+
+extern "C" int b200t5_get_beam_stats(b200t5_handle h, double* reorder_bytes, int32_t* steps) {
+  if (!h || !reorder_bytes || !steps) return fail(h, B200T5_EINVAL, "null argument");
+  if (!h->plan || !h->plan->beam.moved.p) return fail(h, B200T5_ESTATE, "no beam call yet");
+  unsigned long long v = 0;
+  CU_OK(h, cudaMemcpy(&v, h->plan->beam.moved.p, 8, cudaMemcpyDeviceToHost));
+  *reorder_bytes = static_cast<double>(v);
+  *steps = h->last_steps;
+  return B200T5_OK;
+}
+
 // ================================================================== slot pool (continuous batching)
 // N prompts through a pool of `pool` decode slots. A slot whose row has finished (EOS or max_new tokens) is
 // retired at the next poll and refilled with the next prompt: an encoder pass over the newly admitted prompts
@@ -1814,6 +2044,7 @@ extern "C" int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* inp
     p.g_stream = -1;
   }
   p.stream_mode = true;
+  p.beam_k = 0;
   TRY(setup_proc(h, a.ph, s));
   TRY(setup_score(h, a.sh, s));
   double fill = 1.0;
@@ -2139,6 +2370,7 @@ extern "C" int b200t5_decode_logits(b200t5_handle h, const int64_t* input_ids, c
   TRY(run_encoder(h, reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(attention_mask), s));
   TRY(run_cross_kv(h, s));
   p.stream_mode = false;
+  p.beam_k = 0;
   p.xattn_stream = pick_xattn(h, static_cast<double>(p.rows_valid) / (static_cast<double>(B) * S)) != 0;
   CU_OK(h, cudaMemcpyAsync(p.live_extent.p, p.extent.p, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToDevice, s));
   CU_OK(h, cudaMemcpyAsync(p.live_key_ok.p, p.key_ok.p, static_cast<size_t>(B) * S, cudaMemcpyDeviceToDevice, s));
@@ -2443,6 +2675,64 @@ extern "C" int b200t5_test_ffo(int device, const void* A, const void* W, void* R
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_ffo: %s", cudaGetErrorString(e));
   return B200T5_OK;
 #endif
+}
+
+extern "C" int b200t5_test_beam_step(int device, const float* logits, int B, int k, int V, int step, int T, int eos, int min_new,
+                                     double length_penalty, int early_stopping, float* run_score, void* fin, int32_t* heur, float* lse,
+                                     float* cand_lp, int32_t* cand_tok, int32_t* parent, int32_t* token, int32_t* retired, void* stream) {
+  int rc = hook_device(device);
+  if (rc < 0) return rc;
+  if (B < 1 || k < 1 || k > kBeamMax || V < 2 * k || step < 0 || step >= T || early_stopping < 0 || early_stopping > 2)
+    return fail(nullptr, B200T5_EINVAL, "bad beam step arguments");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int rows = B * k;
+  DevBuf prm, ls, hp, ht, hl, st, unf;
+  const BeamParams bp{k, T, min_new, eos, early_stopping, early_stopping == 2 && length_penalty > 0.0};
+  const std::vector<float> lsv = beam_len_scale(length_penalty, T);
+  const std::vector<int> ones(rows, 1);
+  if (prm.alloc(sizeof(bp)) || ls.alloc(T * 4) || hp.alloc(static_cast<size_t>(T) * rows * 4) || ht.alloc(static_cast<size_t>(T) * rows * 4) ||
+      hl.alloc(static_cast<size_t>(T) * rows * 4) || st.alloc(sizeof(DecodeState)) || unf.alloc(rows * 4))
+    return fail(nullptr, B200T5_ECUDA, "allocation failed");
+  CU_OK(nullptr, cudaMemcpy(prm.p, &bp, sizeof(bp), cudaMemcpyHostToDevice));
+  CU_OK(nullptr, cudaMemcpy(ls.p, lsv.data(), T * 4, cudaMemcpyHostToDevice));
+  CU_OK(nullptr, cudaMemcpy(unf.p, ones.data(), rows * 4, cudaMemcpyHostToDevice));
+  set_state_kernel<<<1, 1, 0, s>>>(st.as<DecodeState>(), step);
+  const BeamDev d{prm.as<BeamParams>(), ls.as<float>(), logits, lse, cand_lp, cand_tok, run_score, hp.as<int>(), ht.as<int>(), hl.as<float>(),
+                  static_cast<BeamFin*>(fin), heur, parent, rows};
+  beam_row_kernel<<<rows, kBeamRowThreads, 0, s>>>(d, V, st.as<DecodeState>(), unf.as<int>());
+  beam_select_kernel<<<B, 32, 0, s>>>(d, V, st.as<DecodeState>(), unf.as<int>(), nullptr, nullptr, nullptr, 0);
+  cudaError_t e = cudaMemcpyAsync(token, ht.as<int>() + static_cast<size_t>(step) * rows, rows * 4, cudaMemcpyDeviceToDevice, s);
+  std::vector<int> u(rows);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(u.data(), unf.p, rows * 4, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  for (int& x : u) x = !x;
+  if (e == cudaSuccess) e = cudaMemcpy(retired, u.data(), rows * 4, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "beam step: %s", cudaGetErrorString(e));
+  return B200T5_OK;
+}
+
+extern "C" int b200t5_test_beam_reorder(int device, void* kv, int planes, int B, int k, int H, int Tmax, int step, const int32_t* parent,
+                                        void* stream) {
+  int rc = hook_device(device);
+  if (rc < 0) return rc;
+  if (planes < 1 || B < 1 || k < 1 || k > kBeamMax || H < 1 || step < 0 || step >= Tmax) return fail(nullptr, B200T5_EINVAL, "bad reorder arguments");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  DevBuf prm, st, unf;
+  const BeamParams bp{k, Tmax, 0, 0, 0, 0};
+  const std::vector<int> ones(B * k, 1);
+  if (prm.alloc(sizeof(bp)) || st.alloc(sizeof(DecodeState)) || unf.alloc(B * k * 4)) return fail(nullptr, B200T5_ECUDA, "allocation failed");
+  CU_OK(nullptr, cudaMemcpy(prm.p, &bp, sizeof(bp), cudaMemcpyHostToDevice));
+  CU_OK(nullptr, cudaMemcpy(unf.p, ones.data(), B * k * 4, cudaMemcpyHostToDevice));
+  set_state_kernel<<<1, 1, 0, s>>>(st.as<DecodeState>(), step);
+  BeamDev d{};
+  d.prm = prm.as<BeamParams>();
+  d.parent = const_cast<int*>(parent);
+  d.rows = B * k;
+  beam_reorder_kernel<<<dim3(planes * H, B), kBeamReorderThreads, 0, s>>>(static_cast<act_t*>(kv), d, unf.as<int>(), st.as<DecodeState>(), H, Tmax,
+                                                                         nullptr);
+  cudaError_t e = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "beam reorder: %s", cudaGetErrorString(e));
+  return B200T5_OK;
 }
 
 extern "C" int b200t5_test_rmsnorm(int device, const void* x, const void* w, void* y, int M, int d, float eps, void* stream) {

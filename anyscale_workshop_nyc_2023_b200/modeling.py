@@ -144,15 +144,51 @@ def logits_processor_args(kw: Dict[str, Any], eos_ids, default_eos: int, vocab_s
     return _LogitsArgs(p, arrays, eos_list) if active else None
 
 
+MAX_BEAMS = 16  # b200t5_beam_params.num_beams
+_EARLY_STOPPING = {False: 0, True: 1, "never": 2}
+
+
+def beam_params(num_beams, kw: Dict[str, Any], eos_ids, default_eos: int, vocab_size: int) -> Optional[_lib.BeamParams]:
+    """b200t5_beam_params of a generate call, checked as transformers checks them (ValueError), or None for num_beams=1:
+    greedy decoding. What the CUDA beam path does not implement raises NotImplementedError naming the argument: more
+    than MAX_BEAMS beams, several EOS ids, and logits processors that would change anything."""
+    if num_beams is None or (not isinstance(num_beams, bool) and num_beams == 1):
+        return None
+    if isinstance(num_beams, bool) or int(num_beams) != num_beams or num_beams < 1:
+        raise ValueError(f"`num_beams` has to be a positive integer, but is {num_beams}")
+    k = int(num_beams)
+    if k > MAX_BEAMS:
+        raise NotImplementedError(f"generate(num_beams={k}) is not supported by the CUDA path: at most {MAX_BEAMS} beams")
+    n = kw.get("num_return_sequences")
+    n = 1 if n is None else n
+    if isinstance(n, bool) or int(n) != n or not 1 <= n <= k:
+        raise ValueError(f"`num_return_sequences` ({n}) has to be between 1 and `num_beams` ({k})")
+    es = kw.get("early_stopping")
+    es = False if es is None else es
+    if not (isinstance(es, bool) or es == "never"):
+        raise ValueError(f"`early_stopping` must be a boolean or 'never', but is {es}")
+    lp = kw.get("length_penalty")
+    lp = 1.0 if lp is None else float(lp)
+    if not np.isfinite(lp):
+        raise ValueError(f"`length_penalty` must be finite, but is {lp}")
+    if eos_ids is not None and len(eos_ids) > 1:
+        raise NotImplementedError("generate(eos_token_id=[...]) with several ids and num_beams > 1 is not supported by the CUDA path")
+    for name in LOGITS_PROCESSOR_KWARGS:
+        if kw.get(name) is not None and logits_processor_args({name: kw[name]}, None, default_eos, vocab_size) is not None:
+            raise NotImplementedError(f"generate({name}=...) with num_beams > 1 is not supported by the CUDA path")
+    return _lib.BeamParams(num_beams=k, num_return_sequences=int(n), length_penalty=lp, early_stopping=_EARLY_STOPPING[es])
+
+
 class TokenScores:
     """What `generate(..., output_scores=True)` returns as `.scores`: per generated position, the chosen token's
     processed score (`token_logits`) and its log-softmax (`token_logprobs`), fp32 [B, T'], 0 after a row's EOS.
     NOT transformers' tuple of T' tensors [B, vocab]: the fused lm_head epilogue never writes the vocabulary-wide
     scores. `compute_transition_scores` accepts it in place of that tuple."""
 
-    def __init__(self, token_logprobs, token_logits):
+    def __init__(self, token_logprobs, token_logits, beam: bool = False):
         self.token_logprobs = token_logprobs
         self.token_logits = token_logits
+        self.beam = beam  # of a beam-search call: one row per returned hypothesis, aligned with its sequence
 
     def __len__(self):
         return int(self.token_logprobs.shape[1])
@@ -169,6 +205,19 @@ class GenerateOutput:
 
     def __getitem__(self, key):
         return getattr(self, key)
+
+
+class BeamGenerateOutput(GenerateOutput):
+    """`generate(num_beams=k, return_dict_in_generate=True)`: `.sequences` [B*n, 1+T'] as a plain call returns,
+    `.sequences_scores` fp32 [B*n] (the length-penalised scores), `.beam_indices` int64 [B*n, T'] (transformers' b*k + beam
+    of each step, -1 after a hypothesis ends) and, with output_scores=True, `.scores`: a TokenScores whose rows are the
+    returned hypotheses' token log-probabilities (transformers' beam scores are log-probabilities, so token_logits holds
+    the same values)."""
+
+    def __init__(self, sequences, sequences_scores, beam_indices, scores: Optional[TokenScores] = None):
+        super().__init__(sequences, scores)
+        self.sequences_scores = sequences_scores
+        self.beam_indices = beam_indices
 
 
 def generate_output_flags(kw: Dict[str, Any]):
@@ -403,9 +452,10 @@ class B200T5ForConditionalGeneration:
             input_ids = unused.pop("inputs", None)
         if input_ids is None:
             raise ValueError("input_ids is required")
-        if do_sample or (num_beams is not None and num_beams != 1):
-            raise NotImplementedError("only greedy decoding (do_sample=False, num_beams=1) is implemented")
-        for k in ("temperature", "top_k", "top_p", "num_return_sequences"):
+        if do_sample:
+            raise NotImplementedError("only greedy decoding and beam search (do_sample=False) are implemented")
+        bp = beam_params(num_beams, unused, _eos_ids(eos_token_id), self.generation_config.eos_token_id, self.config.vocab_size)
+        for k in ("temperature", "top_k", "top_p") + (() if bp is not None else ("num_return_sequences",)):
             v = unused.get(k)
             if v is not None and not (isinstance(v, (int, float)) and v == 1):
                 raise NotImplementedError(f"generate({k}=...) is not supported by the CUDA path")
@@ -419,6 +469,11 @@ class B200T5ForConditionalGeneration:
         host = torch.as_tensor(input_ids)
         if host.dim() != 2:
             raise ValueError(f"input_ids must be [batch, seq], got {tuple(host.shape)}")
+        if bp is not None:
+            seq, scores, bidx, logp = self._generate_beam(host, attention_mask, gp, bp)
+            if not as_dict:
+                return seq
+            return BeamGenerateOutput(seq, scores, bidx, TokenScores(logp, logp, beam=True) if want_scores else None)
         if as_dict:
             if not want_scores:  # the unchanged greedy call, wrapped
                 return GenerateOutput(self.generate(input_ids=input_ids, attention_mask=attention_mask, max_new_tokens=gp.max_new_tokens,
@@ -454,8 +509,8 @@ class B200T5ForConditionalGeneration:
         deviation: positions after a row's EOS are 0 (transformers reports the score of the pad token it fed)."""
         if not isinstance(scores, TokenScores):
             raise TypeError("scores must be the `.scores` of this model's generate(..., output_scores=True)")
-        if beam_indices is not None:
-            raise NotImplementedError("beam search is not implemented")
+        if beam_indices is not None and not scores.beam:
+            raise ValueError("beam_indices belong to the output of a beam-search generate (num_beams > 1)")
         return scores.token_logprobs if normalize_logits else scores.token_logits
 
     @torch.no_grad()
@@ -493,6 +548,42 @@ class B200T5ForConditionalGeneration:
             out, lens, logp, logit = (torch.cat([p[i] for p in parts], dim=0) for i in range(4))
         steps = T if labels is not None else int(lens.max().item())
         return out[:, : steps + 1], lens, logp[:, :steps], logit[:, :steps]
+
+    def _generate_beam(self, host: torch.Tensor, attention_mask, gp, bp):
+        """Beam search (b200t5_generate_beam) in static chunks of pool_size // num_beams prompts: (sequences [B*n, 1+T'],
+        sequences_scores [B*n], beam_indices [B*n, T'], token_logprobs [B*n, T']) on the device, T' the longest returned
+        hypothesis. beam_indices count prompts across the whole call, as transformers' do."""
+        ids, mask = self._device_inputs(host, attention_mask, gp, None)
+        B = ids.shape[0]
+        k, n = bp.num_beams, bp.num_return_sequences
+        chunk = max(1, self.pool_size // k)
+        parts = [self._generate_beam_static(ids[lo:lo + chunk], None if mask is None else mask[lo:lo + chunk], gp, bp)
+                 for lo in range(0, B, chunk)]
+        L = max(int(p[1].max().item()) for p in parts)
+        seq = torch.cat([p[0][:, : L + 1] for p in parts], dim=0)  # (each chunk is padded to max_new_tokens)
+        bidx = torch.cat([torch.where(p[3][:, :L] >= 0, p[3][:, :L] + i * chunk * k, p[3][:, :L]) for i, p in enumerate(parts)], dim=0)
+        return seq, torch.cat([p[2] for p in parts]), bidx, torch.cat([p[4][:, :L] for p in parts], dim=0)
+
+    def _generate_beam_static(self, ids: torch.Tensor, mask: Optional[torch.Tensor], gp, bp):
+        B, S = ids.shape
+        ids = ids.contiguous()
+        mask = None if mask is None else mask.contiguous()
+        T, rows = gp.max_new_tokens, B * bp.num_return_sequences
+        dev = self._device
+        with torch.cuda.device(self._index):
+            seq = torch.empty((rows, T + 1), dtype=torch.long, device=dev)
+            lens = torch.empty((rows,), dtype=torch.int32, device=dev)
+            scores = torch.empty((rows,), dtype=torch.float32, device=dev)
+            bidx = torch.empty((rows, T), dtype=torch.long, device=dev)
+            logp = torch.empty((rows, T), dtype=torch.float32, device=dev)
+            io = _lib.BeamIO(*(_ptr(t) for t in (seq, lens, scores, bidx, logp)))
+            stream = torch.cuda.current_stream(dev)
+            with self._gpu_lock:
+                _chk(self, self._lib.b200t5_generate_beam(self._h, _ptr(ids), _ptr(mask), B, S, C.byref(gp), C.byref(bp), C.byref(io),
+                                                          C.c_void_p(stream.cuda_stream)), self._h)
+                self.last_lengths = lens
+                stream.synchronize()
+        return seq, lens, scores, bidx, logp
 
     def _score_io(self, logp, logit, labels):
         """b200t5_score_io over two result arrays and optional labels (torch tensors or numpy arrays, all on the side
@@ -602,10 +693,16 @@ class B200T5ForConditionalGeneration:
         gp = self._gen_params(kw.get("max_new_tokens"), kw.get("max_length"), kw.get("min_new_tokens"),
                               kw.get("min_length"), kw.get("eos_token_id"), kw.get("pad_token_id"),
                               kw.get("decoder_start_token_id"), kw.get("poll_interval", 8))
+        if kw.get("do_sample") and kw.get("num_beams") not in (None, 1):
+            raise NotImplementedError("beam sampling (do_sample=True, num_beams > 1) is not implemented")
+        bp = beam_params(kw.get("num_beams"), kw, _eos_ids(kw.get("eos_token_id")), self.generation_config.eos_token_id,
+                         self.config.vocab_size)
         lp = self._logits_args(kw, kw.get("eos_token_id"))
         ids = np.ascontiguousarray(input_ids, dtype=np.int64)
         B, S = ids.shape
         mask = self._infer_mask_np(ids, gp, lp) if attention_mask is None else np.ascontiguousarray(attention_mask, dtype=np.int64)
+        if bp is not None:
+            return self._generate_host_beam(ids, mask, gp, bp)
         out = np.empty((B, gp.max_new_tokens + 1), dtype=np.int64)
         lens = np.empty((B,), dtype=np.int32)
         want_scores = generate_output_flags(kw)[1]
@@ -625,6 +722,44 @@ class B200T5ForConditionalGeneration:
             return out[:, : steps + 1], lens, logp[:, :steps], logit[:, :steps]
         return out[:, : steps + 1], lens
 
+    def _generate_host_beam(self, ids: np.ndarray, mask: Optional[np.ndarray], gp, bp):
+        """generate_host(num_beams=k): b200t5_generate_host_beam -> (sequences [B*n, 1+T'], lengths [B*n], sequences_scores
+        [B*n], beam_indices [B*n, T'], token_logprobs [B*n, T']), numpy; in static chunks of pool_size // k prompts, as
+        generate runs them."""
+        self._check_inputs(ids, mask)
+        chunk = max(1, self.pool_size // bp.num_beams)
+        parts = [self._generate_host_beam_chunk(ids[lo:lo + chunk], None if mask is None else mask[lo:lo + chunk], gp, bp)
+                 for lo in range(0, ids.shape[0], chunk)]
+        L = max(int(p[1].max()) for p in parts)
+        k = bp.num_beams
+        return (np.concatenate([p[0][:, : L + 1] for p in parts]), np.concatenate([p[1] for p in parts]),
+                np.concatenate([p[2] for p in parts]),
+                np.concatenate([np.where(p[3][:, :L] >= 0, p[3][:, :L] + i * chunk * k, p[3][:, :L]) for i, p in enumerate(parts)]),
+                np.concatenate([p[4][:, :L] for p in parts]))
+
+    def _generate_host_beam_chunk(self, ids: np.ndarray, mask: Optional[np.ndarray], gp, bp):
+        ids = np.ascontiguousarray(ids)
+        mask = None if mask is None else np.ascontiguousarray(mask)
+        B, S = ids.shape
+        T, rows = gp.max_new_tokens, B * bp.num_return_sequences
+        seq = np.empty((rows, T + 1), np.int64)
+        lens = np.empty((rows,), np.int32)
+        scores = np.empty((rows,), np.float32)
+        bidx = np.empty((rows, T), np.int64)
+        logp = np.empty((rows, T), np.float32)
+        io = _lib.BeamIO(*(a.ctypes.data_as(C.c_void_p) for a in (seq, lens, scores, bidx, logp)))
+        with self._gpu_lock:
+            _chk(self, self._lib.b200t5_generate_host_beam(self._h, ids.ctypes.data_as(C.c_void_p),
+                                                           None if mask is None else mask.ctypes.data_as(C.c_void_p), B, S, C.byref(gp),
+                                                           C.byref(bp), C.byref(io)), self._h)
+        return seq, lens, scores, bidx, logp
+
+    def beam_stats(self) -> Dict[str, float]:
+        """Of the last beam call: bytes the self-attention cache reordering read and wrote, and the decode steps."""
+        nbytes, steps = C.c_double(), C.c_int32()
+        _chk(self, self._lib.b200t5_get_beam_stats(self._h, C.byref(nbytes), C.byref(steps)), self._h)
+        return {"reorder_bytes": nbytes.value, "steps": int(steps.value)}
+
     def generate_stream(self, input_ids: np.ndarray, attention_mask: Optional[np.ndarray] = None, *, pool: Optional[int] = None,
                         admit_min: int = 0, _gen_params=None, _logits=None, _labels=None, **kw):
         """N prompts through a pool of decode slots (b200t5_generate_stream): a slot whose row has finished is
@@ -637,6 +772,8 @@ class B200T5ForConditionalGeneration:
                                              kw.get("min_length"), kw.get("eos_token_id"), kw.get("pad_token_id"),
                                              kw.get("decoder_start_token_id"), kw.get("poll_interval", 8))
         lp = _logits if _gen_params is not None else self._logits_args(kw, kw.get("eos_token_id"))
+        if kw.get("num_beams") not in (None, 1):
+            raise NotImplementedError("generate_stream(num_beams > 1): beam search runs as static batches (generate)")
         ids = np.ascontiguousarray(input_ids, dtype=np.int64)
         if ids.ndim != 2:
             raise ValueError(f"input_ids must be [batch, seq], got {ids.shape}")

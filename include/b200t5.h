@@ -204,6 +204,40 @@ int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* input_ids, con
                                   int admit_min, int64_t* out_ids, int32_t* out_len, const b200t5_score_io* score);
 int b200t5_get_stats(b200t5_handle h, b200t5_stats* out);
 
+/* Beam search (transformers' GenerationMixin._beam_search with do_sample=False and one EOS id): each prompt decodes as
+ * num_beams rows. Length penalty: a finished hypothesis of l generated tokens scores sum(log-probs) * fp32(1 / l**p),
+ * the reciprocal taken in double. Ties: value descending, then token (beam * vocab + token across a prompt) ascending. */
+typedef struct b200t5_beam_params {
+  int32_t num_beams;             /* 2..16 */
+  int32_t num_return_sequences;  /* 1..num_beams */
+  double length_penalty;
+  int32_t early_stopping;        /* 0 False, 1 True, 2 "never" */
+} b200t5_beam_params;
+
+/* Results of a beam call, n = num_return_sequences, row b*n + i = the i-th best hypothesis of prompt b. Device pointers
+ * for b200t5_generate_beam, host pointers for b200t5_generate_host_beam. */
+typedef struct b200t5_beam_io {
+  int64_t* sequences;        /* out [B*n, max_new_tokens+1]: start token, the hypothesis (ending in EOS unless it reached
+                              * max_new_tokens), then pad_token_id */
+  int32_t* lengths;          /* out [B*n]: generated tokens of each hypothesis */
+  float* sequences_scores;   /* out, may be NULL: [B*n] length-penalised scores */
+  int64_t* beam_indices;     /* out, may be NULL: [B*n, max_new_tokens] beam of each step as b*num_beams + beam, -1 after
+                              * the hypothesis ends */
+  float* token_logprobs;     /* out, may be NULL: [B*n, max_new_tokens] each token's log-probability, 0 after the end */
+} b200t5_beam_io;
+
+/* Beam-search generate: input_ids / attention_mask as b200t5_generate; gen_params' min_new_tokens masks EOS as in greedy
+ * decoding. The encoder and the cross-attention K/V projection run once per prompt; the decode step runs B*num_beams rows.
+ * Parameters out of range return B200T5_EINVAL. Enqueued on `stream`, like b200t5_generate. */
+int b200t5_generate_beam(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                         const b200t5_gen_params* params, const b200t5_beam_params* beam, const b200t5_beam_io* io,
+                         void* stream);
+/* The same with host buffers; synchronous. */
+int b200t5_generate_host_beam(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                              const b200t5_gen_params* params, const b200t5_beam_params* beam, const b200t5_beam_io* io);
+/* Bytes the self-attention cache reordering of the last beam call read and wrote (beam_reorder_kernel), and its steps. */
+int b200t5_get_beam_stats(b200t5_handle h, double* reorder_bytes, int32_t* steps);
+
 /* ---- measurement hooks (bench.py) --------------------------------------------------- */
 /* Times the cross-attention decode kernel alone over the cross-KV arena of the last generate call, in launches of
  * `rows_per_launch` batch rows (0 = the whole batch; the step graph launches one row-chain at a time): reps sweeps
@@ -254,6 +288,20 @@ int b200t5_test_lm_process(int device, const void* x, const void* W, int M, int 
 int b200t5_test_lm_score(int device, const void* x, const void* W, int M, int V, int K, int step, int eos, int min_new,
                          const b200t5_logits_params* logits, const int64_t* hist, const int64_t* enc_ids, int S,
                          const int64_t* forced, int64_t* tokens, float* logprob, float* logit, float* vals, void* stream);
+
+/* One beam step as the step graph runs it (csrc/beam.cuh: beam_row_kernel -> beam_select_kernel) on given fp32 logits
+ * [B*k, V] (device) at decode position `step` of max_new_tokens T. In/out state (device): run_score fp32 [B*k]; fin
+ * [B][16] records {float score; int32 t, par, tok; float lp; int32 flag} (a prompt's finished set, best first, k used);
+ * heur int32 [B]. Out (device): lse fp32 [B*k]; cand_lp fp32 / cand_tok int32 [B*k][32] (each row's top 2k, best first);
+ * parent int32 [B*k] (the row each row continues); token int32 [B*k]; retired int32 [B*k] (1: the row's prompt stopped).
+ * Test hook; both builds. */
+int b200t5_test_beam_step(int device, const float* logits, int B, int k, int V, int step, int T, int eos, int min_new,
+                          double length_penalty, int early_stopping, float* run_score, void* fin, int32_t* heur, float* lse,
+                          float* cand_lp, int32_t* cand_tok, int32_t* parent, int32_t* token, int32_t* retired, void* stream);
+/* beam_reorder_kernel on a self-attention cache [planes][B*k][H][Tmax][64] of the build's 2-byte type (device): row r takes
+ * positions 0..step of row parent[r] (int32 [B*k], device, within r's prompt). Test hook; both builds. */
+int b200t5_test_beam_reorder(int device, void* kv, int planes, int B, int k, int H, int Tmax, int step, const int32_t* parent,
+                             void* stream);
 
 /* ---- parity hooks (used by tests/ only) --------------------------------------------- */
 /* Encoder last hidden state after the final RMSNorm, bf16 [B,S,d_model] (device). */
