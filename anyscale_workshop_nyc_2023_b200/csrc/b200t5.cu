@@ -17,6 +17,7 @@
 #include <algorithm>
 #include <map>
 #include <memory>
+#include <optional>
 #include <string>
 #include <vector>
 
@@ -272,12 +273,30 @@ struct ProcBufs {
 };
 
 // Beam-search state of a plan (beam.cuh), allocated by the first beam call. The step graph bakes these addresses.
+// seq / len / score / bidx / lp: the host entry point's results, written by beam_output_kernel and copied to the caller.
 struct BeamBufs {
   DevBuf logits, cand_lp, cand_tok, run_score, hist_par, hist_tok, hist_lp, fin, heur, parent, prm, len_scale, moved;
+  DevBuf seq, len, score, bidx, lp;
   BeamDev dev(int rows) const {
     return BeamDev{prm.as<BeamParams>(), len_scale.as<float>(), logits.as<float>(), nullptr, cand_lp.as<float>(), cand_tok.as<int>(),
                    run_score.as<float>(), hist_par.as<int>(), hist_tok.as<int>(), hist_lp.as<float>(), fin.as<BeamFin>(), heur.as<int>(),
                    parent.as<int>(), rows};
+  }
+};
+
+// What the step graph bakes in besides buffer addresses (the values of processors, labels and beam parameters are read
+// from device memory at replay). A call whose mode differs from the one the graph was captured for re-captures it.
+struct StepMode {
+  long long eos = -1, pad = -1;
+  int min_new = 0;
+  bool pool = false;  // slot pool: per-slot positions and the pool's results; else one position for a static batch
+  bool proc = false;  // logits processors: EpiLmHead<true, *>
+  int score = 0;      // 0 plain head, 1 EpiLmHead<*, true> + finalize_step_kernel<*, true>, 2 those with teacher forcing
+  int beam = 0;       // k > 0: the beam head (lm_head -> fp32 logits -> beam.cuh)
+  bool xattn_stream = false;  // cross-attention kernel: the TMA stream kernel, else the per-thread-load kernel
+  bool operator==(const StepMode& o) const {
+    return eos == o.eos && pad == o.pad && min_new == o.min_new && pool == o.pool && proc == o.proc && score == o.score &&
+           beam == o.beam && xattn_stream == o.xattn_stream;
   }
 };
 
@@ -314,26 +333,14 @@ struct Plan {
     size_t cap = 0;
   };
   Results batch, pool;
-  Results& res() { return stream_mode ? pool : batch; }
-  // logits processors (allocated by the first call that uses them); proc_on: this call's step runs EpiLmHead<true, *>
-  ProcBufs proc;
-  bool proc_on = false;
-  int g_proc = -1;
-  // token log-probabilities (allocated by the first call that asks for them); score_on: 0 = this call's step runs the
-  // plain head, 1 = EpiLmHead<*, true> + finalize_step_kernel<*, true>, 2 = those with teacher forcing. Part of the
-  // step graph's key, like proc_on.
-  DevBuf psum, fval, ftok;              // [B][n_tiles], [B], [B]
-  int score_on = 0;
-  int g_score = -1;
-  bool stream_mode = false;
-  int g_stream = -1;
-  // beam search: beam_k > 0 when this call's step runs the beam head (lm_head -> fp32 logits -> beam.cuh); part of the
-  // step graph's key. Every other value of a beam call lives in device memory.
+  Results& res() { return mode.pool ? pool : batch; }
+  ProcBufs proc;                 // logits processors (allocated by the first call that uses them)
+  DevBuf psum, fval, ftok;       // token log-probabilities (likewise): [B][n_tiles], [B], [B]
   BeamBufs beam;
-  int beam_k = 0;
-  int g_beam = -1;
-  int g_xattn = -1;           // cross-attention kernel baked into the step graph (0 per-thread-load, 1 stream)
-  bool xattn_stream = false;  // ... and the one launch_cross_attention issues now
+  StepMode mode;                 // what this call's steps run
+  std::optional<StepMode> graph_mode;  // what the step graphs were captured for (none: re-capture)
+  // after a reallocation of a buffer the step graph bakes: the next ensure_graph re-captures
+  void invalidate_graph() { graph_mode.reset(); }
   long long rows_valid = 0;   // valid prompt tokens of the last encoder pass (packed rows)
   int* h_unf = nullptr;    // pinned: unfinished[B] read back every graph launch
   int* h_admit = nullptr;  // pinned: [3][B] = row_on flags, slots, rows
@@ -356,8 +363,6 @@ struct Plan {
   // the same step captured kStepsPerGraph times back to back: one launch per 8 decode steps (= the poll interval)
   cudaGraph_t graph8 = nullptr;
   cudaGraphExec_t gexec8 = nullptr;
-  long long g_eos = -1, g_pad = -1;
-  int g_min_new = -1;
   // pinned staging for the host-buffer entry point and polling
   long long* h_ids = nullptr;
   long long* h_mask = nullptr;
@@ -1212,8 +1217,8 @@ static int chain_layer_pre(b200t5_ctx* h, cudaStream_t s, const ChainView& v, in
   const int B = p.B, d = c.d, I = c.I, H = c.H, T = p.Tmax;
   const bool pdl = h->use_pdl;
   // static batch: one position for all rows; slot pool: row b of the chain is at pos[b0 + b]
-  const int sstride = p.stream_mode ? 1 : 0;
-  const int* step = p.stream_mode ? p.pos.as<int>() + v.b0 : &p.state.as<DecodeState>()->step;
+  const int sstride = p.mode.pool ? 1 : 0;
+  const int* step = p.mode.pool ? p.pos.as<int>() + v.b0 : &p.state.as<DecodeState>()->step;
   DecLayerW& w = h->dec[l];
   // [kv][B][H][T][64]: a row offset of b0 is a pointer offset inside each kv plane
   act_t* skv = p.self_kv.as<act_t>() + l * (static_cast<size_t>(2) * B * I * T) + static_cast<size_t>(v.b0) * I * T;
@@ -1248,7 +1253,7 @@ static cudaError_t launch_cross_attention(b200t5_ctx* h, cudaStream_t s, bool pd
   Plan& p = *h->plan;
   const int B = p.B, S = p.S, I = c.I;
   XsStamps st{slot >= 0 && p.xs_stamps.p ? p.xs_stamps.as<unsigned long long>() : nullptr, slot >= 0 ? slot : 0};
-  if (p.xattn_stream) {
+  if (p.mode.xattn_stream) {
     const int items = nb * c.H;
     const int k_row0 = ((l * 2) * B + b0) * c.H * S, v_row0 = ((l * 2 + 1) * B + b0) * c.H * S;
     return launch_kernel(attn_cross_stream_kernel, dim3(xs_grid(items, h->num_sms)), dim3(kXsThreads),
@@ -1297,10 +1302,10 @@ static int chain_layer_post(b200t5_ctx* h, cudaStream_t s, const ChainView& v, i
 }
 
 // final norm, lm_head and either the fused arg-max + greedy bookkeeping or fp32 logits (teacher forcing)
-static int chain_head(b200t5_ctx* h, cudaStream_t s, const ChainView& v, float* logits_out, int ldl, long long eos,
-                      long long pad, int min_new) {
+static int chain_head(b200t5_ctx* h, cudaStream_t s, const ChainView& v, float* logits_out, int ldl) {
   const Cfg& c = h->c;
   Plan& p = *h->plan;
+  const StepMode& m = p.mode;
   const int d = c.d, T = p.Tmax;
   const bool pdl = h->use_pdl;
   CU_OK(h, run_rmsnorm(h, v.dx, h->dec_final_ln.as<act_t>(), v.dxn, v.nb, d, c.eps, s, pdl));
@@ -1310,7 +1315,7 @@ static int chain_head(b200t5_ctx* h, cudaStream_t s, const ChainView& v, float* 
     CU_OK(h, (launch_gemm<128, EpiStoreF32>(v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, 1, ep, h->num_sms, s, pdl)));
     return B200T5_OK;
   }
-  const bool sm = p.stream_mode;
+  const bool sm = m.pool;
   const Plan::Results& r = p.res();
   // result rows: b0.. of the static batch's, out_row[slot] of the slot pool's
   const size_t r0 = sm ? 0 : static_cast<size_t>(v.b0);
@@ -1319,24 +1324,24 @@ static int chain_head(b200t5_ctx* h, cudaStream_t s, const ChainView& v, float* 
   ep.pidx = p.pidx.as<int>() + static_cast<size_t>(v.b0) * p.n_vtiles;
   ep.n_tiles = p.n_vtiles;
   ep.step = sm ? p.pos.as<int>() + v.b0 : &p.state.as<DecodeState>()->step;
-  ep.eos = static_cast<int>(eos);
-  ep.min_new = min_new;
+  ep.eos = static_cast<int>(m.eos);
+  ep.min_new = m.min_new;
   ep.step_stride = sm ? 1 : 0;
-  if (p.proc_on) ep.pd = p.proc.dev(v.b0);
+  if (m.proc) ep.pd = p.proc.dev(v.b0);
   FinalizeArgs fa{ep.pval, ep.pidx, p.n_vtiles, p.state.as<DecodeState>(), p.unfinished.as<int>() + v.b0,
-                  r.ids.as<long long>() + r0 * (T + 1), r.len.as<int>() + r0, T + 1, eos, pad, h->shared.as<act_t>(), v.dx, d,
+                  r.ids.as<long long>() + r0 * (T + 1), r.len.as<int>() + r0, T + 1, m.eos, m.pad, h->shared.as<act_t>(), v.dx, d,
                   p.live_extent.as<int>() + v.b0, sm ? p.pos.as<int>() + v.b0 : nullptr, sm ? p.out_row.as<int>() + v.b0 : nullptr,
                   T, ep.pd, ScoreDev()};
-  if (p.score_on) {
+  if (m.score) {
     ep.psum = p.psum.as<float>() + static_cast<size_t>(v.b0) * p.n_vtiles;
     ep.fval = p.fval.as<float>() + v.b0;
     fa.sd = {ep.psum, ep.fval, p.ftok.as<int>() + v.b0, nullptr, r.lp.as<float>() + r0 * T, r.lg.as<float>() + r0 * T};
-    if (p.score_on == 2) {
+    if (m.score == 2) {
       ep.ftok = fa.sd.ftok;
       fa.sd.forced = r.forced.as<long long>() + r0 * T;
     }
   }
-  CU_OK(h, run_lm_head(h, p.proc_on, p.score_on != 0, v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, ep, fa, s, pdl));
+  CU_OK(h, run_lm_head(h, m.proc, m.score != 0, v.ch->tm_dxn, h->tm_lm, v.nb, c.V, d, ep, fa, s, pdl));
   return B200T5_OK;
 }
 
@@ -1344,7 +1349,7 @@ static int chain_head(b200t5_ctx* h, cudaStream_t s, const ChainView& v, float* 
 static int run_beam_step(b200t5_ctx* h, cudaStream_t s) {
   Plan& p = *h->plan;
   const Cfg& c = h->c;
-  const int rows = p.B, prompts = p.B / p.beam_k;
+  const int rows = p.B, prompts = p.B / p.mode.beam;
   const BeamDev bd = p.beam.dev(rows);
   DecodeState* st = p.state.as<DecodeState>();
   CU_OK(h, launch_kernel(beam_row_kernel, dim3(rows), dim3(kBeamRowThreads), 0, s, false, bd, c.V, static_cast<const DecodeState*>(st),
@@ -1360,14 +1365,13 @@ static int run_beam_step(b200t5_ctx* h, cudaStream_t s) {
 
 // All chains of one step. `fork` (used while capturing the step graph) runs the chains on their own streams, so
 // that one chain's HBM-streaming cross-attention overlaps the other chain's latency-bound GEMM phases.
-static int run_decode_step(b200t5_ctx* h, cudaStream_t s, bool fork, float* logits_out, int ldl, long long eos,
-                           long long pad, int min_new) {
+static int run_decode_step(b200t5_ctx* h, cudaStream_t s, bool fork, float* logits_out, int ldl) {
   Plan& p = *h->plan;
   const Cfg& c = h->c;
   const int nc = p.n_chains;
   ChainView v[kMaxChains];
   for (int i = 0; i < nc; ++i) v[i] = chain_view(h, p.chains[i]);
-  if (!logits_out && p.beam_k) {  // beam search: the lm_head stores the fp32 logits for beam_row_kernel
+  if (!logits_out && p.mode.beam) {  // beam search: the lm_head stores the fp32 logits for beam_row_kernel
     logits_out = p.beam.logits.as<float>();
     ldl = c.V;
   }
@@ -1385,7 +1389,7 @@ static int run_decode_step(b200t5_ctx* h, cudaStream_t s, bool fork, float* logi
       }
     }
     for (int i = 0; i < nc; ++i) {
-      TRY(chain_head(h, cs[i], v[i], logits_out, ldl, eos, pad, min_new));
+      TRY(chain_head(h, cs[i], v[i], logits_out, ldl));
       if (i > 0) {
         CU_OK(h, cudaEventRecord(h->chain_ev[i], cs[i]));
         CU_OK(h, cudaStreamWaitEvent(s, h->chain_ev[i], 0));
@@ -1398,10 +1402,10 @@ static int run_decode_step(b200t5_ctx* h, cudaStream_t s, bool fork, float* logi
         TRY(chain_layer_cross(h, s, v[i], l, i));
         TRY(chain_layer_post(h, s, v[i], l));
       }
-      TRY(chain_head(h, s, v[i], logits_out, ldl, eos, pad, min_new));
+      TRY(chain_head(h, s, v[i], logits_out, ldl));
     }
   }
-  if (p.beam_k && logits_out == p.beam.logits.as<float>()) TRY(run_beam_step(h, s));
+  if (p.mode.beam && logits_out == p.beam.logits.as<float>()) TRY(run_beam_step(h, s));
   // joins every chain; not PDL-launched so that it sees all of them complete
   CU_OK(h, launch_kernel(advance_step_kernel, dim3(1), dim3(32), 0, s, false, p.state.as<DecodeState>(),
                          h->profile_xattn ? p.xs_stamps.as<unsigned long long>() : static_cast<unsigned long long*>(nullptr),
@@ -1411,21 +1415,17 @@ static int run_decode_step(b200t5_ctx* h, cudaStream_t s, bool fork, float* logi
   return B200T5_OK;
 }
 
-// Graph of one decode step; eos/pad/min_new are baked in, so the graph is rebuilt when they change. Whether logits
-// processors run and whether the step scores its token (and is teacher-forced) are baked in too; their values are read
-// from device memory at replay.
-// The cross-attention kernel is baked in as well: `fill` = valid prompt tokens / (B * S) of the batch at hand.
+// Graphs of one decode step and of kStepsPerGraph steps, for p.mode. The cross-attention kernel is part of the mode:
+// picked here from `fill` = valid prompt tokens / (B * S) of the batch at hand.
 constexpr double kXattnStreamFill = 0.9;
-static int pick_xattn(const b200t5_ctx* h, double fill) {
-  return h->xattn_mode == 2 ? (fill >= kXattnStreamFill ? 1 : 0) : h->xattn_mode;
+static bool pick_xattn(const b200t5_ctx* h, double fill) {
+  return h->xattn_mode == 2 ? fill >= kXattnStreamFill : h->xattn_mode != 0;
 }
-static int ensure_graph(b200t5_ctx* h, long long eos, long long pad, int min_new, double fill) {
+static int ensure_graph(b200t5_ctx* h, double fill) {
   Plan& p = *h->plan;
-  const int want = pick_xattn(h, fill);
-  p.xattn_stream = want != 0;
-  if (p.gexec && p.g_eos == eos && p.g_pad == pad && p.g_min_new == min_new && p.g_stream == (p.stream_mode ? 1 : 0) && p.g_xattn == want &&
-      p.g_proc == (p.proc_on ? 1 : 0) && p.g_score == p.score_on && p.g_beam == p.beam_k)
-    return B200T5_OK;
+  p.mode.xattn_stream = pick_xattn(h, fill);
+  if (p.graph_mode == p.mode) return B200T5_OK;
+  p.invalidate_graph();
   if (p.gexec) cudaGraphExecDestroy(p.gexec);
   if (p.graph) cudaGraphDestroy(p.graph);
   if (p.gexec8) cudaGraphExecDestroy(p.gexec8);
@@ -1438,7 +1438,7 @@ static int ensure_graph(b200t5_ctx* h, long long eos, long long pad, int min_new
     const int64_t before = h->launches;
     CU_OK(h, cudaStreamBeginCapture(h->cap_stream, cudaStreamCaptureModeThreadLocal));
     int rc = B200T5_OK;
-    for (int r = 0; r < reps && rc == B200T5_OK; ++r) rc = run_decode_step(h, h->cap_stream, true, nullptr, 0, eos, pad, min_new);
+    for (int r = 0; r < reps && rc == B200T5_OK; ++r) rc = run_decode_step(h, h->cap_stream, true, nullptr, 0);
     cudaError_t e = cudaStreamEndCapture(h->cap_stream, g);
     if (!which) p.graph_nodes = static_cast<int>(h->launches - before);
     h->launches = before;
@@ -1446,14 +1446,7 @@ static int ensure_graph(b200t5_ctx* h, long long eos, long long pad, int min_new
     CU_OK(h, e);
     CU_OK(h, cudaGraphInstantiate(which ? &p.gexec8 : &p.gexec, *g, 0));
   }
-  p.g_eos = eos;
-  p.g_pad = pad;
-  p.g_min_new = min_new;
-  p.g_stream = p.stream_mode ? 1 : 0;
-  p.g_xattn = want;
-  p.g_proc = p.proc_on ? 1 : 0;
-  p.g_score = p.score_on;
-  p.g_beam = p.beam_k;
+  p.graph_mode = p.mode;
   return B200T5_OK;
 }
 
@@ -1550,7 +1543,6 @@ static int parse_logits_params(b200t5_ctx* h, int V, const b200t5_logits_params*
 // launched). A reallocation drops the step graph, which bakes the addresses.
 static int setup_proc(b200t5_ctx* h, const ProcHost& ph, cudaStream_t s) {
   Plan& p = *h->plan;
-  p.proc_on = ph.on;
   if (!ph.on) return B200T5_OK;
   const int W = (h->c.V + 31) / 32;
   const int cap = std::min(W * 32, p.Tmax + 1 + p.S + ph.cfg.n_bad);  // distinct bans of one step, at most
@@ -1558,7 +1550,7 @@ static int setup_proc(b200t5_ctx* h, const ProcHost& ph, cudaStream_t s) {
     CU_OK(h, cudaStreamSynchronize(s));
     CU_OK(h, p.proc.alloc(p.B, p.S, W, std::max(cap, p.proc.ban_cap), std::max<size_t>(ph.bad_ids.size(), 2 * p.proc.n_bad_ids),
                           std::max<size_t>(ph.bad_off.size(), 2 * p.proc.n_bad_off)));
-    p.g_proc = -1;
+    p.invalidate_graph();
   }
   CU_OK(h, p.proc.upload(ph, s));
   return B200T5_OK;
@@ -1567,7 +1559,7 @@ static int setup_proc(b200t5_ctx* h, const ProcHost& ph, cudaStream_t s) {
 // b200t5_score_io -> ScoreHost for a call of `rows` rows and T = max_new_tokens. `host`: the struct's pointers are
 // host pointers (else device pointers: the labels are read back to be checked). The destinations are set by the
 // caller, which knows where the results must go.
-static int parse_score(b200t5_ctx* h, const b200t5_score_io* sc, long long rows, int T, bool host, bool proc_on, ScoreHost* sh) {
+static int parse_score(b200t5_ctx* h, const b200t5_score_io* sc, long long rows, int T, bool host, bool proc, ScoreHost* sh) {
   *sh = ScoreHost();
   if (!sc) return B200T5_OK;
   if (!sc->token_logprobs) return fail(h, B200T5_EINVAL, "score: token_logprobs is NULL");
@@ -1575,7 +1567,7 @@ static int parse_score(b200t5_ctx* h, const b200t5_score_io* sc, long long rows,
   if (!sc->forced_ids) return B200T5_OK;
   const int L = sc->forced_len;
   if (L < 1 || L > T) return fail(h, B200T5_EINVAL, "score: forced_len=%d outside [1, max_new_tokens=%d]", L, T);
-  if (proc_on) return fail(h, B200T5_EINVAL, "score: forced_ids cannot be combined with logits processors");
+  if (proc) return fail(h, B200T5_EINVAL, "score: forced_ids cannot be combined with logits processors");
   std::vector<long long> f(static_cast<size_t>(rows) * L);
   if (host) memcpy(f.data(), sc->forced_ids, f.size() * 8);
   else CU_OK(h, cudaMemcpy(f.data(), sc->forced_ids, f.size() * 8, cudaMemcpyDeviceToHost));
@@ -1601,7 +1593,6 @@ static int parse_score(b200t5_ctx* h, const b200t5_score_io* sc, long long rows,
 // and queue the labels on `s`. A new allocation drops the step graph, which bakes the addresses.
 static int setup_score(b200t5_ctx* h, const ScoreHost& sh, cudaStream_t s) {
   Plan& p = *h->plan;
-  p.score_on = sh.on ? (sh.forced.empty() ? 1 : 2) : 0;
   if (!sh.on) return B200T5_OK;
   Plan::Results& r = p.res();
   const size_t n = r.cap * p.Tmax;
@@ -1616,9 +1607,9 @@ static int setup_score(b200t5_ctx* h, const ScoreHost& sh, cudaStream_t s) {
     CU_OK(h, r.lp.alloc(n * 4));
     CU_OK(h, r.lg.alloc(n * 4));
     CU_OK(h, r.forced.alloc(n * 8));
-    p.g_score = -1;
+    p.invalidate_graph();
   }
-  if (p.score_on == 2) CU_OK(h, cudaMemcpyAsync(r.forced.p, sh.forced.data(), sh.forced.size() * 8, cudaMemcpyHostToDevice, s));
+  if (!sh.forced.empty()) CU_OK(h, cudaMemcpyAsync(r.forced.p, sh.forced.data(), sh.forced.size() * 8, cudaMemcpyHostToDevice, s));
   return B200T5_OK;
 }
 
@@ -1653,6 +1644,18 @@ struct CallArgs {
   int T = 0, min_new = 0;
   ProcHost ph;
   ScoreHost sh;
+  // The step mode of this call. A beam call's min_new_tokens lives in its BeamParams, not in the graph.
+  StepMode mode(bool pool, int beam = 0) const {
+    StepMode m;
+    m.eos = eos;
+    m.pad = pad;
+    m.min_new = beam ? 0 : min_new;
+    m.pool = pool;
+    m.proc = ph.on;
+    m.score = sh.on ? (sh.forced.empty() ? 1 : 2) : 0;
+    m.beam = beam;
+    return m;
+  }
 };
 
 // Checks a call of B rows (the slot pool: B slots) for `rows` prompts and resolves what it asks for. `host`: the pointers
@@ -1683,45 +1686,32 @@ static int copy_results(b200t5_ctx* h, size_t n, void* ids, void* len, void* lp,
   const size_t T = static_cast<size_t>(p.Tmax);
   CU_OK(h, cudaMemcpyAsync(ids, r.ids.p, n * (T + 1) * 8, kind, s));
   CU_OK(h, cudaMemcpyAsync(len, r.len.p, n * 4, kind, s));
-  if (p.score_on) {
+  if (p.mode.score) {
     CU_OK(h, cudaMemcpyAsync(lp, r.lp.p, n * T * 4, kind, s));
     if (lg) CU_OK(h, cudaMemcpyAsync(lg, r.lg.p, n * T * 4, kind, s));
   }
   return B200T5_OK;
 }
 
-// A static batch of B rows; its results stay in the plan's buffers (copy_results).
-static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* mask, int B, int S, const b200t5_gen_params* gp,
-                         const CallArgs& a, cudaStream_t s) {
-  const Cfg& c = h->c;
-  const int T = a.T;
-  const int poll = gp->poll_interval > 0 ? gp->poll_interval : 8;
-  TRY(ensure_plan(h, B, S, T));
+// The start of a static batch's decoding, after its encoder pass: the decode kernels attend to live copies of extent /
+// key_ok, and every row starts from the start token.
+static int begin_static_decode(b200t5_ctx* h, const CallArgs& a, cudaStream_t s) {
   Plan& p = *h->plan;
-  p.stream_mode = false;
-  p.beam_k = 0;
-  TRY(setup_proc(h, a.ph, s));
-  TRY(setup_score(h, a.sh, s));
-  h->launches = 0;
-  CU_OK(h, cudaEventRecord(h->ev[0], s));
-  TRY(run_encoder(h, ids, mask, s));
-  TRY(run_cross_kv(h, s));
-  // (host-side capture, only when something baked into the graph changed; the GPU is busy with the encoder meanwhile)
-  TRY(ensure_graph(h, a.eos, a.pad, a.min_new, static_cast<double>(p.rows_valid) / (static_cast<double>(B) * S)));
+  const int B = p.B;
   CU_OK(h, cudaMemcpyAsync(p.live_extent.p, p.extent.p, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToDevice, s));
-  CU_OK(h, cudaMemcpyAsync(p.live_key_ok.p, p.key_ok.p, static_cast<size_t>(B) * S, cudaMemcpyDeviceToDevice, s));
+  CU_OK(h, cudaMemcpyAsync(p.live_key_ok.p, p.key_ok.p, static_cast<size_t>(B) * p.S, cudaMemcpyDeviceToDevice, s));
   decode_init_kernel<<<B, 128, 0, s>>>(p.state.as<DecodeState>(), p.unfinished.as<int>(), p.batch.ids.as<long long>(),
-                                       p.batch.len.as<int>(), T + 1, B, a.start, a.pad, h->shared.as<act_t>(), p.dx.as<res_t>(), c.d);
+                                       p.batch.len.as<int>(), a.T + 1, B, a.start, a.pad, h->shared.as<act_t>(), p.dx.as<res_t>(),
+                                       h->c.d);
   h->launches++;
-  if (p.proc_on) {
-    proc_reset_kernel<<<B, 128, 0, s>>>(p.proc.dev(), nullptr, ids, p.batch.ids.as<long long>(), T + 1, nullptr, 1);
-    h->launches++;
-  }
-  if (p.score_on) {
-    score_reset_kernel<<<B, 128, 0, s>>>(p.batch.lp.as<float>(), p.batch.lg.as<float>(), static_cast<size_t>(B) * T, p.ftok.as<int>(),
-                                         B, nullptr, nullptr, p.score_on == 2 ? p.batch.forced.as<long long>() : nullptr, T);
-    h->launches++;
-  }
+  return B200T5_OK;
+}
+
+// The T decode steps of a static batch, from the end of its encoder pass (ev[1]) to ev[2]. `early_exit`: stop at a
+// poll once every row has finished.
+static int run_static_steps(b200t5_ctx* h, const b200t5_gen_params* gp, int T, bool early_exit, cudaStream_t s) {
+  Plan& p = *h->plan;
+  const int poll = gp->poll_interval > 0 ? gp->poll_interval : 8;
   CU_OK(h, cudaGetLastError());
   CU_OK(h, cudaEventRecord(h->ev[1], s));
   int steps = 0;
@@ -1737,17 +1727,45 @@ static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* m
       h->launches += p.graph_nodes;
       ++steps;
     }
-    if ((t + 1) % poll == 0 && t + 1 < T && a.min_new < T) {
-      // every row emitted EOS -> the remaining steps would only append pad tokens
+    if ((t + 1) % poll == 0 && t + 1 < T && early_exit) {
+      // every row finished (greedy: emitted EOS; beam: its prompt retired) -> the remaining steps would change nothing
       CU_OK(h, cudaMemcpyAsync(p.h_state, p.state.p, sizeof(DecodeState), cudaMemcpyDeviceToHost, s));
       CU_OK(h, cudaStreamSynchronize(s));
-      if (p.h_state->finished_rows >= B) break;
+      if (p.h_state->finished_rows >= p.B) break;
     }
   }
   CU_OK(h, cudaEventRecord(h->ev[2], s));
   h->last_steps = steps;
   h->ev_valid = true;
   return B200T5_OK;
+}
+
+// A static batch of B rows; its results stay in the plan's buffers (copy_results).
+static int generate_impl(b200t5_ctx* h, const long long* ids, const long long* mask, int B, int S, const b200t5_gen_params* gp,
+                         const CallArgs& a, cudaStream_t s) {
+  const int T = a.T;
+  TRY(ensure_plan(h, B, S, T));
+  Plan& p = *h->plan;
+  p.mode = a.mode(false);
+  TRY(setup_proc(h, a.ph, s));
+  TRY(setup_score(h, a.sh, s));
+  h->launches = 0;
+  CU_OK(h, cudaEventRecord(h->ev[0], s));
+  TRY(run_encoder(h, ids, mask, s));
+  TRY(run_cross_kv(h, s));
+  // (host-side capture, only when something baked into the graph changed; the GPU is busy with the encoder meanwhile)
+  TRY(ensure_graph(h, static_cast<double>(p.rows_valid) / (static_cast<double>(B) * S)));
+  TRY(begin_static_decode(h, a, s));
+  if (p.mode.proc) {
+    proc_reset_kernel<<<B, 128, 0, s>>>(p.proc.dev(), nullptr, ids, p.batch.ids.as<long long>(), T + 1, nullptr, 1);
+    h->launches++;
+  }
+  if (p.mode.score) {
+    score_reset_kernel<<<B, 128, 0, s>>>(p.batch.lp.as<float>(), p.batch.lg.as<float>(), static_cast<size_t>(B) * T, p.ftok.as<int>(),
+                                         B, nullptr, nullptr, p.mode.score == 2 ? p.batch.forced.as<long long>() : nullptr, T);
+    h->launches++;
+  }
+  return run_static_steps(h, gp, T, a.min_new < T, s);
 }
 
 extern "C" int b200t5_generate_scored(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
@@ -1810,13 +1828,16 @@ extern "C" int b200t5_generate_host_scored(b200t5_handle h, const int64_t* input
 }
 
 // ================================================================== beam search
-static int parse_beam(b200t5_ctx* h, const b200t5_beam_params* bp) {
+// A beam call's parameters, for B prompts.
+static int parse_beam(b200t5_ctx* h, const b200t5_beam_params* bp, int B) {
   if (!bp) return fail(h, B200T5_EINVAL, "null beam params");
   if (bp->num_beams < 2 || bp->num_beams > kBeamMax) return fail(h, B200T5_EINVAL, "num_beams=%d outside [2, %d]", bp->num_beams, kBeamMax);
   if (bp->num_return_sequences < 1 || bp->num_return_sequences > bp->num_beams)
     return fail(h, B200T5_EINVAL, "num_return_sequences=%d outside [1, num_beams=%d]", bp->num_return_sequences, bp->num_beams);
   if (bp->early_stopping < 0 || bp->early_stopping > 2) return fail(h, B200T5_EINVAL, "early_stopping=%d outside {0, 1, 2}", bp->early_stopping);
   if (!std::isfinite(bp->length_penalty)) return fail(h, B200T5_EINVAL, "length_penalty is not finite");
+  const int rows = B * bp->num_beams;
+  if (rows > 65535) return fail(h, B200T5_EINVAL, "B * num_beams = %d rows is too many", rows);
   return B200T5_OK;
 }
 
@@ -1825,6 +1846,11 @@ static int ensure_beam_bufs(b200t5_ctx* h, Plan& p) {
   BeamBufs& b = p.beam;
   if (b.prm.p) return B200T5_OK;
   const size_t rows = static_cast<size_t>(p.B), T = static_cast<size_t>(p.Tmax), prompts = rows / p.group;
+  CU_OK(h, b.seq.alloc(rows * (T + 1) * 8));
+  CU_OK(h, b.len.alloc(rows * 4));
+  CU_OK(h, b.score.alloc(rows * 4));
+  CU_OK(h, b.bidx.alloc(rows * T * 8));
+  CU_OK(h, b.lp.alloc(rows * T * 4));
   CU_OK(h, b.logits.alloc(rows * h->c.V * 4));
   CU_OK(h, b.cand_lp.alloc(rows * kBeamCand * 4));
   CU_OK(h, b.cand_tok.alloc(rows * kBeamCand * 4));
@@ -1838,7 +1864,7 @@ static int ensure_beam_bufs(b200t5_ctx* h, Plan& p) {
   CU_OK(h, b.len_scale.alloc(T * 4));
   CU_OK(h, b.moved.alloc(8));
   CU_OK(h, b.prm.alloc(sizeof(BeamParams)));
-  p.g_beam = -1;
+  p.invalidate_graph();
   return B200T5_OK;
 }
 
@@ -1850,18 +1876,14 @@ static std::vector<float> beam_len_scale(double length_penalty, int T) {
 }
 
 // A static batch of B prompts as B * k decode rows; the results stay in the plan's beam state (beam_output_kernel).
-static int generate_beam_impl(b200t5_ctx* h, const long long* ids, const long long* mask, int Bp, int S, const b200t5_gen_params* gp,
-                              const b200t5_beam_params* bp, const CallArgs& a, cudaStream_t s) {
+// `ids` / `mask` are device buffers, or host buffers with kind = cudaMemcpyHostToDevice.
+static int generate_beam_impl(b200t5_ctx* h, const long long* ids, const long long* mask, cudaMemcpyKind kind, int Bp, int S,
+                              const b200t5_gen_params* gp, const b200t5_beam_params* bp, const CallArgs& a, cudaStream_t s) {
   const Cfg& c = h->c;
   const int T = a.T, k = bp->num_beams, rows = Bp * k;
-  const int poll = gp->poll_interval > 0 ? gp->poll_interval : 8;
-  if (rows > 65535) return fail(h, B200T5_EINVAL, "B * num_beams = %d rows is too many", rows);
   TRY(ensure_plan(h, rows, S, T, k));
   Plan& p = *h->plan;
-  p.stream_mode = false;
-  p.proc_on = false;
-  p.score_on = 0;
-  p.beam_k = k;
+  p.mode = a.mode(false, k);
   TRY(ensure_beam_bufs(h, p));
   const BeamDev bd = p.beam.dev(rows);
   const BeamParams prm{k, T, a.min_new, static_cast<int>(a.eos), bp->early_stopping, bp->early_stopping == 2 && bp->length_penalty > 0.0};
@@ -1876,8 +1898,8 @@ static int generate_beam_impl(b200t5_ctx* h, const long long* ids, const long lo
   const bool packed = S <= kEncPackMaxS;
   const size_t rb = static_cast<size_t>(S) * 8;
   for (int j = 0; j < (packed ? 1 : k); ++j) {
-    CU_OK(h, cudaMemcpy2DAsync(p.ids_dev.as<long long>() + static_cast<size_t>(j) * S, k * rb, ids, rb, rb, Bp, cudaMemcpyDeviceToDevice, s));
-    if (mask) CU_OK(h, cudaMemcpy2DAsync(p.mask_dev.as<long long>() + static_cast<size_t>(j) * S, k * rb, mask, rb, rb, Bp, cudaMemcpyDeviceToDevice, s));
+    CU_OK(h, cudaMemcpy2DAsync(p.ids_dev.as<long long>() + static_cast<size_t>(j) * S, k * rb, ids, rb, rb, Bp, kind, s));
+    if (mask) CU_OK(h, cudaMemcpy2DAsync(p.mask_dev.as<long long>() + static_cast<size_t>(j) * S, k * rb, mask, rb, rb, Bp, kind, s));
   }
   const int* row_on = nullptr;
   if (packed) {
@@ -1893,39 +1915,13 @@ static int generate_beam_impl(b200t5_ctx* h, const long long* ids, const long lo
     h->launches++;
   }
   const double valid = packed ? static_cast<double>(p.rows_valid) * k : static_cast<double>(p.rows_valid);
-  TRY(ensure_graph(h, a.eos, a.pad, 0, valid / (static_cast<double>(rows) * S)));
-  CU_OK(h, cudaMemcpyAsync(p.live_extent.p, p.extent.p, static_cast<size_t>(rows) * 4, cudaMemcpyDeviceToDevice, s));
-  CU_OK(h, cudaMemcpyAsync(p.live_key_ok.p, p.key_ok.p, static_cast<size_t>(rows) * S, cudaMemcpyDeviceToDevice, s));
-  decode_init_kernel<<<rows, 128, 0, s>>>(p.state.as<DecodeState>(), p.unfinished.as<int>(), p.batch.ids.as<long long>(),
-                                          p.batch.len.as<int>(), T + 1, rows, a.start, a.pad, h->shared.as<act_t>(), p.dx.as<res_t>(), c.d);
+  TRY(ensure_graph(h, valid / (static_cast<double>(rows) * S)));
+  TRY(begin_static_decode(h, a, s));
   beam_init_kernel<<<(std::max(rows, Bp * kBeamMax) + 255) / 256, 256, 0, s>>>(bd, Bp, k);
-  h->launches += 2;
+  h->launches++;
   CU_OK(h, cudaMemsetAsync(p.beam.moved.p, 0, 8, s));
-  CU_OK(h, cudaGetLastError());
-  CU_OK(h, cudaEventRecord(h->ev[1], s));
-  int steps = 0;
-  for (int t = 0; t < T; ++t) {
-    if (t % kStepsPerGraph == 0 && t + kStepsPerGraph <= T && poll % kStepsPerGraph == 0) {
-      CU_OK(h, cudaGraphLaunch(p.gexec8, s));
-      h->launches += static_cast<int64_t>(p.graph_nodes) * kStepsPerGraph;
-      steps += kStepsPerGraph;
-      t += kStepsPerGraph - 1;
-    } else {
-      CU_OK(h, cudaGraphLaunch(p.gexec, s));
-      h->launches += p.graph_nodes;
-      ++steps;
-    }
-    if ((t + 1) % poll == 0 && t + 1 < T) {
-      // every prompt retired: its finished set can no longer change
-      CU_OK(h, cudaMemcpyAsync(p.h_state, p.state.p, sizeof(DecodeState), cudaMemcpyDeviceToHost, s));
-      CU_OK(h, cudaStreamSynchronize(s));
-      if (p.h_state->finished_rows >= rows) break;
-    }
-  }
-  CU_OK(h, cudaEventRecord(h->ev[2], s));
-  h->last_steps = steps;
-  h->ev_valid = true;
-  return B200T5_OK;
+  // a beam row finishes when its prompt retires: the prompt's finished set can no longer change
+  return run_static_steps(h, gp, T, true, s);
 }
 
 static int beam_output(b200t5_ctx* h, int Bp, const b200t5_beam_params* bp, long long start, long long pad, int64_t* seq, int32_t* len,
@@ -1945,10 +1941,10 @@ extern "C" int b200t5_generate_beam(b200t5_handle h, const int64_t* input_ids, c
   CallArgs a;
   if (!io) return fail(h, B200T5_EINVAL, "null beam io");
   TRY(set_up_call(h, B, S, B, params, input_ids, io->sequences, io->lengths, nullptr, nullptr, false, &a));
-  TRY(parse_beam(h, beam));
+  TRY(parse_beam(h, beam, B));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  TRY(generate_beam_impl(h, reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(attention_mask), B, S,
-                         params, beam, a, s));
+  TRY(generate_beam_impl(h, reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(attention_mask),
+                         cudaMemcpyDeviceToDevice, B, S, params, beam, a, s));
   return beam_output(h, B, beam, a.start, a.pad, io->sequences, io->lengths, io->sequences_scores, io->beam_indices, io->token_logprobs, s);
 }
 
@@ -1957,30 +1953,24 @@ extern "C" int b200t5_generate_host_beam(b200t5_handle h, const int64_t* input_i
   CallArgs a;
   if (!io) return fail(h, B200T5_EINVAL, "null beam io");
   TRY(set_up_call(h, B, S, B, params, input_ids, io->sequences, io->lengths, nullptr, nullptr, true, &a));
-  TRY(parse_beam(h, beam));
+  TRY(parse_beam(h, beam, B));
   cudaStream_t s = h->exec_stream;
+  TRY(ensure_plan(h, B * beam->num_beams, S, a.T, beam->num_beams));
+  Plan& p = *h->plan;
+  // the prompts through the pinned staging; the results through the plan's beam buffers
   const size_t nb = static_cast<size_t>(B) * S * 8;
+  memcpy(p.h_ids, input_ids, nb);
+  if (attention_mask) memcpy(p.h_mask, attention_mask, nb);
+  TRY(generate_beam_impl(h, p.h_ids, attention_mask ? p.h_mask : nullptr, cudaMemcpyHostToDevice, B, S, params, beam, a, s));
+  const BeamBufs& o = p.beam;
+  TRY(beam_output(h, B, beam, a.start, a.pad, o.seq.as<int64_t>(), o.len.as<int32_t>(), o.score.as<float>(), o.bidx.as<int64_t>(),
+                  o.lp.as<float>(), s));
   const size_t n = static_cast<size_t>(B) * beam->num_return_sequences, T = static_cast<size_t>(a.T);
-  DevBuf in_ids, in_mask, o_seq, o_len, o_sc, o_bi, o_lp;
-  CU_OK(h, in_ids.alloc(nb));
-  CU_OK(h, cudaMemcpyAsync(in_ids.p, input_ids, nb, cudaMemcpyHostToDevice, s));
-  if (attention_mask) {
-    CU_OK(h, in_mask.alloc(nb));
-    CU_OK(h, cudaMemcpyAsync(in_mask.p, attention_mask, nb, cudaMemcpyHostToDevice, s));
-  }
-  CU_OK(h, o_seq.alloc(n * (T + 1) * 8));
-  CU_OK(h, o_len.alloc(n * 4));
-  CU_OK(h, o_sc.alloc(n * 4));
-  CU_OK(h, o_bi.alloc(n * T * 8));
-  CU_OK(h, o_lp.alloc(n * T * 4));
-  TRY(generate_beam_impl(h, in_ids.as<long long>(), attention_mask ? in_mask.as<long long>() : nullptr, B, S, params, beam, a, s));
-  TRY(beam_output(h, B, beam, a.start, a.pad, o_seq.as<int64_t>(), o_len.as<int32_t>(), o_sc.as<float>(), o_bi.as<int64_t>(),
-                  o_lp.as<float>(), s));
-  CU_OK(h, cudaMemcpyAsync(io->sequences, o_seq.p, o_seq.bytes, cudaMemcpyDeviceToHost, s));
-  CU_OK(h, cudaMemcpyAsync(io->lengths, o_len.p, o_len.bytes, cudaMemcpyDeviceToHost, s));
-  if (io->sequences_scores) CU_OK(h, cudaMemcpyAsync(io->sequences_scores, o_sc.p, o_sc.bytes, cudaMemcpyDeviceToHost, s));
-  if (io->beam_indices) CU_OK(h, cudaMemcpyAsync(io->beam_indices, o_bi.p, o_bi.bytes, cudaMemcpyDeviceToHost, s));
-  if (io->token_logprobs) CU_OK(h, cudaMemcpyAsync(io->token_logprobs, o_lp.p, o_lp.bytes, cudaMemcpyDeviceToHost, s));
+  CU_OK(h, cudaMemcpyAsync(io->sequences, o.seq.p, n * (T + 1) * 8, cudaMemcpyDeviceToHost, s));
+  CU_OK(h, cudaMemcpyAsync(io->lengths, o.len.p, n * 4, cudaMemcpyDeviceToHost, s));
+  if (io->sequences_scores) CU_OK(h, cudaMemcpyAsync(io->sequences_scores, o.score.p, n * 4, cudaMemcpyDeviceToHost, s));
+  if (io->beam_indices) CU_OK(h, cudaMemcpyAsync(io->beam_indices, o.bidx.p, n * T * 8, cudaMemcpyDeviceToHost, s));
+  if (io->token_logprobs) CU_OK(h, cudaMemcpyAsync(io->token_logprobs, o.lp.p, n * T * 4, cudaMemcpyDeviceToHost, s));
   CU_OK(h, cudaStreamSynchronize(s));
   return B200T5_OK;
 }
@@ -2031,6 +2021,7 @@ extern "C" int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* inp
   const int poll = gp->poll_interval > 0 ? (gp->poll_interval > 64 ? 64 : gp->poll_interval) : kStepsPerGraph;
   TRY(ensure_plan(h, B, S, T));
   Plan& p = *h->plan;
+  p.mode = a.mode(true);
   cudaStream_t s = h->exec_stream;
   Plan::Results& r = p.pool;
   if (r.cap < static_cast<size_t>(N)) {
@@ -2041,10 +2032,8 @@ extern "C" int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* inp
     CU_OK(h, r.ids.alloc(cap * (T + 1) * 8));
     CU_OK(h, r.len.alloc(cap * 4));
     r.cap = cap;
-    p.g_stream = -1;
+    p.invalidate_graph();
   }
-  p.stream_mode = true;
-  p.beam_k = 0;
   TRY(setup_proc(h, a.ph, s));
   TRY(setup_score(h, a.sh, s));
   double fill = 1.0;
@@ -2054,7 +2043,7 @@ extern "C" int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* inp
     for (long long i = 0; i < rows * S; ++i) ones += attention_mask[i] != 0;
     fill = static_cast<double>(ones) / static_cast<double>(rows * S);
   }
-  TRY(ensure_graph(h, a.eos, a.pad, a.min_new, fill));
+  TRY(ensure_graph(h, fill));
   h->launches = 0;
   CU_OK(h, cudaEventRecord(h->ev[0], s));
   {
@@ -2064,7 +2053,7 @@ extern "C" int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* inp
                                                                   r.len.as<int>(), T + 1, static_cast<int>(N), B, a.start, a.pad,
                                                                   h->shared.as<act_t>(), p.dx.as<res_t>(), c.d);
     h->launches++;
-    if (p.score_on) {  // every result position 0, no slot forced until it is admitted
+    if (p.mode.score) {  // every result position 0, no slot forced until it is admitted
       score_reset_kernel<<<1024, 128, 0, s>>>(r.lp.as<float>(), r.lg.as<float>(), static_cast<size_t>(N) * T,
                                               p.ftok.as<int>(), B, nullptr, nullptr, nullptr, T);
       h->launches++;
@@ -2094,12 +2083,12 @@ extern "C" int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* inp
                                          p.key_ok.as<unsigned char>(), p.live_key_ok.as<unsigned char>(), S, a.start,
                                          h->shared.as<act_t>(), p.dx.as<res_t>(), c.d);
     h->launches++;
-    if (p.proc_on) {  // the admitted slots' processor state, from their prompts (still in ids_dev) and start token
+    if (p.mode.proc) {  // the admitted slots' processor state, from their prompts (still in ids_dev) and start token
       proc_reset_kernel<<<k, 128, 0, s>>>(p.proc.dev(), p.admit.as<int>() + B, p.ids_dev.as<long long>(),
                                           r.ids.as<long long>(), T + 1, p.out_row.as<int>(), 1);
       h->launches++;
     }
-    if (p.score_on == 2) {  // the admitted slots' first labels
+    if (p.mode.score == 2) {  // the admitted slots' first labels
       score_reset_kernel<<<(k + 127) / 128, 128, 0, s>>>(nullptr, nullptr, 0, p.ftok.as<int>(), k, p.admit.as<int>() + B,
                                                          p.admit.as<int>() + 2 * B, r.forced.as<long long>(), T);
       h->launches++;
@@ -2211,7 +2200,7 @@ extern "C" int b200t5_get_stats(b200t5_handle h, b200t5_stats* out) {
   fill_stats_model(h, h->last_steps);
   out->decode_algo_bytes = h->last_decode_bytes;
   out->encoder_flops = h->last_enc_flops;
-  out->xattn_kernel = h->plan->xattn_stream ? 1 : 0;
+  out->xattn_kernel = h->plan->mode.xattn_stream ? 1 : 0;
   out->row_chains = h->plan->n_chains;
   return B200T5_OK;
 }
@@ -2369,9 +2358,8 @@ extern "C" int b200t5_decode_logits(b200t5_handle h, const int64_t* input_ids, c
   const Cfg& c = h->c;
   TRY(run_encoder(h, reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(attention_mask), s));
   TRY(run_cross_kv(h, s));
-  p.stream_mode = false;
-  p.beam_k = 0;
-  p.xattn_stream = pick_xattn(h, static_cast<double>(p.rows_valid) / (static_cast<double>(B) * S)) != 0;
+  p.mode = StepMode();  // the step's head stores logits: only the cross-attention kernel matters
+  p.mode.xattn_stream = pick_xattn(h, static_cast<double>(p.rows_valid) / (static_cast<double>(B) * S));
   CU_OK(h, cudaMemcpyAsync(p.live_extent.p, p.extent.p, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToDevice, s));
   CU_OK(h, cudaMemcpyAsync(p.live_key_ok.p, p.key_ok.p, static_cast<size_t>(B) * S, cudaMemcpyDeviceToDevice, s));
   set_state_kernel<<<1, 1, 0, s>>>(p.state.as<DecodeState>(), 0);
@@ -2380,7 +2368,7 @@ extern "C" int b200t5_decode_logits(b200t5_handle h, const int64_t* input_ids, c
   for (int t = 0; t < T; ++t) {
     CU_OK(h, cudaMemcpy2DAsync(col.p, 8, reinterpret_cast<const long long*>(decoder_input_ids) + t, static_cast<size_t>(T) * 8, 8, B, cudaMemcpyDeviceToDevice, s));
     force_token_kernel<<<B, 128, 0, s>>>(col.as<long long>(), h->shared.as<act_t>(), p.dx.as<res_t>(), c.d);
-    TRY(run_decode_step(h, s, false, logits + static_cast<size_t>(t) * c.V, T * c.V, c.eos, c.pad, 0));
+    TRY(run_decode_step(h, s, false, logits + static_cast<size_t>(t) * c.V, T * c.V));
   }
   CU_OK(h, cudaStreamSynchronize(s));
   return B200T5_OK;

@@ -407,8 +407,9 @@ class B200T5ForConditionalGeneration:
             self._h = None
 
     # ------------------------------------------------------------------ generation
-    def _gen_params(self, max_new_tokens, max_length, min_new_tokens, min_length, eos_token_id, pad_token_id,
-                    decoder_start_token_id, poll_interval) -> _lib.GenParams:
+    def _gen_params(self, max_new_tokens=None, max_length=None, min_new_tokens=None, min_length=None, eos_token_id=None,
+                    pad_token_id=None, decoder_start_token_id=None, poll_interval=8, **_) -> _lib.GenParams:
+        # takes a call's whole kwargs (generate_host, generate_stream) and ignores the ones that are not its own.
         # GenerationMixin._prepare_generated_length (generation/utils.py:1619-1639): the decoder
         # prompt is the single start token, so max_length = max_new_tokens + 1.
         if max_new_tokens is None:
@@ -470,38 +471,34 @@ class B200T5ForConditionalGeneration:
         if host.dim() != 2:
             raise ValueError(f"input_ids must be [batch, seq], got {tuple(host.shape)}")
         if bp is not None:
-            seq, scores, bidx, logp = self._generate_beam(host, attention_mask, gp, bp)
+            ids, mask = self._device_inputs(host, attention_mask, gp, None)
+            seq, _, scores, bidx, logp = self._generate_beam(ids, mask, gp, bp, self._generate_beam_static)
             if not as_dict:
                 return seq
             return BeamGenerateOutput(seq, scores, bidx, TokenScores(logp, logp, beam=True) if want_scores else None)
-        if as_dict:
-            if not want_scores:  # the unchanged greedy call, wrapped
-                return GenerateOutput(self.generate(input_ids=input_ids, attention_mask=attention_mask, max_new_tokens=gp.max_new_tokens,
-                                                    min_new_tokens=gp.min_new_tokens, eos_token_id=eos_token_id, pad_token_id=pad_token_id,
-                                                    decoder_start_token_id=decoder_start_token_id, poll_interval=poll_interval,
-                                                    **{k: unused[k] for k in LOGITS_PROCESSOR_KWARGS if k in unused}))
+        if as_dict and want_scores:
             seq, _, logp, logit = self._run_scored(host, attention_mask, gp, lp, None)
             return GenerateOutput(seq, TokenScores(logp, logit))
+        seq = self._generate_greedy(host, attention_mask, gp, lp)
+        return GenerateOutput(seq) if as_dict else seq
+
+    def _generate_greedy(self, host: torch.Tensor, attention_mask, gp, lp) -> torch.Tensor:
+        """generate's routing: the sequences [B, 1+T'] on the device, from one static batch, the slot pool or static
+        chunks."""
         if self.takes_host_batches(host.shape[0], host.shape[1]) and host.device.type == "cpu":
             # more rows than one pool of decode slots, still in host memory: the slot pool admits prompts from host
             # buffers as slots free up, so nothing is copied to the device (and back) up front
             return self._generate_pool_from_host(host, attention_mask, gp, lp)
         ids, mask = self._device_inputs(host, attention_mask, gp, lp)
-        B, S = ids.shape
-        if B > self.pool_size:
-            if self.takes_host_batches(B, S):
-                # more rows than one pool of decode slots: continuous batching, same tokens row for row. The pool
-                # admits prompts from host memory as slots free up (its entry point takes host buffers).
-                out_np, _ = self.generate_stream(ids.cpu().numpy(), None if mask is None else mask.cpu().numpy(), _gen_params=gp,
-                                                 _logits=lp)
-                return torch.from_numpy(out_np).to(self._device)
-            # prompts the slot pool cannot take (it needs the packed encoder, S <= 512): static batches
-            outs = [self._generate_static(ids[lo:lo + self.pool_size], None if mask is None else mask[lo:lo + self.pool_size], gp, lp)
-                    for lo in range(0, B, self.pool_size)]
-            width = max(o.shape[1] for o in outs)
-            pad = gp.pad_token_id if gp.pad_token_id >= 0 else self.generation_config.pad_token_id
-            return torch.cat([torch.nn.functional.pad(o, (0, width - o.shape[1]), value=pad) for o in outs], dim=0)
-        return self._generate_static(ids, mask, gp, lp)
+        if self.takes_host_batches(ids.shape[0], ids.shape[1]):
+            # more rows than one pool of decode slots: continuous batching, same tokens row for row. The pool
+            # admits prompts from host memory as slots free up (its entry point takes host buffers).
+            out_np, _ = self.generate_stream(ids.cpu().numpy(), None if mask is None else mask.cpu().numpy(), _gen_params=gp,
+                                             _logits=lp)
+            return torch.from_numpy(out_np).to(self._device)
+        # one static batch, or chunks of pool_size rows for prompts the slot pool cannot take (it needs the packed
+        # encoder, S <= 512)
+        return self._generate_chunks(ids, mask, gp, lp)[0]
 
     def compute_transition_scores(self, sequences, scores, beam_indices=None, normalize_logits: bool = False):
         """transformers' GenerationMixin.compute_transition_scores for the `.scores` of this model's generate: the
@@ -535,34 +532,38 @@ class B200T5ForConditionalGeneration:
         lengths [B], token_logprobs [B, T'], token_logits [B, T']) on the device. With `labels` the call is
         teacher-forced and T' = labels.shape[1]."""
         ids, mask = self._device_inputs(host, attention_mask, gp, lp)
-        B, S = ids.shape
-        T = gp.max_new_tokens
-        if B > self.pool_size and self.takes_host_batches(B, S):
-            out, lens, logp, logit = self.generate_stream(ids.cpu().numpy(), None if mask is None else mask.cpu().numpy(),
-                                                          _gen_params=gp, _logits=lp, _labels=labels, output_scores=True)
-            out, lens, logp, logit = (torch.from_numpy(np.ascontiguousarray(a)).to(self._device) for a in (out, lens, logp, logit))
-        else:
-            parts = [self._generate_static(ids[lo:lo + self.pool_size], None if mask is None else mask[lo:lo + self.pool_size], gp, lp,
-                                           score=True, labels=None if labels is None else labels[lo:lo + self.pool_size])
-                     for lo in range(0, B, self.pool_size)]
-            out, lens, logp, logit = (torch.cat([p[i] for p in parts], dim=0) for i in range(4))
-        steps = T if labels is not None else int(lens.max().item())
-        return out[:, : steps + 1], lens, logp[:, :steps], logit[:, :steps]
+        if self.takes_host_batches(ids.shape[0], ids.shape[1]):
+            res = self.generate_stream(ids.cpu().numpy(), None if mask is None else mask.cpu().numpy(), _gen_params=gp, _logits=lp,
+                                       _labels=labels, output_scores=True)
+            return tuple(torch.from_numpy(np.ascontiguousarray(a)).to(self._device) for a in res)
+        return self._generate_chunks(ids, mask, gp, lp, score=True, labels=labels)
 
-    def _generate_beam(self, host: torch.Tensor, attention_mask, gp, bp):
-        """Beam search (b200t5_generate_beam) in static chunks of pool_size // num_beams prompts: (sequences [B*n, 1+T'],
-        sequences_scores [B*n], beam_indices [B*n, T'], token_logprobs [B*n, T']) on the device, T' the longest returned
-        hypothesis. beam_indices count prompts across the whole call, as transformers' do."""
-        ids, mask = self._device_inputs(host, attention_mask, gp, None)
-        B = ids.shape[0]
-        k, n = bp.num_beams, bp.num_return_sequences
+    def _generate_chunks(self, ids: torch.Tensor, mask: Optional[torch.Tensor], gp, lp, score: bool = False, labels=None):
+        """Static batches of at most pool_size rows: (sequences [B, 1+T'], lengths [B]) and, with score=True,
+        (token_logprobs [B, T'], token_logits [B, T']), on the device. T' = the steps of the longest row, or
+        labels.shape[1] for a teacher-forced call."""
+        parts = [self._generate_static(ids[lo:lo + self.pool_size], None if mask is None else mask[lo:lo + self.pool_size], gp, lp,
+                                       score, None if labels is None else labels[lo:lo + self.pool_size])
+                 for lo in range(0, ids.shape[0], self.pool_size)]
+        out, lens, *scores = parts[0] if len(parts) == 1 else [torch.cat(c, dim=0) for c in zip(*parts)]
+        steps = gp.max_new_tokens if labels is not None else int(lens.max().item())  # HF returns exactly the steps it ran
+        return (out[:, : steps + 1], lens, *(a[:, :steps] for a in scores))
+
+    def _generate_beam(self, ids, mask, gp, bp, run_chunk):
+        """Beam search in static chunks of pool_size // num_beams prompts, each run by run_chunk(ids, mask, gp, bp), which
+        returns torch tensors or numpy arrays: (sequences [n, 1+T], lengths, sequences_scores, beam_indices [n, T],
+        token_logprobs [n, T]). Returns the same for the whole call, T' = the longest returned hypothesis: (sequences
+        [B*n, 1+T'], lengths [B*n], sequences_scores [B*n], beam_indices [B*n, T'], token_logprobs [B*n, T']).
+        beam_indices count prompts across the whole call, as transformers' do."""
+        k = bp.num_beams
         chunk = max(1, self.pool_size // k)
-        parts = [self._generate_beam_static(ids[lo:lo + chunk], None if mask is None else mask[lo:lo + chunk], gp, bp)
-                 for lo in range(0, B, chunk)]
-        L = max(int(p[1].max().item()) for p in parts)
-        seq = torch.cat([p[0][:, : L + 1] for p in parts], dim=0)  # (each chunk is padded to max_new_tokens)
-        bidx = torch.cat([torch.where(p[3][:, :L] >= 0, p[3][:, :L] + i * chunk * k, p[3][:, :L]) for i, p in enumerate(parts)], dim=0)
-        return seq, torch.cat([p[2] for p in parts]), bidx, torch.cat([p[4][:, :L] for p in parts], dim=0)
+        parts = [run_chunk(ids[lo:lo + chunk], None if mask is None else mask[lo:lo + chunk], gp, bp)
+                 for lo in range(0, ids.shape[0], chunk)]
+        cat = torch.cat if isinstance(parts[0][0], torch.Tensor) else np.concatenate
+        L = max(int(p[1].max()) for p in parts)
+        bidx = [p[3][:, :L] for p in parts]
+        return (cat([p[0][:, : L + 1] for p in parts]), cat([p[1] for p in parts]), cat([p[2] for p in parts]),
+                cat([b + (b >= 0) * (i * chunk * k) for i, b in enumerate(bidx)]), cat([p[4][:, :L] for p in parts]))
 
     def _generate_beam_static(self, ids: torch.Tensor, mask: Optional[torch.Tensor], gp, bp):
         B, S = ids.shape
@@ -653,6 +654,8 @@ class B200T5ForConditionalGeneration:
         return (~is_pad).to(torch.long).contiguous()
 
     def _generate_static(self, ids: torch.Tensor, mask: Optional[torch.Tensor], gp, lp=None, score: bool = False, labels=None):
+        """One static batch, full width: (ids [B, T+1], lengths [B]) and, with score=True, (token_logprobs [B, T],
+        token_logits [B, T]). The library pads every row to T+1 with pad_token_id."""
         B, S = ids.shape
         ids = ids.contiguous()
         mask = None if mask is None else mask.contiguous()
@@ -663,7 +666,7 @@ class B200T5ForConditionalGeneration:
             stream = torch.cuda.current_stream(self._device)
             with self._gpu_lock:
                 io = None
-                if score:  # full-width results: (ids [B, T+1], lengths, token_logprobs [B, T], token_logits [B, T])
+                if score:
                     logp = torch.empty((B, T), dtype=torch.float32, device=self._device)
                     logit = torch.empty((B, T), dtype=torch.float32, device=self._device)
                     forced = None if labels is None else torch.from_numpy(np.ascontiguousarray(labels)).to(self._device)
@@ -673,11 +676,8 @@ class B200T5ForConditionalGeneration:
                                                             None if io is None else C.byref(io), C.c_void_p(stream.cuda_stream)),
                      self._h)
                 self.last_lengths = lens
-                if score:
-                    torch.cuda.current_stream(self._device).synchronize()
-                    return out, lens, logp, logit
-                steps = int(lens.max().item())  # synchronises; HF returns exactly the steps it ran
-        return out[:, : steps + 1]
+                stream.synchronize()
+        return (out, lens, logp, logit) if score else (out, lens)
 
     def _infer_mask_np(self, ids: np.ndarray, gp, lp=None) -> Optional[np.ndarray]:
         pad = gp.pad_token_id if gp.pad_token_id >= 0 else self.generation_config.pad_token_id
@@ -690,9 +690,7 @@ class B200T5ForConditionalGeneration:
         H2D copy, generation, D2H copy and synchronisation all happen inside the library. Takes the logits
         processor kwargs `generate` takes. With output_scores=True it returns (ids, lengths, token_logprobs,
         token_logits), the last two fp32 [B, T']."""
-        gp = self._gen_params(kw.get("max_new_tokens"), kw.get("max_length"), kw.get("min_new_tokens"),
-                              kw.get("min_length"), kw.get("eos_token_id"), kw.get("pad_token_id"),
-                              kw.get("decoder_start_token_id"), kw.get("poll_interval", 8))
+        gp = self._gen_params(**kw)
         if kw.get("do_sample") and kw.get("num_beams") not in (None, 1):
             raise NotImplementedError("beam sampling (do_sample=True, num_beams > 1) is not implemented")
         bp = beam_params(kw.get("num_beams"), kw, _eos_ids(kw.get("eos_token_id")), self.generation_config.eos_token_id,
@@ -702,7 +700,8 @@ class B200T5ForConditionalGeneration:
         B, S = ids.shape
         mask = self._infer_mask_np(ids, gp, lp) if attention_mask is None else np.ascontiguousarray(attention_mask, dtype=np.int64)
         if bp is not None:
-            return self._generate_host_beam(ids, mask, gp, bp)
+            self._check_inputs(ids, mask)
+            return self._generate_beam(ids, mask, gp, bp, self._generate_host_beam_chunk)
         out = np.empty((B, gp.max_new_tokens + 1), dtype=np.int64)
         lens = np.empty((B,), dtype=np.int32)
         want_scores = generate_output_flags(kw)[1]
@@ -721,21 +720,6 @@ class B200T5ForConditionalGeneration:
         if want_scores:
             return out[:, : steps + 1], lens, logp[:, :steps], logit[:, :steps]
         return out[:, : steps + 1], lens
-
-    def _generate_host_beam(self, ids: np.ndarray, mask: Optional[np.ndarray], gp, bp):
-        """generate_host(num_beams=k): b200t5_generate_host_beam -> (sequences [B*n, 1+T'], lengths [B*n], sequences_scores
-        [B*n], beam_indices [B*n, T'], token_logprobs [B*n, T']), numpy; in static chunks of pool_size // k prompts, as
-        generate runs them."""
-        self._check_inputs(ids, mask)
-        chunk = max(1, self.pool_size // bp.num_beams)
-        parts = [self._generate_host_beam_chunk(ids[lo:lo + chunk], None if mask is None else mask[lo:lo + chunk], gp, bp)
-                 for lo in range(0, ids.shape[0], chunk)]
-        L = max(int(p[1].max()) for p in parts)
-        k = bp.num_beams
-        return (np.concatenate([p[0][:, : L + 1] for p in parts]), np.concatenate([p[1] for p in parts]),
-                np.concatenate([p[2] for p in parts]),
-                np.concatenate([np.where(p[3][:, :L] >= 0, p[3][:, :L] + i * chunk * k, p[3][:, :L]) for i, p in enumerate(parts)]),
-                np.concatenate([p[4][:, :L] for p in parts]))
 
     def _generate_host_beam_chunk(self, ids: np.ndarray, mask: Optional[np.ndarray], gp, bp):
         ids = np.ascontiguousarray(ids)
@@ -768,9 +752,7 @@ class B200T5ForConditionalGeneration:
         (int64 [N, 1+T'], int32 lengths [N]) with the rows in input order; every row equals what `generate` returns
         for that prompt. Takes the logits processor kwargs `generate` takes. With output_scores=True it returns (ids,
         lengths, token_logprobs, token_logits), the last two fp32 [N, T'] (b200t5_generate_stream_scored)."""
-        gp = _gen_params or self._gen_params(kw.get("max_new_tokens"), kw.get("max_length"), kw.get("min_new_tokens"),
-                                             kw.get("min_length"), kw.get("eos_token_id"), kw.get("pad_token_id"),
-                                             kw.get("decoder_start_token_id"), kw.get("poll_interval", 8))
+        gp = _gen_params or self._gen_params(**kw)
         lp = _logits if _gen_params is not None else self._logits_args(kw, kw.get("eos_token_id"))
         if kw.get("num_beams") not in (None, 1):
             raise NotImplementedError("generate_stream(num_beams > 1): beam search runs as static batches (generate)")
