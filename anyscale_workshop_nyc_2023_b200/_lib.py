@@ -141,6 +141,9 @@ SIGNATURES = {
     "b200t5_test_beam_step": (_i, [_i, _vp, _i, _i, _i, _i, _i, _i, _i, C.c_double, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                    _vp]),
     "b200t5_test_beam_reorder": (_i, [_i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "b200t5_test_beam_replicate": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "b200t5_test_beam_search": (_i, [_i, _vp, _i, _i, _i, _i, _i, _i, C.c_double, _i, _i, C.c_int64, C.c_int64, C.POINTER(BeamIO),
+                                     C.POINTER(C.c_int32), _vp, _vp, _vp]),
     "b200t5_get_stats": (_i, [_vp, C.POINTER(Stats)]),
     "b200t5_bench_cross_attn": (_i, [_vp, _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_double), _vp]),
     "b200t5_set_option": (_i, [_vp, C.c_char_p, _i]),

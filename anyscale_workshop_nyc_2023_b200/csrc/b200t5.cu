@@ -2723,6 +2723,73 @@ extern "C" int b200t5_test_beam_reorder(int device, void* kv, int planes, int B,
   return B200T5_OK;
 }
 
+extern "C" int b200t5_test_beam_replicate(int device, void* cross_kv, int32_t* extent, uint8_t* key_ok, int planes, int B, int k, int H,
+                                          int S, void* stream) {
+  int rc = hook_device(device);
+  if (rc < 0) return rc;
+  if (planes < 1 || B < 1 || k < 1 || k > kBeamMax || H < 1 || S < 1 || B * k > 65535) return fail(nullptr, B200T5_EINVAL, "bad replicate arguments");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  beam_replicate_kernel<<<dim3(planes * H, B * k), 256, 0, s>>>(static_cast<act_t*>(cross_kv), extent, key_ok, B * k, k, H, S);
+  cudaError_t e = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "beam replicate: %s", cudaGetErrorString(e));
+  return B200T5_OK;
+}
+
+extern "C" int b200t5_test_beam_search(int device, const float* logits, int B, int k, int V, int T, int eos, int min_new,
+                                       double length_penalty, int early_stopping, int n, int64_t start, int64_t pad,
+                                       const b200t5_beam_io* io, int32_t* steps, float* cand_lp, int32_t* cand_tok, void* stream) {
+  int rc = hook_device(device);
+  if (rc < 0) return rc;
+  if (B < 1 || k < 2 || k > kBeamMax || V < 2 * k || T < 1 || early_stopping < 0 || early_stopping > 2 || n < 1 || n > k || !io ||
+      !io->sequences || !io->lengths || (cand_lp == nullptr) != (cand_tok == nullptr))
+    return fail(nullptr, B200T5_EINVAL, "bad beam search arguments");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int rows = B * k;
+  DevBuf prm, ls, clp, ctk, rsc, hp, ht, hl, fin, heur, par, st, unf;
+  const BeamParams bp{k, T, min_new, eos, early_stopping, early_stopping == 2 && length_penalty > 0.0};
+  const std::vector<float> lsv = beam_len_scale(length_penalty, T);
+  const std::vector<int> ones(rows, 1);
+  const size_t hist = static_cast<size_t>(T) * rows * 4;
+  if (prm.alloc(sizeof(bp)) || ls.alloc(T * 4) || clp.alloc(rows * kBeamCand * 4) || ctk.alloc(rows * kBeamCand * 4) || rsc.alloc(rows * 4) ||
+      hp.alloc(hist) || ht.alloc(hist) || hl.alloc(hist) || fin.alloc(static_cast<size_t>(B) * kBeamMax * sizeof(BeamFin)) ||
+      heur.alloc(B * 4) || par.alloc(rows * 4) || st.alloc(sizeof(DecodeState)) || unf.alloc(rows * 4))
+    return fail(nullptr, B200T5_ECUDA, "allocation failed");
+  CU_OK(nullptr, cudaMemcpy(prm.p, &bp, sizeof(bp), cudaMemcpyHostToDevice));
+  CU_OK(nullptr, cudaMemcpy(ls.p, lsv.data(), T * 4, cudaMemcpyHostToDevice));
+  CU_OK(nullptr, cudaMemcpy(unf.p, ones.data(), rows * 4, cudaMemcpyHostToDevice));
+  BeamDev d{prm.as<BeamParams>(), ls.as<float>(), nullptr, nullptr, clp.as<float>(), ctk.as<int>(), rsc.as<float>(), hp.as<int>(), ht.as<int>(),
+            hl.as<float>(), fin.as<BeamFin>(), heur.as<int>(), par.as<int>(), rows};
+  beam_init_kernel<<<(std::max(rows, B * kBeamMax) + 255) / 256, 256, 0, s>>>(d, B, k);
+  // the decode loop of run_static_steps without the model: one unfinished array for the whole search, and a stop
+  // once every prompt has retired
+  std::vector<int> u(rows);
+  int ran = 0;
+  cudaError_t e = cudaSuccess;
+  for (int t = 0; t < T && e == cudaSuccess; ++t) {
+    d.logits = logits + static_cast<size_t>(t) * rows * V;
+    if (cand_lp != nullptr) {
+      d.cand_lp = cand_lp + static_cast<size_t>(t) * rows * kBeamCand;
+      d.cand_tok = cand_tok + static_cast<size_t>(t) * rows * kBeamCand;
+    }
+    set_state_kernel<<<1, 1, 0, s>>>(st.as<DecodeState>(), t);
+    beam_row_kernel<<<rows, kBeamRowThreads, 0, s>>>(d, V, st.as<DecodeState>(), unf.as<int>());
+    beam_select_kernel<<<B, 32, 0, s>>>(d, V, st.as<DecodeState>(), unf.as<int>(), nullptr, nullptr, nullptr, 0);
+    ++ran;
+    e = cudaMemcpyAsync(u.data(), unf.p, rows * 4, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (std::all_of(u.begin(), u.end(), [](int x) { return x == 0; })) break;
+  }
+  if (e == cudaSuccess) {
+    beam_output_kernel<<<(B * n + 127) / 128, 128, 0, s>>>(d, B, n, reinterpret_cast<long long*>(io->sequences), io->lengths,
+                                                            io->sequences_scores, reinterpret_cast<long long*>(io->beam_indices),
+                                                            io->token_logprobs, start, pad);
+    e = cudaStreamSynchronize(s);
+  }
+  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "beam search: %s", cudaGetErrorString(e));
+  if (steps != nullptr) *steps = ran;
+  return B200T5_OK;
+}
+
 extern "C" int b200t5_test_rmsnorm(int device, const void* x, const void* w, void* y, int M, int d, float eps, void* stream) {
   const int sms = hook_device(device);
   if (sms < 0) return sms;

@@ -302,6 +302,20 @@ int b200t5_test_beam_step(int device, const float* logits, int B, int k, int V, 
  * positions 0..step of row parent[r] (int32 [B*k], device, within r's prompt). Test hook; both builds. */
 int b200t5_test_beam_reorder(int device, void* kv, int planes, int B, int k, int H, int Tmax, int step, const int32_t* parent,
                              void* stream);
+/* beam_replicate_kernel on a cross-attention K/V [planes][B*k][H][S][64] of the build's 2-byte type, extent int32 [B*k]
+ * and key_ok uint8 [B*k][S] (device): rows b*k + j, j > 0, take the first extent[b*k] positions of row b*k, its extent and
+ * its key_ok. Test hook; both builds. */
+int b200t5_test_beam_replicate(int device, void* cross_kv, int32_t* extent, uint8_t* key_ok, int planes, int B, int k, int H, int S,
+                               void* stream);
+/* A whole beam search without the model, on the kernels the step graph runs: beam_init_kernel, then per step
+ * beam_row_kernel -> beam_select_kernel on the fp32 logits [T][B*k][V] (device) of that step (rows of retired prompts
+ * stop, as in b200t5_generate_beam; the search ends once every prompt has retired), then beam_output_kernel into io
+ * (device pointers, layout of b200t5_beam_io with max_new_tokens T and num_return_sequences n). Out: steps (host) the
+ * steps run; cand_lp fp32 / cand_tok int32 [T][B*k][32] (device, both NULL or neither) each live row's top 2k of each step,
+ * as b200t5_test_beam_step; a retired row's entries are left as they were. Test hook; both builds. */
+int b200t5_test_beam_search(int device, const float* logits, int B, int k, int V, int T, int eos, int min_new, double length_penalty,
+                            int early_stopping, int n, int64_t start, int64_t pad, const b200t5_beam_io* io, int32_t* steps,
+                            float* cand_lp, int32_t* cand_tok, void* stream);
 
 /* ---- parity hooks (used by tests/ only) --------------------------------------------- */
 /* Encoder last hidden state after the final RMSNorm, bf16 [B,S,d_model] (device). */

@@ -37,6 +37,24 @@ def length_scale(x, length: int, length_penalty: float, division: str = "recipro
     return (x * np.float32(1.0 / p) if division == "reciprocal" else x / np.float32(p)).astype(np.float32)
 
 
+def fma32(a, b, c) -> np.ndarray:
+    """fl(a * b + c) of fp32 values with one rounding, as a fused multiply-add computes it. The product is exact in
+    double; TwoSum gives the error of the double sum, which decides the fp32 rounding only when that sum lies halfway
+    between two fp32 values."""
+    a, b, c = np.broadcast_arrays(*(np.asarray(x, np.float32).astype(np.float64) for x in (a, b, c)))
+    with np.errstate(invalid="ignore", over="ignore"):
+        p = a * b
+        s = p + c
+        z = s - p
+        e = (p - (s - z)) + (c - z)
+        r = s.astype(np.float32)
+        other = np.nextafter(r, np.where(s > r, np.float32(np.inf), np.float32(-np.inf)))
+        tie = np.isfinite(s) & (s != r) & (np.abs(s - r) == np.abs(other.astype(np.float64) - s)) & (e != 0)
+        up = np.maximum(r, other)
+        down = np.minimum(r, other)
+    return np.where(tie, np.where(e > 0, up, down), r).astype(np.float32)
+
+
 class BeamState:
     """Per-prompt state of `_beam_search` for B prompts of k beams and at most T new tokens."""
 
@@ -59,10 +77,13 @@ class BeamState:
 
 
 def step(st: BeamState, logp: np.ndarray, t: int, eos: int, length_penalty: float = 1.0, early_stopping=False,
-         division: str = "reciprocal"):
+         division: str = "reciprocal", fma: bool = False):
     """Steps c-g of one `_beam_search` iteration at decode step t (cur_len = t + 1, max_length = T + 1) for every
     prompt. logp: fp32 [B*k, V], the log-probabilities after the EOS mask. Returns the flat parent rows [B*k] the cache
-    must be reordered by, and the next decoder tokens [B*k]. Also updates the decision gaps of live prompts."""
+    must be reordered by, and the next decoder tokens [B*k]. Also updates the decision gaps of live prompts.
+    fma: a candidate's finished-set score is fl(score * fp32(1 / l**p) + penalty) with one rounding, as
+    beam_select_kernel computes it (the compiler contracts it to an FFMA); transformers rounds the product first. The
+    two differ only in scores that carry the -1e9 penalty."""
     B, k, T = st.B, st.k, st.T
     V = logp.shape[1]
     K = 2 * k
@@ -93,17 +114,22 @@ def step(st: BeamState, logp: np.ndarray, t: int, eos: int, length_penalty: floa
         real = [rval[i] for i in ro[:k + 1] if rval[i] > _REAL]
         gaps += [a - b for a, b in zip(real, real[1:])]
         if len(real) == k and acc.size > K:  # the next candidate that does not hit lies beyond the top 2k
-            nxt = [acc[i] for i in o[K:] if not ((i % V) == eos or t + 1 >= T)][:1]
-            gaps += [real[-1] - nxt[0]] if nxt else []
+            nxt = next((acc[i] for i in o[K:] if not ((i % V) == eos or t + 1 >= T)), None)
+            gaps += [real[-1] - nxt] if nxt is not None else []
         # whether a candidate that hits is among the first k
         gaps += [cval[c] - cval[c + 1] for c in range(K - 1) if c + 1 <= k and hit[c] != hit[c + 1] and cval[c] > _REAL]
         # f. finished set
         did = hit & (np.arange(K) < k)
-        s = length_scale(cval, t + 1, length_penalty, division)
         full = bool(st.fin_flag[b].all()) and early_stopping is True
-        s = (s + (NEG if full else np.float32(0))).astype(np.float32)
-        s = (s + (np.float32(0) if st.heur[b] else NEG)).astype(np.float32)
-        s = (s + np.where(did, np.float32(0), NEG)).astype(np.float32)
+        if fma:
+            s = fma32(cval, length_scale(1.0, t + 1, length_penalty, division), np.where(did, np.float32(0), NEG))
+            s = (s + (NEG if full else np.float32(0))).astype(np.float32)
+            s = (s + (np.float32(0) if st.heur[b] else NEG)).astype(np.float32)
+        else:
+            s = length_scale(cval, t + 1, length_penalty, division)
+            s = (s + (NEG if full else np.float32(0))).astype(np.float32)
+            s = (s + (np.float32(0) if st.heur[b] else NEG)).astype(np.float32)
+            s = (s + np.where(did, np.float32(0), NEG)).astype(np.float32)
         merged = np.concatenate([st.fin_score[b], s])
         mo = order(merged)
         # the finished set, its order (the returned rows) and the best entry left out

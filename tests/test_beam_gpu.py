@@ -95,16 +95,29 @@ def test_beam_step_matches_torch_and_the_oracle_step(flavour, k, lp, es):
         assert ((heur.cpu().numpy() != 0) == st.heur)[live].all()
 
 
+# FLAN-T5-base's 24 planes and 12 heads: (k, Tmax, step), steps whose (step + 1) * 8 chunks take the 128-thread loop
+# 1 to 9 times
+REORDER_CASES = {f"k{k}-T{T}-s{s}": (k, T, s) for k in (2, 5, 16) for T in (40, 129) for s in sorted({0, 15, 16, 127, T - 1}) if s < T}
+
+
 @pytest.mark.parametrize("flavour", FLAVOURS)
-@pytest.mark.parametrize("pmap", ["identity", "all_from_one", "cycle"])
+@pytest.mark.parametrize("pmap", ["identity", "all_from_one", "cycle", *REORDER_CASES])
 def test_reorder_matches_index_select(flavour, pmap):
     lib = _lib.load(flavour)
     dt = torch.bfloat16 if flavour == "bf16" else torch.float16
-    planes, B, k, H, Tmax, step = 4, 3, 4, 2, 16, 9
+    if pmap in REORDER_CASES:  # parents drawn with replacement inside each prompt; prompt 0 keeps its own rows
+        k, Tmax, step = REORDER_CASES[pmap]
+        planes, B, H = 24, 3, 12
+        rng = np.random.default_rng(Tmax * 100 + step * 10 + k)
+        parent = torch.tensor([b * k + (j if b == 0 else int(rng.integers(k))) for b in range(B) for j in range(k)], dtype=torch.int32,
+                              device="cuda")
+    else:
+        planes, B, k, H, Tmax, step = 4, 3, 4, 2, 16, 9
+        base = {"identity": [0, 1, 2, 3], "all_from_one": [2, 2, 2, 2], "cycle": [1, 0, 3, 2]}[pmap]
+        parent = torch.tensor([b * k + j for b in range(B) for j in base], dtype=torch.int32, device="cuda")
     g = torch.Generator(device="cuda").manual_seed(7)
     kv = (torch.randn(planes, B * k, H, Tmax, 64, device="cuda", generator=g)).to(dt)
-    base = {"identity": [0, 1, 2, 3], "all_from_one": [2, 2, 2, 2], "cycle": [1, 0, 3, 2]}[pmap]
-    parent = torch.tensor([b * k + j for b in range(B) for j in base], dtype=torch.int32, device="cuda")
+    kv[:, :, :, step + 1:] = float("nan")  # positions the step has not reached: neither read nor written
     want = kv.clone()
     want[:, :, :, : step + 1] = kv.index_select(1, parent.long())[:, :, :, : step + 1]
     _lib.check(lib.b200t5_test_beam_reorder(DEV, P(kv), planes, B, k, H, Tmax, step, P(parent), None), lib=lib)
@@ -113,8 +126,17 @@ def test_reorder_matches_index_select(flavour, pmap):
 
 
 # ----------------------------------------------------------------------------------------------------- model
-BEAM_CASES = [("tiny", 1, 4, 1, 1.0, False, 0), ("tiny", 1, 2, 2, 2.0, "never", 3), ("mini", 2, 4, 4, 0.0, True, 0),
-              ("mini", 2, 3, 1, -0.5, False, 0)]
+# (model, seed, k, n, length_penalty, early_stopping, min_new_tokens, prompt lengths); "full" prompts fill the window,
+# so the stream cross-attention kernel runs
+BEAM_CASES = [("tiny", 1, 4, 1, 1.0, False, 0, "uniform"), ("tiny", 1, 2, 2, 2.0, "never", 3, "uniform"),
+              ("mini", 2, 4, 4, 0.0, True, 0, "uniform"), ("mini", 2, 3, 1, -0.5, False, 0, "uniform"),
+              ("mini", 2, 8, 1, 1.0, "never", 0, "uniform"), ("tiny", 1, 8, 8, 1.0, False, 2, "full"),
+              ("tiny", 1, 16, 1, 0.0, True, 0, "full"), ("tiny", 1, 16, 16, 1.0, False, 0, "uniform"),
+              ("mini", 2, 4, 2, 1.0, False, 0, "full")]
+
+
+def _beam_case_id(c):
+    return f"{c[0]}-k{c[2]}-n{c[3]}" + ("" if c[7] == "uniform" else f"-{c[7]}")
 
 
 def _compare(out, ref, gaps, n, tau, lp):
@@ -137,14 +159,14 @@ def _compare(out, ref, gaps, n, tau, lp):
     return safe, equal
 
 
-@pytest.mark.parametrize("case", BEAM_CASES, ids=[f"{c[0]}-k{c[2]}-n{c[3]}" for c in BEAM_CASES])
+@pytest.mark.parametrize("case", BEAM_CASES, ids=[_beam_case_id(c) for c in BEAM_CASES])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16], ids=["bf16", "fp16"])
 def test_model_matches_the_oracle(models, case, dtype):
-    name, seed, k, n, lp, es, mn = case
+    name, seed, k, n, lp, es, mn, lengths = case
     model, _ = models(name, seed, dtype)
     spec = SPECS[name]
     B, T = 12, 12
-    ids, mask = synthetic_token_batch(B, 32, spec.vocab_size, seed=41 + k, lengths="uniform")
+    ids, mask = synthetic_token_batch(B, 32, spec.vocab_size, seed=41 + k, lengths=lengths)
     o = T5Oracle(make_state_dict(spec, seed), spec, emulate="bf16" if dtype == torch.bfloat16 else "fp16")
     ref = obeam.beam_search(o, ids, mask, num_beams=k, max_new_tokens=T, min_new_tokens=mn, num_return_sequences=n,
                             length_penalty=lp, early_stopping=es)
@@ -152,6 +174,7 @@ def test_model_matches_the_oracle(models, case, dtype):
                          num_beams=k, num_return_sequences=n, length_penalty=lp, early_stopping=es, return_dict_in_generate=True,
                          output_scores=True)
     assert out.sequences.shape[0] == B * n and out.sequences.dtype == torch.long and out.sequences.device.type == "cuda"
+    assert model.stats()["xattn_kernel"] == (1 if lengths == "full" else 0)  # 1: the stream kernel
     tau = TAU[dtype]
     # 1. Every returned hypothesis, whatever near-ties chose it, is what the oracle computes along it: each token's
     #    log-probability given the prompt and the hypothesis' own prefix (the EOS mask of min_new_tokens included), its
