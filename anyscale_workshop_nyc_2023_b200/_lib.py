@@ -99,6 +99,13 @@ class BeamIO(C.Structure):
     ]
 
 
+class ForwardIO(C.Structure):
+    _fields_ = [
+        ("logits", C.c_void_p),
+        ("token_logprobs", C.c_void_p),
+    ]
+
+
 class Stats(C.Structure):
     _fields_ = [
         ("encoder_ms", C.c_float),
@@ -155,6 +162,7 @@ SIGNATURES = {
                                   _vp, _vp, _vp, _vp]),
     "b200t5_encode": (_i, [_vp, _i64p, _i64p, _i, _i, _vp, _vp]),
     "b200t5_decode_logits": (_i, [_vp, _i64p, _i64p, _i, _i, _i64p, _i, _vp, _vp]),
+    "b200t5_forward": (_i, [_vp, _i64p, _i64p, _i, _i, _i64p, _i64p, _i, C.POINTER(ForwardIO), _vp]),
     "b200t5_relative_bucket": (_i, [_i, _i, _i, _i]),
     "b200t5_test_gemm": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "b200t5_test_enc_gemm": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp]),
@@ -163,6 +171,8 @@ SIGNATURES = {
     "b200t5_test_rmsnorm": (_i, [_i, _vp, _vp, _vp, _i, _i, C.c_float, _vp]),
     "b200t5_test_attn_decode": (_i, [_i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "b200t5_test_encoder_attn": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "b200t5_test_decoder_self_attn": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "b200t5_test_decoder_cross_attn": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b200t5_test_geglu": (_i, [_i, _vp, _vp, _vp, C.c_int64, _i, _vp]),
     "b200t5_version": (C.c_char_p, []),
 }

@@ -15,6 +15,8 @@
 // p = 0 times a NaN or Inf there would still poison P.V.
 // Packed rows (cu != NULL): prompt b occupies rows cu[b] .. cu[b] + extent[b] - 1 of qkv and ctx, and only
 // those query rows are computed and written.
+// attention_decoder.cuh (attn_tile_2pass) repeats this kernel's two-pass loop for the decoder's forward-pass attentions:
+// a change to the rounding contract here belongs there too. (A shared function changes this kernel's SASS.)
 #pragma once
 #include "attention_decode.cuh"
 #include "ptx.cuh"

@@ -25,6 +25,7 @@
 #include "attention_decode.cuh"
 #include "attention_cross_stream.cuh"
 #include "attention_encoder.cuh"
+#include "attention_decoder.cuh"
 #include "beam.cuh"
 #include "elementwise.cuh"
 #include "gemm.cuh"
@@ -187,6 +188,8 @@ struct EncLayerW {
 struct DecLayerW {
   DevBuf ln0, ln1, ln2, wqkv, wo, wcq, wco, wi, wff_o;  // wi interleaved per N-tile of the decode wi GEMM
   CUtensorMap tm_qkv, tm_o, tm_cq, tm_co, tm_wi, tm_ffo;
+  // the same weights in boxes of 128 rows, for the 128 x 256 GEMMs of the forward pass (b200t5_forward)
+  CUtensorMap tm2_qkv, tm2_o, tm2_cq, tm2_co, tm2_ffo;
   int wi_rows = 0;
 };
 
@@ -303,8 +306,9 @@ struct StepMode {
 struct Plan {
   int B = 0, S = 0, Tmax = 0;
   int group = 1;  // rows per prompt (num_beams): the row-chains split on prompt boundaries
-  // encoder workspace
-  DevBuf x, xn, qkv, ctx, hff;          // [B*S, d], [B*S, d], [B*S, 3I], [B*S, I], [B*S, F]
+  int ws_S = 0;   // rows per prompt of the encoder workspace: S, or the forward pass's T when that is longer
+  // encoder workspace, and the forward pass's decoder workspace once the cross-K/V projection has run
+  DevBuf x, xn, qkv, ctx, hff;          // [B*ws_S, d], [B*ws_S, d], [B*ws_S, 3I], [B*ws_S, I], [B*ws_S, F]
   DevBuf key_ok, extent, enc_bias;      // uint8 [B,S], int [B], float [H][2S-1]
   DevBuf cu, row_b, row_s;              // packed encoder rows: int [B+1] offsets, int [B*S] row -> (prompt, position)
   int* h_cu = nullptr;                  // pinned copy of cu[B] (number of packed rows)
@@ -337,6 +341,10 @@ struct Plan {
   ProcBufs proc;                 // logits processors (allocated by the first call that uses them)
   DevBuf psum, fval, ftok;       // token log-probabilities (likewise): [B][n_tiles], [B], [B]
   BeamBufs beam;
+  // the forward pass (b200t5_forward), allocated by its first call: the decoder ids int64 [B*T], the label columns
+  // int32 [B*T] and a zero step; the causal bias float [H][fwd_T]; the lm_head partials when they do not fit in hff
+  DevBuf fwd_ids, fwd_bias, fwd_part;
+  int fwd_T = 0;
   StepMode mode;                 // what this call's steps run
   std::optional<StepMode> graph_mode;  // what the step graphs were captured for (none: re-capture)
   // after a reallocation of a buffer the step graph bakes: the next ensure_graph re-captures
@@ -579,6 +587,14 @@ static cudaError_t init_kernel_attrs() {
   if ((e = prepare_gemm_2cta<EpiResidual, B200T5_F16 != 0>()) != cudaSuccess) return e;
   if ((e = prepare_gemm_splitk<64, EpiResidual, B200T5_F16 != 0>()) != cudaSuccess) return e;
   if ((e = prepare_gemm_splitk<128, EpiResidual, B200T5_F16 != 0>()) != cudaSuccess) return e;
+  // the teacher-forced forward pass (b200t5_forward): the GeGLU product on the decode packing, the lm_head variants
+  if ((e = prepare_gemm<128, EpiGegluNarrow>()) != cudaSuccess) return e;
+  if ((e = prepare_gemm<128, EpiLmLogits<false>>()) != cudaSuccess) return e;
+  if ((e = prepare_gemm<128, EpiLmLogits<true>>()) != cudaSuccess) return e;
+  if ((e = cudaFuncSetAttribute(decoder_attn_kernel<kAttnCausal>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024)) != cudaSuccess)
+    return e;
+  if ((e = cudaFuncSetAttribute(decoder_attn_kernel<kAttnCross>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024)) != cudaSuccess)
+    return e;
   if ((e = cudaFuncSetAttribute(attn_cross_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 static_cast<int>(XsSmem::bytes(kXsMaxStages, 4096)))) != cudaSuccess)
     return e;
@@ -983,6 +999,11 @@ extern "C" int b200t5_finalize(b200t5_handle h) {
     TMAP(h, &w.tm_co, w.wco.p, d, I, bn_proj);
     TMAP(h, &w.tm_wi, w.wi.p, wi_rows, d, bn_wi);
     TMAP_FFO(h, &w.tm_ffo, w.wff_o.p, d, h->ffo_k, bn_ffo);
+    TMAP(h, &w.tm2_qkv, w.wqkv.p, 3 * I, d, k2ctaBox);
+    TMAP(h, &w.tm2_o, w.wo.p, d, I, k2ctaBox);
+    TMAP(h, &w.tm2_cq, w.wcq.p, I, d, k2ctaBox);
+    TMAP(h, &w.tm2_co, w.wco.p, d, I, k2ctaBox);
+    TMAP_FFO(h, &w.tm2_ffo, w.wff_o.p, d, h->ffo_k, k2ctaBox);
   }
   TMAP(h, &h->tm_crosskv, h->wcrosskv.p, static_cast<uint64_t>(c.Ld) * 2 * I, d, k2ctaBox);
 
@@ -995,20 +1016,21 @@ extern "C" int b200t5_finalize(b200t5_handle h) {
 
 
 // ================================================================== plans
-static int build_plan(b200t5_ctx* h, int B, int S, int Tmax, int group) {
+static int build_plan(b200t5_ctx* h, int B, int S, int Tmax, int group, int ws_S) {
   const Cfg& c = h->c;
   std::unique_ptr<Plan> pl(new Plan());
   pl->B = B;
   pl->S = S;
   pl->Tmax = Tmax;
   pl->group = group;
-  const size_t M = static_cast<size_t>(B) * S;
+  pl->ws_S = ws_S;
+  const size_t M = static_cast<size_t>(B) * S, Mw = static_cast<size_t>(B) * ws_S;
   const int d = c.d, I = c.I, F = c.F, H = c.H;
-  CU_OK(h, pl->x.alloc(M * d * sizeof(res_t)));
-  CU_OK(h, pl->xn.alloc(M * d * 2));
-  CU_OK(h, pl->qkv.alloc(M * 3 * I * 2));
-  CU_OK(h, pl->ctx.alloc(M * I * 2));
-  CU_OK(h, pl->hff.alloc(M * F * sizeof(ffh_t)));
+  CU_OK(h, pl->x.alloc(Mw * d * sizeof(res_t)));
+  CU_OK(h, pl->xn.alloc(Mw * d * 2));
+  CU_OK(h, pl->qkv.alloc(Mw * 3 * I * 2));
+  CU_OK(h, pl->ctx.alloc(Mw * I * 2));
+  CU_OK(h, pl->hff.alloc(Mw * F * sizeof(ffh_t)));
   CU_OK(h, pl->key_ok.alloc(M));
   CU_OK(h, pl->extent.alloc(static_cast<size_t>(B) * 4));
   CU_OK(h, pl->cu.alloc(static_cast<size_t>(B + 1) * 4));
@@ -1071,9 +1093,9 @@ static int build_plan(b200t5_ctx* h, int B, int S, int Tmax, int group) {
     CU_OK(h, pl->dec_bias.alloc(db.size() * 4));
     CU_OK(h, cudaMemcpy(pl->dec_bias.p, db.data(), db.size() * 4, cudaMemcpyHostToDevice));
   }
-  TMAP(h, &pl->tm_xn, pl->xn.p, M, d, 128);
-  TMAP(h, &pl->tm_ctx, pl->ctx.p, M, I, 128);
-  TMAP_FFO(h, &pl->tm_hff, pl->hff.p, M, F, 128);
+  TMAP(h, &pl->tm_xn, pl->xn.p, Mw, d, 128);
+  TMAP(h, &pl->tm_ctx, pl->ctx.p, Mw, I, 128);
+  TMAP_FFO(h, &pl->tm_hff, pl->hff.p, Mw, F, 128);
   TMAP(h, &pl->tm_cross_kv, pl->cross_kv.p, static_cast<uint64_t>(c.Ld) * 2 * B * H * S, 64, kXsChunkKeys);
   CU_OK(h, cudaMemset(pl->ctx.p, 0, pl->ctx.bytes));  // padded query tiles are skipped: keep them finite
   {
@@ -1102,7 +1124,7 @@ static int ensure_plan(b200t5_ctx* h, int B, int S, int Tmax, int group = 1) {
   if (h->plan && h->plan->B == B && h->plan->S == S && h->plan->Tmax == Tmax && h->plan->group == group) return B200T5_OK;
   CU_OK(h, cudaDeviceSynchronize());
   h->plan.reset();
-  return build_plan(h, B, S, Tmax, group);
+  return build_plan(h, B, S, Tmax, group, S);
 }
 
 // ================================================================== encoder
@@ -2374,6 +2396,185 @@ extern "C" int b200t5_decode_logits(b200t5_handle h, const int64_t* input_ids, c
   return B200T5_OK;
 }
 
+// ================================================================== teacher-forced forward pass
+// The forward pass's GeGLU product: the decoder's wi is interleaved per 128-row tile for the split-K decode GEMM, so its
+// B*T-row product runs 128 x 128 tiles that read that packing (the encoder's 128 x 256 tiles would need a second copy).
+static cudaError_t run_geglu_fwd(b200t5_ctx* h, const CUtensorMap& tmA, const DecLayerW& w, int M, const EpiGeglu::Params& ep, cudaStream_t s) {
+  h->launches++;
+  return launch_gemm<128, EpiGegluNarrow>(tmA, w.tm_wi, M, w.wi_rows, h->c.d, 0, ep, h->num_sms, s);
+}
+
+// The decoder layer stack over all B*T positions at once (T5Stack with is_decoder, no cache), from x = the embedded
+// decoder ids to xn = the final RMSNorm, in the plan's encoder workspace; the epilogue flags of each product are the
+// decode step's (chain_layer_pre / chain_layer_post). The products run the encoder's 128 x 256 GEMMs through the
+// layer's 128-row-box tensor maps, except GeGLU (run_geglu_fwd).
+static int run_decoder_forward(b200t5_ctx* h, int T, cudaStream_t s) {
+  const Cfg& c = h->c;
+  Plan& p = *h->plan;
+  const int B = p.B, S = p.S, d = c.d, I = c.I, F = c.F, H = c.H, M = B * T;
+  res_t* x = p.x.as<res_t>();
+  act_t* xn = p.xn.as<act_t>();
+  act_t* qkv = p.qkv.as<act_t>();
+  act_t* ctx = p.ctx.as<act_t>();
+  const dim3 agrid((T + kEncQ - 1) / kEncQ, B * H);
+  for (int l = 0; l < c.Ld; ++l) {
+    DecLayerW& w = h->dec[l];
+    CU_OK(h, run_rmsnorm(h, x, w.ln0.as<act_t>(), xn, M, d, c.eps, s));
+    CU_OK(h, run_gemm_2cta<EpiStore>(h, p.tm_xn, w.tm2_qkv, M, 3 * I, d, EpiStore::Params{qkv, 3 * I}, s));
+    decoder_attn_kernel<kAttnCausal><<<agrid, kEncThreads, encoder_attn_smem_bytes(T), s>>>(
+        qkv, nullptr, ctx, p.fwd_bias.as<float>(), nullptr, nullptr, B, T, T, H);
+    h->launches++;
+    CU_OK(h, cudaGetLastError());
+    {
+      EpiResidual::Params ep{x, x, d};
+      ep.round_out = l == 0;  // (fp16 build) the stream is still fp16 before the first feed-forward block
+      CU_OK(h, run_gemm_2cta<EpiResidual>(h, p.tm_ctx, w.tm2_o, M, d, I, ep, s));
+    }
+    CU_OK(h, run_rmsnorm(h, x, w.ln1.as<act_t>(), xn, M, d, c.eps, s));
+    CU_OK(h, run_gemm_2cta<EpiStore>(h, p.tm_xn, w.tm2_cq, M, I, d, EpiStore::Params{qkv, I}, s));
+    decoder_attn_kernel<kAttnCross><<<agrid, kEncThreads, encoder_attn_smem_bytes(S), s>>>(
+        qkv, p.cross_kv.as<act_t>() + static_cast<size_t>(l) * 2 * B * I * S, ctx, nullptr, p.key_ok.as<unsigned char>(),
+        p.extent.as<int>(), B, T, S, H);
+    h->launches++;
+    CU_OK(h, cudaGetLastError());
+    {
+      EpiResidual::Params ep{x, x, d};
+      ep.round_out = l == 0;
+      CU_OK(h, run_gemm_2cta<EpiResidual>(h, p.tm_ctx, w.tm2_co, M, d, I, ep, s));
+    }
+    CU_OK(h, run_rmsnorm(h, x, w.ln2.as<act_t>(), xn, M, d, c.eps, s));
+    CU_OK(h, run_geglu_fwd(h, p.tm_xn, w, M, EpiGeglu::Params{p.hff.as<ffh_t>(), F, h->gelu_lut}, s));
+    {
+      EpiResidual::Params ep{x, x, d};
+      ep.round_acc = B200T5_F16 ? 0 : 1;  // fp16 build: `wo` is an fp32 Linear, its output is not rounded
+      ep.round_out = B200T5_F16 ? 0 : 1;
+      CU_OK(h, run_ffo_2cta(h, p.tm_hff, w.tm2_ffo, M, d, ep, s));
+    }
+  }
+  CU_OK(h, run_rmsnorm(h, x, h->dec_final_ln.as<act_t>(), xn, M, d, c.eps, s));
+  return B200T5_OK;
+}
+
+extern "C" int b200t5_forward(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                              const int64_t* decoder_input_ids, const int64_t* labels, int T, const b200t5_forward_io* io,
+                              void* stream) {
+  TRY(validate(h, B, S, nullptr));
+  if (!input_ids || !io) return fail(h, B200T5_EINVAL, "forward: null argument");
+  if (!decoder_input_ids && !labels) return fail(h, B200T5_EINVAL, "forward: decoder_input_ids or labels is required");
+  if (!io->logits && !io->token_logprobs) return fail(h, B200T5_EINVAL, "forward: neither logits nor token_logprobs requested");
+  if (io->token_logprobs && !labels) return fail(h, B200T5_EINVAL, "forward: token_logprobs needs labels");
+  if (T < 1 || T > 4096) return fail(h, B200T5_EINVAL, "forward: T=%d outside [1, 4096]", T);
+  if (h->sk_wi.bn != 128)
+    return fail(h, B200T5_EINVAL, "forward: needs the feed-forward wi packed in 128-row tiles, but B200T5_SK set the wi tile to %d rows "
+                "(unset B200T5_SK or give wi a bn of 128)", h->sk_wi.bn);
+  CU_OK(h, cudaSetDevice(h->device));
+  const Cfg& c = h->c;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t M = static_cast<size_t>(B) * T;
+  if (M > static_cast<size_t>(INT32_MAX) / 8) return fail(h, B200T5_EINVAL, "forward: B*T too large");
+  // labels and decoder ids are read back and checked; without decoder ids they are transformers' _shift_right(labels)
+  std::vector<long long> lab, dec(M);
+  CU_OK(h, cudaStreamSynchronize(s));
+  if (labels) {
+    lab.resize(M);
+    CU_OK(h, cudaMemcpy(lab.data(), labels, M * 8, cudaMemcpyDeviceToHost));
+    for (long long v : lab)
+      if (v != -100 && (v < 0 || v >= c.V)) return fail(h, B200T5_EINVAL, "forward: label %lld outside [0, %d) and not -100", v, c.V);
+  }
+  if (decoder_input_ids) {
+    CU_OK(h, cudaMemcpy(dec.data(), decoder_input_ids, M * 8, cudaMemcpyDeviceToHost));
+    for (long long v : dec)
+      if (v < 0 || v >= c.V) return fail(h, B200T5_EINVAL, "forward: decoder id %lld outside [0, %d)", v, c.V);
+  } else {
+    if (c.start < 0 || c.start >= c.V || c.pad < 0 || c.pad >= c.V) return fail(h, B200T5_EINVAL, "forward: special token id out of range");
+    for (size_t b = 0; b < static_cast<size_t>(B); ++b)
+      for (int t = 0; t < T; ++t) {
+        const long long v = t == 0 ? c.start : lab[b * T + t - 1];
+        dec[b * T + t] = v == -100 ? c.pad : v;
+      }
+  }
+  // the plan of (B, S): reused whatever its Tmax when its workspace holds B*T rows, else rebuilt with the same Tmax
+  // (1 for a new shape: the forward pass has no self-attention cache)
+  {
+    const int ws = std::max(S, T);
+    const bool same = h->plan && h->plan->B == B && h->plan->S == S && h->plan->group == 1;
+    if (!same || h->plan->ws_S < ws) {
+      const int Tm = same ? h->plan->Tmax : 1;
+      CU_OK(h, cudaDeviceSynchronize());
+      h->plan.reset();
+      TRY(build_plan(h, B, S, Tm, 1, ws));
+    }
+  }
+  Plan& p = *h->plan;
+  const int nt = p.n_vtiles;
+  // ids [M] int64, label columns [M] int32, one zero int (the lm_head's step: min_new is 0)
+  const size_t ids_bytes = M * 8 + M * 4 + 16;
+  if (p.fwd_ids.bytes < ids_bytes) CU_OK(h, p.fwd_ids.alloc(ids_bytes));
+  long long* ids_dev = p.fwd_ids.as<long long>();
+  int* ftok_dev = reinterpret_cast<int*>(ids_dev + M);
+  int* zero_dev = ftok_dev + M;
+  std::vector<int> ftok(M + 4, 0);
+  for (size_t m = 0; m < M && labels; ++m) ftok[m] = lab[m] == -100 ? -1 : static_cast<int>(lab[m]);
+  CU_OK(h, cudaMemcpyAsync(ids_dev, dec.data(), M * 8, cudaMemcpyHostToDevice, s));
+  CU_OK(h, cudaMemcpyAsync(ftok_dev, ftok.data(), (M + 4) * 4, cudaMemcpyHostToDevice, s));
+  if (p.fwd_T != T) {
+    // dec_relbias by distance i - j, as the decode step's dec_bias
+    std::vector<float> db(static_cast<size_t>(c.H) * T);
+    for (int n = 0; n < T; ++n) {
+      const int bk = b200t5_relative_bucket(-n, 0, c.nb, c.maxdist);
+      for (int hh = 0; hh < c.H; ++hh) db[static_cast<size_t>(hh) * T + n] = h->dec_relbias_h[static_cast<size_t>(bk) * c.H + hh];
+    }
+    CU_OK(h, p.fwd_bias.alloc(db.size() * 4));
+    CU_OK(h, cudaMemcpy(p.fwd_bias.p, db.data(), db.size() * 4, cudaMemcpyHostToDevice));
+    p.fwd_T = T;
+  }
+  // lm_head partials [M][n_tiles] x 3 + fval [M]: in hff (free after the last feed-forward block) when they fit
+  const bool lp_on = io->token_logprobs != nullptr;
+  const size_t part_bytes = lp_on ? M * (static_cast<size_t>(3) * nt + 1) * 4 : 0;
+  float* part = p.hff.as<float>();
+  if (part_bytes > p.hff.bytes) {
+    if (p.fwd_part.bytes < part_bytes) CU_OK(h, p.fwd_part.alloc(part_bytes));
+    part = p.fwd_part.as<float>();
+  }
+  h->launches = 0;
+  CU_OK(h, cudaEventRecord(h->ev[0], s));
+  TRY(run_encoder(h, reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(attention_mask), s));
+  TRY(run_cross_kv(h, s));
+  CU_OK(h, cudaEventRecord(h->ev[1], s));
+  embed_rows_kernel<<<static_cast<unsigned>((M + 7) / 8), 256, 0, s>>>(ids_dev, h->shared.as<act_t>(), p.x.as<res_t>(), static_cast<int>(M), c.d, c.V);
+  h->launches++;
+  TRY(run_decoder_forward(h, T, s));
+  LmHeadParams ep{};
+  ep.pval = part;
+  ep.pidx = reinterpret_cast<int*>(part + M * nt);
+  ep.psum = part + 2 * M * nt;
+  ep.fval = part + 3 * M * nt;
+  ep.ftok = ftok_dev;
+  ep.n_tiles = nt;
+  ep.step = zero_dev;
+  ep.eos = -1;
+  ep.min_new = 0;
+  h->launches++;
+  if (io->logits) {
+    const size_t ldc = static_cast<size_t>(c.V);
+    if (lp_on) CU_OK(h, (launch_gemm<128, EpiLmLogits<true>>(p.tm_xn, h->tm_lm, static_cast<int>(M), c.V, c.d, 1,
+                                                             EpiLmLogits<true>::Params{ep, static_cast<act_t*>(io->logits), ldc}, h->num_sms, s)));
+    else CU_OK(h, (launch_gemm<128, EpiLmLogits<false>>(p.tm_xn, h->tm_lm, static_cast<int>(M), c.V, c.d, 1,
+                                                        EpiLmLogits<false>::Params{ep, static_cast<act_t*>(io->logits), ldc}, h->num_sms, s)));
+  } else {
+    CU_OK(h, (launch_gemm<128, EpiLmHead<false, true>>(p.tm_xn, h->tm_lm, static_cast<int>(M), c.V, c.d, 1, ep, h->num_sms, s)));
+  }
+  if (lp_on) {
+    forward_logprob_kernel<<<static_cast<unsigned>(M), 128, 0, s>>>(ep.pval, ep.psum, ep.fval, ftok_dev, nt, io->token_logprobs);
+    h->launches++;
+  }
+  CU_OK(h, cudaGetLastError());
+  CU_OK(h, cudaEventRecord(h->ev[2], s));
+  h->last_steps = 0;
+  h->ev_valid = true;
+  return B200T5_OK;
+}
+
 // ================================================================== single-kernel hooks
 [[maybe_unused]] static int hook_device(int device) {
   int sms = check_device(nullptr, device);
@@ -2856,6 +3057,31 @@ extern "C" int b200t5_test_encoder_attn(int device, const void* qkv, void* ctx, 
     e = cudaGetLastError();
   }
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "encoder_attn: %s", cudaGetErrorString(e));
+  return B200T5_OK;
+}
+
+extern "C" int b200t5_test_decoder_self_attn(int device, const void* qkv, void* ctx, const float* dist_bias, int B, int T, int H,
+                                             void* stream) {
+  const int sms = hook_device(device);
+  if (sms < 0) return sms;
+  if (!qkv || !ctx || !dist_bias || B < 1 || H < 1 || T < 1 || T > 4096) return fail(nullptr, B200T5_EINVAL, "decoder_self_attn: bad argument");
+  decoder_attn_kernel<kAttnCausal><<<dim3((T + kEncQ - 1) / kEncQ, B * H), kEncThreads, encoder_attn_smem_bytes(T), static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const act_t*>(qkv), nullptr, static_cast<act_t*>(ctx), dist_bias, nullptr, nullptr, B, T, T, H);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "decoder_self_attn: %s", cudaGetErrorString(e));
+  return B200T5_OK;
+}
+
+extern "C" int b200t5_test_decoder_cross_attn(int device, const void* q, const void* kv, void* ctx, const uint8_t* key_ok,
+                                              const int32_t* extent, int B, int T, int S, int H, void* stream) {
+  const int sms = hook_device(device);
+  if (sms < 0) return sms;
+  if (!q || !kv || !ctx || !key_ok || !extent || B < 1 || H < 1 || T < 1 || S < 1 || encoder_attn_smem_bytes(S) > 96 * 1024)
+    return fail(nullptr, B200T5_EINVAL, "decoder_cross_attn: bad argument");
+  decoder_attn_kernel<kAttnCross><<<dim3((T + kEncQ - 1) / kEncQ, B * H), kEncThreads, encoder_attn_smem_bytes(S), static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const act_t*>(q), static_cast<const act_t*>(kv), static_cast<act_t*>(ctx), nullptr, key_ok, extent, B, T, S, H);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "decoder_cross_attn: %s", cudaGetErrorString(e));
   return B200T5_OK;
 }
 

@@ -332,6 +332,7 @@ struct FinalizeArgs {
   ScoreDev sd;  // kScore
 };
 
+// forward_logprob_kernel below repeats the kScore merge in the same order: a change to it belongs there too.
 template <bool kProc, bool kScore>
 __global__ void finalize_step_kernel(const FinalizeArgs a) {
   pdl_launch_dependents();
@@ -506,6 +507,36 @@ __global__ void advance_step_kernel(DecodeState* st, unsigned long long* __restr
         acc[2 * (n_slots + l) + 1] += 1;
       }
     }
+  }
+}
+
+// The teacher-forced forward pass (b200t5_forward): one 128-thread CTA per label position m of the B*T rows, after the
+// lm_head epilogue EpiLmHead<false, true> left the row's partials and, in fval[m], the value of its label column ftok[m]:
+//   logprob[m] = fval[m] - (M + logf(S))   (0 where ftok[m] < 0, i.e. the label is -100)
+// with M and S merged exactly as finalize_step_kernel<*, true> merges them (the order described above), so a
+// position's number is computed as a scored decode step computes it from the same partials.
+__global__ void forward_logprob_kernel(const float* __restrict__ pval, const float* __restrict__ psum, const float* __restrict__ fval,
+                                       const int* __restrict__ ftok, int n_tiles, float* __restrict__ logprob) {
+  const size_t p0 = static_cast<size_t>(blockIdx.x) * n_tiles;
+  __shared__ float s_v[32], s_s[32];
+  const int warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
+  float mx = -INFINITY;
+  for (int i = threadIdx.x; i < n_tiles; i += blockDim.x) mx = fmaxf(mx, pval[p0 + i]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if (lane_id() == 0) s_v[warp] = mx;
+  __syncthreads();
+  mx = s_v[0];
+  for (int w = 1; w < nwarp; ++w) mx = fmaxf(mx, s_v[w]);
+  float ssum = 0.f;
+  for (int i = threadIdx.x; i < n_tiles; i += blockDim.x) ssum += psum[p0 + i] * expf(pval[p0 + i] - mx);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) ssum += __shfl_xor_sync(0xffffffffu, ssum, o);
+  if (lane_id() == 0) s_s[warp] = ssum;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < nwarp; ++w) ssum += s_s[w];
+    logprob[blockIdx.x] = ftok[blockIdx.x] < 0 ? 0.f : fval[blockIdx.x] - (mx + logf(ssum));
   }
 }
 

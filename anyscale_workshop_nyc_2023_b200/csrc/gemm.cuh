@@ -462,6 +462,7 @@ DEVINL float gelu_epilogue(float x, const uint16_t* lut, int lo, int hi) {
 
 // ---- GeGLU: tile columns [0,BN/2) are wi_0 (gate) features, [BN/2,BN) the matching
 // wi_1 features (weights are interleaved per tile at finalize).
+// EpiGegluNarrow below repeats this arithmetic for the forward pass: a change to the rounding here belongs there too.
 //   out = bf16( gelu_new(bf16(gate)) * bf16(up) )          (modeling_t5.py:115-118)
 struct EpiGeglu {
   struct Params {
@@ -525,6 +526,63 @@ struct EpiGeglu {
       acc_ld_32(taddr + HALF + c * 32, u);
       const int f0 = n_tile * HALF + c * 32;
       if (m_ok && f0 < p.F) chunk2(p, g, u, m, f0, epi_smem);
+    }
+  }
+};
+
+// ---- GeGLU of the teacher-forced forward pass (b200t5_forward): EpiGeglu's arithmetic and rounding, element for
+// element, on the decode step's `wi` packing read in 128-wide tiles, eight features at a time instead of 32. The fp16
+// build evaluates gelu_new op by op, and 32 gate + 32 up + 32 outputs per thread spill under this kernel's register
+// budget; eight at a time do not.
+struct EpiGegluNarrow {
+  using Params = EpiGeglu::Params;
+  static DEVINL void prologue(const Params& p, uint8_t* epi_smem, int tid, int nthreads = 128) {
+    EpiGeglu::prologue(p, epi_smem, tid, nthreads);
+  }
+  template <int BN>
+  static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int /*N*/, const uint8_t* epi_smem,
+                         int part, int parts) {
+    constexpr int HALF = BN / 2;
+    constexpr int C = HALF / 8;
+#pragma unroll 1
+    for (int c = part * C / parts; c < (part + 1) * C / parts; ++c) {
+      const int f0 = n_tile * HALF + c * 8;
+      if (!m_ok || f0 >= p.F) continue;  // F is a multiple of 32: a group of 8 is whole or absent
+      uint32_t g[8], u[8];
+#pragma unroll
+      for (int v = 0; v < 2; ++v) {
+        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(g[4 * v]), "=r"(g[4 * v + 1]), "=r"(g[4 * v + 2]), "=r"(g[4 * v + 3])
+                     : "r"((taddr + c * 8 + 4u * v) << 2) : "memory");
+        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(u[4 * v]), "=r"(u[4 * v + 1]), "=r"(u[4 * v + 2]), "=r"(u[4 * v + 3])
+                     : "r"((taddr + HALF + c * 8 + 4u * v) << 2) : "memory");
+      }
+#if B200T5_F16
+      float o[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float x = act_round(__uint_as_float(g[i]));
+        const float lin = act_round(__uint_as_float(u[i]));
+        o[i] = act_round(gelu_epilogue(x, nullptr, 0, 0) * lin);
+      }
+      float4* dst = reinterpret_cast<float4*>(p.out + static_cast<size_t>(m) * p.F + f0);
+      dst[0] = make_float4(o[0], o[1], o[2], o[3]);
+      dst[1] = make_float4(o[4], o[5], o[6], o[7]);
+#else
+      const uint16_t* lut = reinterpret_cast<const uint16_t*>(epi_smem);
+      uint32_t o[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        float r[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float x = act_round(__uint_as_float(g[2 * i + e]));
+          const float lin = act_round(__uint_as_float(u[2 * i + e]));
+          r[e] = gelu_epilogue(x, lut, p.lut.lo, p.lut.hi) * lin;
+        }
+        o[i] = pack_act2(r[0], r[1]);
+      }
+      *reinterpret_cast<uint4*>(p.out + static_cast<size_t>(m) * p.F + f0) = make_uint4(o[0], o[1], o[2], o[3]);
+#endif
     }
   }
 };
@@ -738,6 +796,39 @@ struct EpiLmHead {
       p.pidx[static_cast<size_t>(m) * p.n_tiles + n_tile] = bidx;
       if constexpr (kScore) p.psum[static_cast<size_t>(m) * p.n_tiles + n_tile] = sum;
     }
+  }
+};
+
+// ---- lm_head of the teacher-forced forward pass with logits requested: C [M, ldc] = act(acc), in the build's 2-byte
+// type (HF's logits dtype; the act-rounded values are exact in it), and with kLabels also EpiLmHead<false, true>'s
+// partials of the same values for the label columns lm.ftok.
+template <bool kLabels>
+struct EpiLmLogits {
+  struct Params {
+    LmHeadParams lm;
+    act_t* C;
+    size_t ldc;
+  };
+  static DEVINL void prologue(const Params&, uint8_t*, int, int = 128) {}
+  template <int BN>
+  static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t* es, int part, int parts) {
+#pragma unroll 1
+    for (int c = part * (BN / 32) / parts; c < (part + 1) * (BN / 32) / parts; ++c) {
+      uint32_t acc[32];
+      acc_ld_32(taddr + c * 32, acc);
+      const int n0 = n_tile * BN + c * 32;
+      if (m_ok && n0 < N) {
+        act_t* dst = p.C + static_cast<size_t>(m) * p.ldc + n0;
+        if (n0 + 32 <= N && p.ldc % 8 == 0) {
+          uint32_t o[16];
+          round_pack_32(acc, o);
+          store_row_chunk(dst, o, n0, N);
+        } else {
+          for (int j = 0; j < 32 && n0 + j < N; ++j) dst[j] = float2act(__uint_as_float(acc[j]));
+        }
+      }
+    }
+    if constexpr (kLabels) EpiLmHead<false, true>::template run<BN>(p.lm, taddr, m, m_ok, n_tile, N, es, part, parts);
   }
 };
 

@@ -207,6 +207,18 @@ class GenerateOutput:
         return getattr(self, key)
 
 
+class ForwardOutput:
+    """`forward(...)` / `model(...)`: `.loss`, `.logits` and `.token_logprobs` (see forward), also readable by key."""
+
+    def __init__(self, loss=None, logits=None, token_logprobs=None):
+        self.loss = loss
+        self.logits = logits
+        self.token_logprobs = token_logprobs
+
+    def __getitem__(self, key):
+        return getattr(self, key)
+
+
 class BeamGenerateOutput(GenerateOutput):
     """`generate(num_beams=k, return_dict_in_generate=True)`: `.sequences` [B*n, 1+T'] as a plain call returns,
     `.sequences_scores` fp32 [B*n] (the length-penalised scores), `.beam_indices` int64 [B*n, T'] (transformers' b*k + beam
@@ -526,6 +538,63 @@ class B200T5ForConditionalGeneration:
         _, lens, logp, _ = self._run_scored(host, attention_mask, gp, None, lab)
         count = int((lab != -100).sum())
         return SimpleNamespace(token_logprobs=logp, lengths=lens, loss=-(logp.double().sum() / count).float())
+
+    _FORWARD_UNSUPPORTED = ("decoder_attention_mask", "encoder_outputs", "past_key_values", "inputs_embeds",
+                            "decoder_inputs_embeds", "head_mask", "decoder_head_mask", "cross_attn_head_mask",
+                            "output_attentions", "output_hidden_states")
+
+    @torch.no_grad()
+    def forward(self, input_ids, attention_mask=None, decoder_input_ids=None, labels=None, return_logits: bool = True, **kw):
+        """`T5ForConditionalGeneration(input_ids, attention_mask, decoder_input_ids=..., labels=...)`: the teacher-forced
+        forward pass, with the decoder run over all T positions at once (b200t5_forward). Without decoder_input_ids they
+        are transformers' `_shift_right(labels)`. Labels may hold -100 anywhere (ignored positions). Returns a
+        ForwardOutput: `.loss` fp32 scalar = -sum / count over the labels != -100 (NaN when there is none; None without
+        labels), `.logits` [B, T, vocab] in the model's dtype (None with return_logits=False), `.token_logprobs` fp32
+        [B, T] (0 at ignored positions; None without labels). Batches of more than pool_size prompts run in chunks; a
+        row's results do not depend on its batch or chunk."""
+        for k in self._FORWARD_UNSUPPORTED:
+            if kw.get(k) is not None and kw.get(k) is not False:
+                raise NotImplementedError(f"forward({k}=...) is not supported by the CUDA path")
+        kw.pop("use_cache", None)
+        kw.pop("return_dict", None)
+        unknown = [k for k in kw if k not in self._FORWARD_UNSUPPORTED]
+        if unknown:
+            raise TypeError(f"forward() got unexpected keyword arguments {unknown}")
+        if labels is None and decoder_input_ids is None:
+            raise ValueError("You have to specify either decoder_input_ids or labels")
+        ids = torch.as_tensor(input_ids).to(self._device, torch.long).contiguous()
+        if ids.dim() != 2:
+            raise ValueError(f"input_ids must be [batch, seq], got {tuple(ids.shape)}")
+        B = ids.shape[0]
+        mask = None if attention_mask is None else torch.as_tensor(attention_mask).to(self._device, torch.long).contiguous()
+        self._check_inputs(ids, mask)
+        lab = None if labels is None else torch.as_tensor(labels).to(self._device, torch.long).contiguous()
+        dec = None if decoder_input_ids is None else torch.as_tensor(decoder_input_ids).to(self._device, torch.long).contiguous()
+        T = (lab if lab is not None else dec).shape[1]
+        for name, t in (("labels", lab), ("decoder_input_ids", dec)):
+            if t is not None and (t.dim() != 2 or t.shape[0] != B or t.shape[1] != T):
+                raise ValueError(f"{name} must be [batch={B}, {T}], got {tuple(t.shape)}")
+        if not return_logits and lab is None:
+            raise ValueError("forward(return_logits=False) needs labels")
+        logits = torch.empty((B, T, self.config.vocab_size), dtype=self._dtype, device=self._device) if return_logits else None
+        logp = torch.empty((B, T), dtype=torch.float32, device=self._device) if lab is not None else None
+        with torch.cuda.device(self._index):
+            stream = torch.cuda.current_stream(self._device)
+            for lo in range(0, B, self.pool_size):
+                hi = min(B, lo + self.pool_size)
+                io = _lib.ForwardIO(logits=None if logits is None else logits[lo:hi].data_ptr(),
+                                    token_logprobs=None if logp is None else logp[lo:hi].data_ptr())
+                _chk(self, self._lib.b200t5_forward(self._h, _ptr(ids[lo:hi]), _ptr(None if mask is None else mask[lo:hi]), hi - lo,
+                                                    ids.shape[1], _ptr(None if dec is None else dec[lo:hi]),
+                                                    _ptr(None if lab is None else lab[lo:hi]), T, C.byref(io),
+                                                    C.c_void_p(stream.cuda_stream)), self._h)
+        loss = None
+        if lab is not None:
+            count = int((lab != -100).sum())
+            loss = (-(logp.double().sum() / count)).float() if count else torch.tensor(float("nan"), device=self._device)
+        return ForwardOutput(loss=loss, logits=logits, token_logprobs=logp)
+
+    __call__ = forward
 
     def _run_scored(self, host: torch.Tensor, attention_mask, gp, lp, labels: Optional[np.ndarray]):
         """generate's routing (static batch, slot pool, static chunks) for a scored call: (sequences [B, 1+T'],

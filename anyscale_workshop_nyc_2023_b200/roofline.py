@@ -56,6 +56,19 @@ def encoder_flops(spec, batch: int, extents: Optional[Iterable[int]] = None, seq
             + 2.0 * spec.num_decoder_layers * 2.0 * d * inner * sum_s)
 
 
+def decoder_forward_flops(spec, batch: int, T: int, extents: Optional[Iterable[int]] = None, seq: Optional[int] = None) -> float:
+    """The teacher-forced forward pass's decoder + lm_head FLOPs (b200t5_forward), T label positions per row: per layer
+    and position the QKV, output, cross-query, cross-output and GeGLU products (2 (6 d I + 3 d F)); causal self-attention
+    Q.K and P.V over the keys j <= i (4 I (i + 1)); cross-attention over the row's extent (4 I S_b); the lm_head
+    (2 d V per position). The encoder and the cross-K/V projection are encoder_flops."""
+    ext = list(extents) if extents is not None else [seq] * batch
+    d, inner, f, ld = spec.d_model, spec.inner_dim, spec.d_ff, spec.num_decoder_layers
+    rows = float(batch) * T
+    gemm = rows * (ld * 2.0 * (6 * d * inner + 3 * d * f) + 2.0 * d * spec.vocab_size)
+    attn = ld * (batch * 2.0 * inner * T * (T + 1) + 4.0 * inner * T * float(sum(ext)))
+    return gemm + attn
+
+
 def cross_attention_bytes_per_launch(spec, extents: Iterable[int]) -> float:
     """One launch of the roofline kernel: K and V rows (64 x 2 bytes per head) of every attended key."""
     return 2.0 * 2.0 * spec.inner_dim * float(sum(extents))

@@ -238,6 +238,24 @@ int b200t5_generate_host_beam(b200t5_handle h, const int64_t* input_ids, const i
 /* Bytes the self-attention cache reordering of the last beam call read and wrote (beam_reorder_kernel), and its steps. */
 int b200t5_get_beam_stats(b200t5_handle h, double* reorder_bytes, int32_t* steps);
 
+/* Teacher-forced forward pass (T5ForConditionalGeneration.forward with labels / decoder_input_ids, no cache): the encoder,
+ * then the decoder over all T positions of every row at once - causal self-attention, cross-attention, feed-forward as
+ * GEMMs over B*T rows - and the lm_head. Every product and attention keeps the rounding points of the decode step, so
+ * the results agree with b200t5_decode_logits / the scored entry points within rounding, not bit for bit.
+ * All pointers are device pointers; enqueued on `stream` like b200t5_generate (labels and decoder ids are read back to be
+ * checked). input_ids / attention_mask as b200t5_generate. decoder_input_ids int64 [B,T], may be NULL when labels are
+ * given: then transformers' _shift_right(labels) (the decoder start token, then labels[:, :-1] with -100 replaced by
+ * the pad id). labels int64 [B,T], may be NULL: ids in [0, vocab_size) or -100 (ignored) anywhere in a row.
+ * A row's results do not depend on the batch it sits in. Both inputs NULL, both outputs NULL, token_logprobs without
+ * labels, ids out of range or T outside [1, 4096] return B200T5_EINVAL. */
+typedef struct b200t5_forward_io {
+  void* logits;           /* out, may be NULL: [B, T, vocab] in the build's 2-byte type */
+  float* token_logprobs;  /* out, may be NULL: [B, T] log p(labels[b][t]); 0 where labels is -100; needs labels */
+} b200t5_forward_io;
+int b200t5_forward(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                   const int64_t* decoder_input_ids, const int64_t* labels, int T, const b200t5_forward_io* io,
+                   void* stream);
+
 /* ---- measurement hooks (bench.py) --------------------------------------------------- */
 /* Times the cross-attention decode kernel alone over the cross-KV arena of the last generate call, in launches of
  * `rows_per_launch` batch rows (0 = the whole batch; the step graph launches one row-chain at a time): reps sweeps
@@ -370,6 +388,14 @@ int b200t5_test_attn_decode(int device, int self, const void* q, const void* K, 
  * cu[b] = b * S), where query rows >= extent[b] are not written. */
 int b200t5_test_encoder_attn(int device, const void* qkv, void* ctx, const float* rel_bias, const uint8_t* key_ok,
                              const int32_t* extent, int B, int S, int H, int impl, void* stream);
+/* The decoder attentions of b200t5_forward (csrc/attention_decoder.cuh: decoder_attn_kernel), with the encoder attention's
+ * rounding points. Self: qkv [B*T, 3*H*64] (q | k | v), causal, dist_bias float [H][T] indexed by i - j; T <= 4096.
+ * Cross: q [B*T, H*64], kv [2][B][H][S][64] (one layer of the cross-K/V arena), keys masked by key_ok uint8 [B][S] and
+ * extent int32 [B] (prep_mask's: a row without an attended key has extent S and attends uniformly). ctx [B*T, H*64]. */
+int b200t5_test_decoder_self_attn(int device, const void* qkv, void* ctx, const float* dist_bias, int B, int T, int H,
+                                  void* stream);
+int b200t5_test_decoder_cross_attn(int device, const void* q, const void* kv, void* ctx, const uint8_t* key_ok,
+                                   const int32_t* extent, int B, int T, int S, int H, void* stream);
 /* out[i] = act(gelu_new(gate[i]) * up[i]). mode 0: exactly the GeGLU epilogue's function (bf16 build: the exhaustive
  * gelu table; fp16 build: the op-by-op fp16 arithmetic with single-rounded pow); mode 2: the op-by-op arithmetic with
  * double-rounded pow (x*x*x in act_t); mode 1: same with single-rounded pow. */
