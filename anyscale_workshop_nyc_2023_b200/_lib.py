@@ -142,6 +142,10 @@ SIGNATURES = {
                                          C.POINTER(ScoreIO)]),
     "b200t5_generate_stream_scored": (_i, [_vp, _i64p, _i64p, C.c_int64, _i, C.POINTER(GenParams), C.POINTER(LogitsParams), _i, _i,
                                            _i64p, _i32p, C.POINTER(ScoreIO)]),
+    "b200t5_generate_prefixed": (_i, [_vp, _i64p, _i64p, _i, _i, C.POINTER(GenParams), C.POINTER(LogitsParams), _i64p, _i32p,
+                                      C.POINTER(ScoreIO), _i64p, _i, _vp]),
+    "b200t5_generate_host_prefixed": (_i, [_vp, _i64p, _i64p, _i, _i, C.POINTER(GenParams), C.POINTER(LogitsParams), _i64p,
+                                           _i32p, C.POINTER(ScoreIO), _i64p, _i]),
     "b200t5_generate_beam": (_i, [_vp, _i64p, _i64p, _i, _i, C.POINTER(GenParams), C.POINTER(BeamParams), C.POINTER(BeamIO), _vp]),
     "b200t5_generate_host_beam": (_i, [_vp, _i64p, _i64p, _i, _i, C.POINTER(GenParams), C.POINTER(BeamParams), C.POINTER(BeamIO)]),
     "b200t5_get_beam_stats": (_i, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_int32)]),
@@ -162,6 +166,7 @@ SIGNATURES = {
                                   _vp, _vp, _vp, _vp]),
     "b200t5_encode": (_i, [_vp, _i64p, _i64p, _i, _i, _vp, _vp]),
     "b200t5_decode_logits": (_i, [_vp, _i64p, _i64p, _i, _i, _i64p, _i, _vp, _vp]),
+    "b200t5_test_prefill_cache": (_i, [_vp, _i, _vp, _vp]),
     "b200t5_forward": (_i, [_vp, _i64p, _i64p, _i, _i, _i64p, _i64p, _i, C.POINTER(ForwardIO), _vp]),
     "b200t5_relative_bucket": (_i, [_i, _i, _i, _i]),
     "b200t5_test_gemm": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),

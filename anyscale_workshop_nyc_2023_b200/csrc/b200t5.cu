@@ -345,6 +345,10 @@ struct Plan {
   // int32 [B*T] and a zero step; the causal bias float [H][fwd_T]; the lm_head partials when they do not fit in hff
   DevBuf fwd_ids, fwd_bias, fwd_part;
   int fwd_T = 0;
+  // a call with a decoder prompt (b200t5_generate_prefixed): the prefill's ids int64 [B*(P-1)], then the prompt [B*P];
+  // prompt_steps = P - 1 of the last such call (0 for any other call)
+  DevBuf pre_ids;
+  int prompt_steps = 0;
   StepMode mode;                 // what this call's steps run
   std::optional<StepMode> graph_mode;  // what the step graphs were captured for (none: re-capture)
   // after a reallocation of a buffer the step graph bakes: the next ensure_graph re-captures
@@ -1120,11 +1124,13 @@ static int build_plan(b200t5_ctx* h, int B, int S, int Tmax, int group, int ws_S
   return B200T5_OK;
 }
 
-static int ensure_plan(b200t5_ctx* h, int B, int S, int Tmax, int group = 1) {
-  if (h->plan && h->plan->B == B && h->plan->S == S && h->plan->Tmax == Tmax && h->plan->group == group) return B200T5_OK;
+// `ws`: rows per prompt the encoder workspace must hold besides S (a decoder prompt's prefill runs P - 1 rows per prompt)
+static int ensure_plan(b200t5_ctx* h, int B, int S, int Tmax, int group = 1, int ws = 0) {
+  if (h->plan && h->plan->B == B && h->plan->S == S && h->plan->Tmax == Tmax && h->plan->group == group && h->plan->ws_S >= ws)
+    return B200T5_OK;
   CU_OK(h, cudaDeviceSynchronize());
   h->plan.reset();
-  return build_plan(h, B, S, Tmax, group, S);
+  return build_plan(h, B, S, Tmax, group, std::max(S, ws));
 }
 
 // ================================================================== encoder
@@ -1664,14 +1670,17 @@ static void fill_stats_model(b200t5_ctx* h, int steps) {
 struct CallArgs {
   long long eos = 0, pad = 0, start = 0;
   int T = 0, min_new = 0;
+  int first = 0;  // the first generated position: P - 1 after a decoder prompt of P ids, else 0
   ProcHost ph;
   ScoreHost sh;
-  // The step mode of this call. A beam call's min_new_tokens lives in its BeamParams, not in the graph.
+  // The step mode of this call. A beam call's min_new_tokens lives in its BeamParams, not in the graph. The EOS mask
+  // runs while step < first + min_new: after a decoder prompt the offset is baked into the graph, so a call with
+  // another prompt length (and min_new_tokens > 0) re-captures it.
   StepMode mode(bool pool, int beam = 0) const {
     StepMode m;
     m.eos = eos;
     m.pad = pad;
-    m.min_new = beam ? 0 : min_new;
+    m.min_new = beam ? 0 : (min_new > 0 ? first + min_new : 0);
     m.pool = pool;
     m.proc = ph.on;
     m.score = sh.on ? (sh.forced.empty() ? 1 : 2) : 0;
@@ -1701,14 +1710,20 @@ static int set_up_call(b200t5_ctx* h, int B, int S, long long rows, const b200t5
 }
 
 // Queues the copy of the first n rows of the call's results (p.res()) to ids / len and, for a scored call, to lp / lg
-// (lg may be NULL).
-static int copy_results(b200t5_ctx* h, size_t n, void* ids, void* len, void* lp, void* lg, cudaMemcpyKind kind, cudaStream_t s) {
+// (lg may be NULL). `col0`: the scores start at column col0 of the plan's [rows][Tmax] arrays (a decoder prompt's
+// first generated position) and are copied as [n][Tmax - col0].
+static int copy_results(b200t5_ctx* h, size_t n, void* ids, void* len, void* lp, void* lg, cudaMemcpyKind kind, cudaStream_t s,
+                        int col0 = 0) {
   Plan& p = *h->plan;
   const Plan::Results& r = p.res();
   const size_t T = static_cast<size_t>(p.Tmax);
   CU_OK(h, cudaMemcpyAsync(ids, r.ids.p, n * (T + 1) * 8, kind, s));
   CU_OK(h, cudaMemcpyAsync(len, r.len.p, n * 4, kind, s));
-  if (p.mode.score) {
+  if (p.mode.score && col0 > 0) {
+    const size_t w = (T - col0) * 4;
+    CU_OK(h, cudaMemcpy2DAsync(lp, w, r.lp.as<float>() + col0, T * 4, w, n, kind, s));
+    if (lg) CU_OK(h, cudaMemcpy2DAsync(lg, w, r.lg.as<float>() + col0, T * 4, w, n, kind, s));
+  } else if (p.mode.score) {
     CU_OK(h, cudaMemcpyAsync(lp, r.lp.p, n * T * 4, kind, s));
     if (lg) CU_OK(h, cudaMemcpyAsync(lg, r.lg.p, n * T * 4, kind, s));
   }
@@ -1716,12 +1731,19 @@ static int copy_results(b200t5_ctx* h, size_t n, void* ids, void* len, void* lp,
 }
 
 // The start of a static batch's decoding, after its encoder pass: the decode kernels attend to live copies of extent /
-// key_ok, and every row starts from the start token.
-static int begin_static_decode(b200t5_ctx* h, const CallArgs& a, cudaStream_t s) {
+// key_ok, and every row starts from the start token (`prompt`: from the decoder prompt [B][P] on the device).
+static int begin_static_decode(b200t5_ctx* h, const CallArgs& a, cudaStream_t s, const long long* prompt = nullptr, int P = 1) {
   Plan& p = *h->plan;
   const int B = p.B;
   CU_OK(h, cudaMemcpyAsync(p.live_extent.p, p.extent.p, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToDevice, s));
   CU_OK(h, cudaMemcpyAsync(p.live_key_ok.p, p.key_ok.p, static_cast<size_t>(B) * p.S, cudaMemcpyDeviceToDevice, s));
+  if (prompt) {
+    decode_init_prompt_kernel<<<B, 128, 0, s>>>(p.state.as<DecodeState>(), p.unfinished.as<int>(), p.batch.ids.as<long long>(),
+                                                p.batch.len.as<int>(), p.Tmax + 1, B, prompt, P, a.pad, h->shared.as<act_t>(),
+                                                p.dx.as<res_t>(), h->c.d);
+    h->launches++;
+    return B200T5_OK;
+  }
   decode_init_kernel<<<B, 128, 0, s>>>(p.state.as<DecodeState>(), p.unfinished.as<int>(), p.batch.ids.as<long long>(),
                                        p.batch.len.as<int>(), a.T + 1, B, a.start, a.pad, h->shared.as<act_t>(), p.dx.as<res_t>(),
                                        h->c.d);
@@ -2408,7 +2430,9 @@ static cudaError_t run_geglu_fwd(b200t5_ctx* h, const CUtensorMap& tmA, const De
 // decoder ids to xn = the final RMSNorm, in the plan's encoder workspace; the epilogue flags of each product are the
 // decode step's (chain_layer_pre / chain_layer_post). The products run the encoder's 128 x 256 GEMMs through the
 // layer's 128-row-box tensor maps, except GeGLU (run_geglu_fwd).
-static int run_decoder_forward(b200t5_ctx* h, int T, cudaStream_t s) {
+// `prefill` (a decoder prompt's positions 0 .. T-1): each layer's K/V also go to cache positions 0 .. T-1
+// (prefill_cache_kernel), and the pass ends at the last layer's K/V: nothing reads the prompt positions' outputs.
+static int run_decoder_forward(b200t5_ctx* h, int T, cudaStream_t s, bool prefill = false) {
   const Cfg& c = h->c;
   Plan& p = *h->plan;
   const int B = p.B, S = p.S, d = c.d, I = c.I, F = c.F, H = c.H, M = B * T;
@@ -2421,6 +2445,12 @@ static int run_decoder_forward(b200t5_ctx* h, int T, cudaStream_t s) {
     DecLayerW& w = h->dec[l];
     CU_OK(h, run_rmsnorm(h, x, w.ln0.as<act_t>(), xn, M, d, c.eps, s));
     CU_OK(h, run_gemm_2cta<EpiStore>(h, p.tm_xn, w.tm2_qkv, M, 3 * I, d, EpiStore::Params{qkv, 3 * I}, s));
+    if (prefill) {
+      prefill_cache_kernel<<<M, 128, 0, s>>>(qkv, p.self_kv.as<act_t>() + static_cast<size_t>(l) * 2 * B * I * p.Tmax, T, B, H, p.Tmax);
+      h->launches++;
+      CU_OK(h, cudaGetLastError());
+      if (l == c.Ld - 1) return B200T5_OK;
+    }
     decoder_attn_kernel<kAttnCausal><<<agrid, kEncThreads, encoder_attn_smem_bytes(T), s>>>(
         qkv, nullptr, ctx, p.fwd_bias.as<float>(), nullptr, nullptr, B, T, T, H);
     h->launches++;
@@ -2455,6 +2485,32 @@ static int run_decoder_forward(b200t5_ctx* h, int T, cudaStream_t s) {
   return B200T5_OK;
 }
 
+// run_decoder_forward's GeGLU product (run_geglu_fwd) reads wi in the decode step's packing through 128-row boxes: it
+// needs the default 128-row wi tile of the split-K decode GEMM. Checked before anything is launched.
+static int check_forward_wi(b200t5_ctx* h, const char* who) {
+  if (h->sk_wi.bn != 128)
+    return fail(h, B200T5_EINVAL, "%s: needs the feed-forward wi packed in 128-row tiles, but B200T5_SK set the wi tile to %d rows "
+                "(unset B200T5_SK or give wi a bn of 128)", who, h->sk_wi.bn);
+  return B200T5_OK;
+}
+
+// The forward pass's causal bias for T positions: dec_relbias by distance i - j, float [H][T], as the decode step's
+// dec_bias (kept while T stays the same).
+static int ensure_fwd_bias(b200t5_ctx* h, int T) {
+  const Cfg& c = h->c;
+  Plan& p = *h->plan;
+  if (p.fwd_T == T) return B200T5_OK;
+  std::vector<float> db(static_cast<size_t>(c.H) * T);
+  for (int n = 0; n < T; ++n) {
+    const int bk = b200t5_relative_bucket(-n, 0, c.nb, c.maxdist);
+    for (int hh = 0; hh < c.H; ++hh) db[static_cast<size_t>(hh) * T + n] = h->dec_relbias_h[static_cast<size_t>(bk) * c.H + hh];
+  }
+  CU_OK(h, p.fwd_bias.alloc(db.size() * 4));
+  CU_OK(h, cudaMemcpy(p.fwd_bias.p, db.data(), db.size() * 4, cudaMemcpyHostToDevice));
+  p.fwd_T = T;
+  return B200T5_OK;
+}
+
 extern "C" int b200t5_forward(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
                               const int64_t* decoder_input_ids, const int64_t* labels, int T, const b200t5_forward_io* io,
                               void* stream) {
@@ -2464,9 +2520,7 @@ extern "C" int b200t5_forward(b200t5_handle h, const int64_t* input_ids, const i
   if (!io->logits && !io->token_logprobs) return fail(h, B200T5_EINVAL, "forward: neither logits nor token_logprobs requested");
   if (io->token_logprobs && !labels) return fail(h, B200T5_EINVAL, "forward: token_logprobs needs labels");
   if (T < 1 || T > 4096) return fail(h, B200T5_EINVAL, "forward: T=%d outside [1, 4096]", T);
-  if (h->sk_wi.bn != 128)
-    return fail(h, B200T5_EINVAL, "forward: needs the feed-forward wi packed in 128-row tiles, but B200T5_SK set the wi tile to %d rows "
-                "(unset B200T5_SK or give wi a bn of 128)", h->sk_wi.bn);
+  TRY(check_forward_wi(h, "forward"));
   CU_OK(h, cudaSetDevice(h->device));
   const Cfg& c = h->c;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -2517,17 +2571,7 @@ extern "C" int b200t5_forward(b200t5_handle h, const int64_t* input_ids, const i
   for (size_t m = 0; m < M && labels; ++m) ftok[m] = lab[m] == -100 ? -1 : static_cast<int>(lab[m]);
   CU_OK(h, cudaMemcpyAsync(ids_dev, dec.data(), M * 8, cudaMemcpyHostToDevice, s));
   CU_OK(h, cudaMemcpyAsync(ftok_dev, ftok.data(), (M + 4) * 4, cudaMemcpyHostToDevice, s));
-  if (p.fwd_T != T) {
-    // dec_relbias by distance i - j, as the decode step's dec_bias
-    std::vector<float> db(static_cast<size_t>(c.H) * T);
-    for (int n = 0; n < T; ++n) {
-      const int bk = b200t5_relative_bucket(-n, 0, c.nb, c.maxdist);
-      for (int hh = 0; hh < c.H; ++hh) db[static_cast<size_t>(hh) * T + n] = h->dec_relbias_h[static_cast<size_t>(bk) * c.H + hh];
-    }
-    CU_OK(h, p.fwd_bias.alloc(db.size() * 4));
-    CU_OK(h, cudaMemcpy(p.fwd_bias.p, db.data(), db.size() * 4, cudaMemcpyHostToDevice));
-    p.fwd_T = T;
-  }
+  TRY(ensure_fwd_bias(h, T));
   // lm_head partials [M][n_tiles] x 3 + fval [M]: in hff (free after the last feed-forward block) when they fit
   const bool lp_on = io->token_logprobs != nullptr;
   const size_t part_bytes = lp_on ? M * (static_cast<size_t>(3) * nt + 1) * 4 : 0;
@@ -2572,6 +2616,153 @@ extern "C" int b200t5_forward(b200t5_handle h, const int64_t* input_ids, const i
   CU_OK(h, cudaEventRecord(h->ev[2], s));
   h->last_steps = 0;
   h->ev_valid = true;
+  return B200T5_OK;
+}
+
+// ================================================================== decoder prompt
+// generate(decoder_input_ids=d): a static batch whose decoding starts after a decoder prompt d [B][P] (start token
+// included). The prompt's positions 0 .. P-2 run as one forward pass over B*(P-1) rows (run_decoder_forward with the
+// cache sink), which leaves their K/V in the self-attention cache; then the step loop starts at t = P-1 with input
+// d[P-1] (decode_init_prompt_kernel). Everything the steps index by position (cache, bias, result columns, score
+// columns) is absolute, so the plan's Tmax is P-1 + max_new_tokens and the steps themselves are unchanged.
+
+// The checks of a prefixed call and its prompt, host int64 [B][P] (checked and staged on the host: no stream sync).
+static int read_prompt(b200t5_ctx* h, const int64_t* decoder_input_ids, int B, int P, const b200t5_gen_params* gp,
+                       const b200t5_score_io* score, std::vector<long long>* d) {
+  if (!decoder_input_ids) return fail(h, B200T5_EINVAL, "prefixed: decoder_input_ids is NULL");
+  if (P < 1) return fail(h, B200T5_EINVAL, "prefixed: decoder prompt length P=%d < 1", P);
+  if (P >= 2) TRY(check_forward_wi(h, "prefixed"));  // the prefill is run_decoder_forward
+  if (gp && static_cast<long long>(P) - 1 + gp->max_new_tokens > 4096)
+    return fail(h, B200T5_EINVAL, "prefixed: P-1 + max_new_tokens = %lld exceeds 4096", static_cast<long long>(P) - 1 + gp->max_new_tokens);
+  if (score && score->forced_ids) return fail(h, B200T5_EINVAL, "prefixed: forced_ids cannot be combined with a decoder prompt");
+  d->assign(decoder_input_ids, decoder_input_ids + static_cast<size_t>(B) * P);
+  for (long long v : *d)
+    if (v < 0 || v >= h->c.V) return fail(h, B200T5_EINVAL, "prefixed: decoder id %lld outside [0, %d)", v, h->c.V);
+  return B200T5_OK;
+}
+
+// A prompt of one id shared by every row is the start token of an ordinary call.
+static bool one_start(const std::vector<long long>& d, int P) {
+  return P == 1 && std::all_of(d.begin(), d.end(), [&](long long v) { return v == d[0]; });
+}
+
+// A static batch of B rows after the decoder prompt d [B][P] (P > 1, or rows that start from different ids); its
+// results stay in the plan's buffers (copy_results with col0 = P - 1).
+static int generate_prefixed_impl(b200t5_ctx* h, const long long* ids, const long long* mask, int B, int S, const b200t5_gen_params* gp,
+                                  CallArgs& a, const std::vector<long long>& d, int P, cudaStream_t s) {
+  const Cfg& c = h->c;
+  const int T = a.T, Tp = P - 1;
+  TRY(ensure_plan(h, B, S, Tp + T, 1, Tp));
+  Plan& p = *h->plan;
+  a.first = Tp;
+  a.ph.cfg.begin_t = Tp;
+  p.mode = a.mode(false);
+  TRY(setup_proc(h, a.ph, s));
+  TRY(setup_score(h, a.sh, s));
+  if (Tp > 0) TRY(ensure_fwd_bias(h, Tp));
+  // the prefill's ids [B][Tp] (columns 0 .. P-2), then the prompt [B][P]
+  std::vector<long long> staged(static_cast<size_t>(B) * (Tp + P));
+  for (int b = 0; b < B; ++b)
+    for (int t = 0; t < Tp; ++t) staged[static_cast<size_t>(b) * Tp + t] = d[static_cast<size_t>(b) * P + t];
+  std::copy(d.begin(), d.end(), staged.begin() + static_cast<size_t>(B) * Tp);
+  if (p.pre_ids.bytes < staged.size() * 8) CU_OK(h, p.pre_ids.alloc(staged.size() * 8));
+  CU_OK(h, cudaMemcpyAsync(p.pre_ids.p, staged.data(), staged.size() * 8, cudaMemcpyHostToDevice, s));
+  const long long* prompt = p.pre_ids.as<long long>() + static_cast<size_t>(B) * Tp;
+  p.prompt_steps = Tp;
+  h->launches = 0;
+  CU_OK(h, cudaEventRecord(h->ev[0], s));
+  TRY(run_encoder(h, ids, mask, s));
+  TRY(run_cross_kv(h, s));
+  TRY(ensure_graph(h, static_cast<double>(p.rows_valid) / (static_cast<double>(B) * S)));
+  if (Tp > 0) {
+    const int M = B * Tp;
+    embed_rows_kernel<<<(M + 7) / 8, 256, 0, s>>>(p.pre_ids.as<long long>(), h->shared.as<act_t>(), p.x.as<res_t>(), M, c.d, c.V);
+    h->launches++;
+    TRY(run_decoder_forward(h, Tp, s, true));
+  }
+  TRY(begin_static_decode(h, a, s, prompt, P));
+  if (p.mode.proc) {
+    proc_reset_kernel<<<B, 128, 0, s>>>(p.proc.dev(), nullptr, ids, p.batch.ids.as<long long>(), p.Tmax + 1, nullptr, P);
+    h->launches++;
+  }
+  if (p.mode.score) {
+    score_reset_kernel<<<B, 128, 0, s>>>(p.batch.lp.as<float>(), p.batch.lg.as<float>(), static_cast<size_t>(B) * p.Tmax, p.ftok.as<int>(),
+                                         B, nullptr, nullptr, nullptr, p.Tmax);
+    h->launches++;
+  }
+  TRY(run_static_steps(h, gp, T, a.min_new < T, s));
+  if (Tp > 0) {
+    prompt_len_kernel<<<(B + 127) / 128, 128, 0, s>>>(p.batch.len.as<int>(), B, Tp);
+    h->launches++;
+    CU_OK(h, cudaGetLastError());
+  }
+  return B200T5_OK;
+}
+
+extern "C" int b200t5_generate_prefixed(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                                        const b200t5_gen_params* params, const b200t5_logits_params* logits, int64_t* out_ids,
+                                        int32_t* out_len, const b200t5_score_io* score, const int64_t* decoder_input_ids, int P,
+                                        void* stream) {
+  CallArgs a;
+  TRY(set_up_call(h, B, S, B, params, input_ids, out_ids, out_len, logits, score, false, &a));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  std::vector<long long> d;
+  TRY(read_prompt(h, decoder_input_ids, B, P, params, score, &d));
+  if (one_start(d, P)) {  // exactly b200t5_generate_scored with that start token
+    a.start = d[0];
+    TRY(generate_impl(h, reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(attention_mask), B, S,
+                      params, a, s));
+    return copy_results(h, static_cast<size_t>(B), out_ids, out_len, a.sh.on ? score->token_logprobs : nullptr,
+                        a.sh.on ? score->token_logits : nullptr, cudaMemcpyDeviceToDevice, s);
+  }
+  TRY(generate_prefixed_impl(h, reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(attention_mask), B, S,
+                             params, a, d, P, s));
+  return copy_results(h, static_cast<size_t>(B), out_ids, out_len, a.sh.on ? score->token_logprobs : nullptr,
+                      a.sh.on ? score->token_logits : nullptr, cudaMemcpyDeviceToDevice, s, P - 1);
+}
+
+extern "C" int b200t5_generate_host_prefixed(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                                             const b200t5_gen_params* params, const b200t5_logits_params* logits, int64_t* out_ids,
+                                             int32_t* out_len, const b200t5_score_io* score, const int64_t* decoder_input_ids, int P) {
+  CallArgs a;
+  TRY(set_up_call(h, B, S, B, params, input_ids, out_ids, out_len, logits, score, true, &a));
+  std::vector<long long> d;
+  TRY(read_prompt(h, decoder_input_ids, B, P, params, score, &d));
+  if (one_start(d, P)) {
+    b200t5_gen_params gp = *params;
+    gp.decoder_start_token_id = d[0];
+    return b200t5_generate_host_scored(h, input_ids, attention_mask, B, S, &gp, logits, out_ids, out_len, score);
+  }
+  const int Tmax = P - 1 + a.T;
+  TRY(ensure_plan(h, B, S, Tmax, 1, P - 1));
+  Plan& p = *h->plan;
+  cudaStream_t s = h->exec_stream;
+  const size_t nb = static_cast<size_t>(B) * S * 8;
+  memcpy(p.h_ids, input_ids, nb);
+  CU_OK(h, cudaMemcpyAsync(p.ids_dev.p, p.h_ids, nb, cudaMemcpyHostToDevice, s));
+  if (attention_mask) {
+    memcpy(p.h_mask, attention_mask, nb);
+    CU_OK(h, cudaMemcpyAsync(p.mask_dev.p, p.h_mask, nb, cudaMemcpyHostToDevice, s));
+  }
+  TRY(generate_prefixed_impl(h, p.ids_dev.as<long long>(), attention_mask ? p.mask_dev.as<long long>() : nullptr, B, S, params, a, d, P, s));
+  TRY(copy_results(h, static_cast<size_t>(B), p.h_out, p.h_len, a.sh.on ? score->token_logprobs : nullptr,
+                   a.sh.on ? score->token_logits : nullptr, cudaMemcpyDeviceToHost, s, P - 1));
+  CU_OK(h, cudaStreamSynchronize(s));
+  memcpy(out_ids, p.h_out, static_cast<size_t>(B) * (Tmax + 1) * 8);
+  memcpy(out_len, p.h_len, static_cast<size_t>(B) * 4);
+  return B200T5_OK;
+}
+
+extern "C" int b200t5_test_prefill_cache(b200t5_handle h, int layer, void* kv_out, void* stream) {
+  if (!h || !h->plan || !kv_out) return fail(h, B200T5_EINVAL, "prefill cache: no plan or null argument");
+  Plan& p = *h->plan;
+  if (layer < 0 || layer >= h->c.Ld) return fail(h, B200T5_EINVAL, "prefill cache: layer %d outside [0, %d)", layer, h->c.Ld);
+  if (p.prompt_steps < 1) return fail(h, B200T5_EINVAL, "prefill cache: the last call had no decoder prompt of two or more ids");
+  CU_OK(h, cudaSetDevice(h->device));
+  const size_t row = static_cast<size_t>(p.prompt_steps) * 64 * 2, pitch = static_cast<size_t>(p.Tmax) * 64 * 2;
+  const act_t* src = p.self_kv.as<act_t>() + static_cast<size_t>(layer) * 2 * p.B * h->c.I * p.Tmax;
+  CU_OK(h, cudaMemcpy2DAsync(kv_out, row, src, pitch, row, static_cast<size_t>(2) * p.B * h->c.H, cudaMemcpyDeviceToDevice,
+                             static_cast<cudaStream_t>(stream)));
   return B200T5_OK;
 }
 

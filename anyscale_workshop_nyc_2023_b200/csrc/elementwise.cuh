@@ -230,6 +230,48 @@ __global__ void decode_init_kernel(DecodeState* st, int* __restrict__ unfinished
   for (int i = threadIdx.x; i < d / 8; i += blockDim.x) store_res8_from_act(dst + i * 8, src[i]);
 }
 
+// ---------------------------------------------------------------- decoder prompt (b200t5_generate_prefixed)
+// Start of a call with a decoder prompt d [B][P]: out[b] = d[b] then pad, x_dec[b] = E[d[b][P-1]], step = P-1, every
+// row unfinished (the prompt is not checked for EOS). Cache positions 0 .. P-2 hold the prompt's K/V (prefill_cache_kernel).
+__global__ void decode_init_prompt_kernel(DecodeState* st, int* __restrict__ unfinished, long long* __restrict__ out_ids,
+                                          int* __restrict__ out_len, int out_ld, int B, const long long* __restrict__ prompt, int P,
+                                          long long pad_tok, const act_t* __restrict__ E, res_t* __restrict__ x, int d) {
+  const int b = blockIdx.x;
+  if (b == 0 && threadIdx.x == 0) {
+    st->step = P - 1;
+    st->finished_rows = 0;
+  }
+  if (b >= B) return;
+  const long long* row = prompt + static_cast<size_t>(b) * P;
+  for (int j = threadIdx.x; j < out_ld; j += blockDim.x) out_ids[static_cast<size_t>(b) * out_ld + j] = j < P ? row[j] : pad_tok;
+  if (threadIdx.x == 0) {
+    unfinished[b] = 1;
+    out_len[b] = 0;
+  }
+  const uint4* src = reinterpret_cast<const uint4*>(E + static_cast<size_t>(row[P - 1]) * d);
+  res_t* dst = x + static_cast<size_t>(b) * d;
+  for (int i = threadIdx.x; i < d / 8; i += blockDim.x) store_res8_from_act(dst + i * 8, src[i]);
+}
+
+// The prefill's cache sink: one CTA per prompt position, row m = b * Tp + t of the forward pass's QKV product
+// [B*Tp, 3*H*64] (q | k | v); its K and V go to position t of one layer's cache [2][B][H][Tmax][64], where the decode
+// step's self-attention reads them. A copy: the cache holds exactly what the forward pass's causal attention read.
+__global__ void prefill_cache_kernel(const act_t* __restrict__ qkv, act_t* __restrict__ cache, int Tp, int B, int H, int Tmax) {
+  const int m = blockIdx.x, b = m / Tp, t = m - b * Tp, I = H * 64;
+  const uint4* src = reinterpret_cast<const uint4*>(qkv + static_cast<size_t>(m) * 3 * I + I);
+  for (int i = threadIdx.x; i < 2 * I / 8; i += blockDim.x) {
+    const int c = i * 8, kv = c / I, rem = c - kv * I, h = rem >> 6, d0 = rem & 63;
+    act_t* dst = cache + ((((static_cast<size_t>(kv) * B + b) * H + h) * Tmax + t) << 6) + d0;
+    *reinterpret_cast<uint4*>(dst) = src[i];
+  }
+}
+
+// End of a call with a decoder prompt: the lengths the steps wrote count positions (t + 1); the caller gets new tokens.
+__global__ void prompt_len_kernel(int* __restrict__ len, int B, int prompt_steps) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B) len[b] -= prompt_steps;
+}
+
 // ---------------------------------------------------------------- slot pool (b200t5_generate_stream)
 // Start of a streamed run: result rows = [start, pad, ...], every slot idle (position 0, nothing to attend,
 // decoder input = E[pad] so that idle slots compute on finite numbers).

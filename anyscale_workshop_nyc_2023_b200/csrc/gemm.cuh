@@ -669,7 +669,8 @@ struct EpiQkvDecode {
 //   kProc = true (logits_process.cuh): the logit after transformers' greedy processors. Each logit is rounded to act_t
 //     and widened to fp32 (HF's `.to(torch.float32)`), then in HF's order: encoder repetition penalty, repetition
 //     penalty (on the already penalised value), + 0 when bad words are active (HF adds a zero bias), and -inf where the
-//     row's next-step bans, the static mask, the begin-suppress mask (step 0) or the EOS mask (step < min_new) has the
+//     row's next-step bans, the static mask, the begin-suppress mask (step ProcCfg::begin_t, the first generated position) or the EOS
+//     mask (step < min_new) has the
 //     column's bit.
 //   kScore (token log-probabilities): also, per (row, tile),
 //     psum = sum_n expf(v_n - tile max)   (-inf columns add 0; an all -inf tile emits 0)
@@ -704,7 +705,7 @@ struct EpiLmHead {
     bool enc_pen, rep_pen, bad_add;
     float en, ep, rn, rp;
     size_t rw;
-    int t;
+    int t, begin_t;
   };
   struct Words {
     uint32_t ban, seen, enc;
@@ -721,6 +722,7 @@ struct EpiLmHead {
     r.rp = cf.rep_pos;
     r.rw = static_cast<size_t>(p.pd.row0 + m) * p.pd.W;
     r.t = m_ok ? p.step[m * p.step_stride] : 1;
+    r.begin_t = cf.begin_t;
     return r;
   }
   static DEVINL Words words(const Params& p, const Row& r, bool m_ok, int n0) {
@@ -728,7 +730,7 @@ struct EpiLmHead {
     Words o{0, 0, 0};
     if (m_ok && w < W) {
       o.ban = p.pd.banned[r.rw + w] | p.pd.stat[w];
-      if (r.t == 0) o.ban |= p.pd.stat[W + w];
+      if (r.t == r.begin_t) o.ban |= p.pd.stat[W + w];
       if (r.t < p.min_new) o.ban |= p.pd.stat[2 * W + w];
       if (r.rep_pen) o.seen = p.pd.seen[r.rw + w];
       if (r.enc_pen) o.enc = p.pd.enc[r.rw + w];

@@ -31,6 +31,7 @@ struct ProcCfg {
   int bad_add;           // NoBadWordsLogitsProcessor is active: scores + bias turns -0.0 into +0.0 everywhere
   int n_eos;
   int eos[kProcMaxEos];
+  int begin_t;  // the first generated position, where begin_suppress_tokens apply: 0, or P - 1 after a decoder prompt of P ids
 };
 
 struct ProcDev {
@@ -110,7 +111,8 @@ DEVINL void proc_new_bans(const ProcDev& pd, int r, const long long* __restrict_
 
 // Start of a row (static batch: every row after decode_init_kernel; slot pool: every admitted slot after
 // admit_slots_kernel): clear its bitmaps, keep its prompt ids, mark the prompt's tokens and the L decoder ids of
-// hist (the start token; the test hook passes a longer history) and compute the bans of its first step.
+// hist (the start token, or a call's decoder prompt; the test hook passes a longer history) and compute the bans of
+// its first step.
 // Row r = slots[blockIdx.x] (slots == nullptr: blockIdx.x); its history is row out_row[r] (nullptr: r) of hist_base.
 __global__ void proc_reset_kernel(ProcDev pd, const int* __restrict__ slots, const long long* __restrict__ ids,
                                   const long long* __restrict__ hist_base, int hist_ld, const int* __restrict__ out_row,

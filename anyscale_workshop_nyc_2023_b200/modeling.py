@@ -420,17 +420,25 @@ class B200T5ForConditionalGeneration:
 
     # ------------------------------------------------------------------ generation
     def _gen_params(self, max_new_tokens=None, max_length=None, min_new_tokens=None, min_length=None, eos_token_id=None,
-                    pad_token_id=None, decoder_start_token_id=None, poll_interval=8, **_) -> _lib.GenParams:
+                    pad_token_id=None, decoder_start_token_id=None, poll_interval=8, _prompt_len=None, **_) -> _lib.GenParams:
         # takes a call's whole kwargs (generate_host, generate_stream) and ignores the ones that are not its own.
-        # GenerationMixin._prepare_generated_length (generation/utils.py:1619-1639): the decoder
-        # prompt is the single start token, so max_length = max_new_tokens + 1.
+        # GenerationMixin._prepare_generated_length (generation/utils.py:1619-1639): without a decoder prompt
+        # (_prompt_len None) the decoder input is the single start token, so max_length = max_new_tokens + 1.
+        # With a decoder prompt of P ids (start token included), max_length and min_length count the whole decoder
+        # sequence, the prompt included, max_new_tokens and min_new_tokens the new tokens only; without any of them
+        # transformers 5.5 generates generation_config.max_length new tokens after the prompt.
+        P = 1 if _prompt_len is None else int(_prompt_len)
         if max_new_tokens is None:
-            max_length = self.generation_config.max_length if max_length is None else max_length
-            max_new_tokens = int(max_length) - 1
+            if _prompt_len is not None and max_length is None:
+                max_new_tokens = int(self.generation_config.max_length)
+            else:
+                max_length = self.generation_config.max_length if max_length is None else max_length
+                max_new_tokens = int(max_length) - P
         if max_new_tokens < 1:
-            raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
+            raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}"
+                             + (f" (max_length={max_length} with a decoder prompt of {P} ids)" if _prompt_len is not None else ""))
         if min_new_tokens is None:
-            min_new_tokens = max(int(min_length) - 1, 0) if min_length else 0
+            min_new_tokens = max(int(min_length) - P, 0) if min_length else 0
         if isinstance(eos_token_id, (list, tuple, torch.Tensor)):
             eos_token_id = _eos_ids(eos_token_id)[0]  # the rest go to the logits processors (_logits_args)
         return _lib.GenParams(
@@ -440,6 +448,21 @@ class B200T5ForConditionalGeneration:
             decoder_start_token_id=-1 if decoder_start_token_id is None else int(decoder_start_token_id),
             poll_interval=int(poll_interval),
         )
+
+    def _decoder_prompt(self, decoder_input_ids, batch: int, decoder_start_token_id=None) -> np.ndarray:
+        """decoder_input_ids as the decoder prompt d, int64 [batch, P] on the host, after transformers' rule
+        (GenerationMixin._prepare_decoder_input_ids_for_generation): the decoder start token is prepended only when
+        EVERY row's first id differs from it."""
+        d = decoder_input_ids.detach().cpu().numpy() if isinstance(decoder_input_ids, torch.Tensor) else np.asarray(decoder_input_ids)
+        if d.ndim != 2 or d.shape[0] != batch or d.shape[1] < 1 or d.dtype.kind not in "iu":
+            raise ValueError(f"decoder_input_ids must be integers [batch={batch}, length >= 1], got {d.dtype} {d.shape}")
+        d = d.astype(np.int64)
+        if ((d < 0) | (d >= self.config.vocab_size)).any():
+            raise IndexError("decoder_input_ids contain token ids outside [0, vocab_size)")
+        start = self.generation_config.decoder_start_token_id if decoder_start_token_id is None else int(decoder_start_token_id)
+        if (d[:, 0] != start).all():
+            d = np.concatenate([np.full((batch, 1), start, dtype=np.int64), d], axis=1)
+        return np.ascontiguousarray(d)
 
     def _logits_args(self, kw: Dict[str, Any], eos_token_id) -> Optional[_LogitsArgs]:
         default_eos = self.generation_config.eos_token_id
@@ -460,7 +483,16 @@ class B200T5ForConditionalGeneration:
         return_dict_in_generate=True returns a GenerateOutput (`.sequences` = that tensor); with output_scores=True its
         `.scores` / `.token_logprobs` carry each generated token's processed score and log-probability, computed in
         the lm_head epilogue (see TokenScores, compute_transition_scores). output_logits / output_attentions /
-        output_hidden_states raise NotImplementedError."""
+        output_hidden_states raise NotImplementedError.
+        decoder_input_ids [B, P0] is a decoder prompt (an answer prefix): the decoder start token is prepended when every
+        row's first id differs from it, as transformers does, and the result d of P ids is returned in front of the new
+        tokens: [B, P + T']. max_length / min_length count d, max_new_tokens / min_new_tokens the new tokens; scores cover
+        the new tokens only. Without any length argument a call with decoder_input_ids generates
+        generation_config.max_length (20) new tokens after the prompt, transformers 5.5's rule, while a call without it
+        keeps max_length - 1 = 19 new tokens: generate(decoder_input_ids=[[start]] * B) therefore runs one step more than
+        generate() unless a length is given (with one, the two calls are identical). The prompt runs as one parallel
+        decoder pass (b200t5_generate_prefixed), in static batches of at most pool_size rows. With num_beams > 1, or with
+        decoder_attention_mask, it raises NotImplementedError."""
         if input_ids is None:
             input_ids = unused.pop("inputs", None)
         if input_ids is None:
@@ -472,16 +504,27 @@ class B200T5ForConditionalGeneration:
             v = unused.get(k)
             if v is not None and not (isinstance(v, (int, float)) and v == 1):
                 raise NotImplementedError(f"generate({k}=...) is not supported by the CUDA path")
-        for k in ("logits_processor", "stopping_criteria", "forced_bos_token_id", "decoder_input_ids", "encoder_outputs"):
+        for k in ("logits_processor", "stopping_criteria", "forced_bos_token_id", "encoder_outputs", "decoder_attention_mask"):
             if unused.get(k) is not None:  # (may be tensors: no truth-value tests)
                 raise NotImplementedError(f"generate({k}=...) is not supported by the CUDA path")
+        dec = unused.pop("decoder_input_ids", None)
+        if dec is not None and bp is not None:
+            raise NotImplementedError("generate(decoder_input_ids=...) with num_beams > 1 is not supported by the CUDA path")
         as_dict, want_scores = generate_output_flags(unused)
-        gp = self._gen_params(max_new_tokens, max_length, min_new_tokens, min_length, eos_token_id, pad_token_id,
-                              decoder_start_token_id, poll_interval)
-        lp = self._logits_args(unused, eos_token_id)
         host = torch.as_tensor(input_ids)
         if host.dim() != 2:
             raise ValueError(f"input_ids must be [batch, seq], got {tuple(host.shape)}")
+        prompt = None if dec is None else self._decoder_prompt(dec, host.shape[0], decoder_start_token_id)
+        gp = self._gen_params(max_new_tokens, max_length, min_new_tokens, min_length, eos_token_id, pad_token_id,
+                              decoder_start_token_id, poll_interval, _prompt_len=None if prompt is None else prompt.shape[1])
+        lp = self._logits_args(unused, eos_token_id)
+        if prompt is not None:
+            # never the slot pool: static chunks of pool_size rows
+            ids, mask = self._device_inputs(host, attention_mask, gp, lp)
+            res = self._generate_chunks(ids, mask, gp, lp, score=as_dict and want_scores, prompt=prompt)
+            if as_dict and want_scores:
+                return GenerateOutput(res[0], TokenScores(res[2], res[3]))
+            return GenerateOutput(res[0]) if as_dict else res[0]
         if bp is not None:
             ids, mask = self._device_inputs(host, attention_mask, gp, None)
             seq, _, scores, bidx, logp = self._generate_beam(ids, mask, gp, bp, self._generate_beam_static)
@@ -607,16 +650,19 @@ class B200T5ForConditionalGeneration:
             return tuple(torch.from_numpy(np.ascontiguousarray(a)).to(self._device) for a in res)
         return self._generate_chunks(ids, mask, gp, lp, score=True, labels=labels)
 
-    def _generate_chunks(self, ids: torch.Tensor, mask: Optional[torch.Tensor], gp, lp, score: bool = False, labels=None):
-        """Static batches of at most pool_size rows: (sequences [B, 1+T'], lengths [B]) and, with score=True,
+    def _generate_chunks(self, ids: torch.Tensor, mask: Optional[torch.Tensor], gp, lp, score: bool = False, labels=None,
+                         prompt: Optional[np.ndarray] = None):
+        """Static batches of at most pool_size rows: (sequences [B, P+T'], lengths [B]) and, with score=True,
         (token_logprobs [B, T'], token_logits [B, T']), on the device. T' = the steps of the longest row, or
-        labels.shape[1] for a teacher-forced call."""
+        labels.shape[1] for a teacher-forced call. P = 1, or the decoder prompt's length (`prompt` int64 [B, P])."""
         parts = [self._generate_static(ids[lo:lo + self.pool_size], None if mask is None else mask[lo:lo + self.pool_size], gp, lp,
-                                       score, None if labels is None else labels[lo:lo + self.pool_size])
+                                       score, None if labels is None else labels[lo:lo + self.pool_size],
+                                       None if prompt is None else prompt[lo:lo + self.pool_size])
                  for lo in range(0, ids.shape[0], self.pool_size)]
         out, lens, *scores = parts[0] if len(parts) == 1 else [torch.cat(c, dim=0) for c in zip(*parts)]
         steps = gp.max_new_tokens if labels is not None else int(lens.max().item())  # HF returns exactly the steps it ran
-        return (out[:, : steps + 1], lens, *(a[:, :steps] for a in scores))
+        P = 1 if prompt is None else prompt.shape[1]
+        return (out[:, : steps + P], lens, *(a[:, :steps] for a in scores))
 
     def _generate_beam(self, ids, mask, gp, bp, run_chunk):
         """Beam search in static chunks of pool_size // num_beams prompts, each run by run_chunk(ids, mask, gp, bp), which
@@ -722,15 +768,18 @@ class B200T5ForConditionalGeneration:
             return None
         return (~is_pad).to(torch.long).contiguous()
 
-    def _generate_static(self, ids: torch.Tensor, mask: Optional[torch.Tensor], gp, lp=None, score: bool = False, labels=None):
-        """One static batch, full width: (ids [B, T+1], lengths [B]) and, with score=True, (token_logprobs [B, T],
-        token_logits [B, T]). The library pads every row to T+1 with pad_token_id."""
+    def _generate_static(self, ids: torch.Tensor, mask: Optional[torch.Tensor], gp, lp=None, score: bool = False, labels=None,
+                         prompt: Optional[np.ndarray] = None):
+        """One static batch, full width: (ids [B, P+T], lengths [B]) and, with score=True, (token_logprobs [B, T],
+        token_logits [B, T]). The library pads every row to P+T with pad_token_id. P = 1, or the length of the decoder
+        prompt `prompt` int64 [B, P] (b200t5_generate_prefixed)."""
         B, S = ids.shape
         ids = ids.contiguous()
         mask = None if mask is None else mask.contiguous()
         T = gp.max_new_tokens
+        P = 1 if prompt is None else prompt.shape[1]
         with torch.cuda.device(self._index):
-            out = torch.empty((B, T + 1), dtype=torch.long, device=self._device)
+            out = torch.empty((B, T + P), dtype=torch.long, device=self._device)
             lens = torch.empty((B,), dtype=torch.int32, device=self._device)
             stream = torch.cuda.current_stream(self._device)
             with self._gpu_lock:
@@ -740,10 +789,17 @@ class B200T5ForConditionalGeneration:
                     logit = torch.empty((B, T), dtype=torch.float32, device=self._device)
                     forced = None if labels is None else torch.from_numpy(np.ascontiguousarray(labels)).to(self._device)
                     io, _keep = self._score_io(logp, logit, forced)
-                _chk(self, self._lib.b200t5_generate_scored(self._h, _ptr(ids), _ptr(mask), B, S, C.byref(gp),
-                                                            None if lp is None else lp.ref(), _ptr(out), _ptr(lens),
-                                                            None if io is None else C.byref(io), C.c_void_p(stream.cuda_stream)),
-                     self._h)
+                if prompt is None:
+                    _chk(self, self._lib.b200t5_generate_scored(self._h, _ptr(ids), _ptr(mask), B, S, C.byref(gp),
+                                                                None if lp is None else lp.ref(), _ptr(out), _ptr(lens),
+                                                                None if io is None else C.byref(io), C.c_void_p(stream.cuda_stream)),
+                         self._h)
+                else:  # the prompt stays on the host: the library checks and stages it there
+                    hp = np.ascontiguousarray(prompt, dtype=np.int64)
+                    _chk(self, self._lib.b200t5_generate_prefixed(self._h, _ptr(ids), _ptr(mask), B, S, C.byref(gp),
+                                                                  None if lp is None else lp.ref(), _ptr(out), _ptr(lens),
+                                                                  None if io is None else C.byref(io), hp.ctypes.data_as(C.c_void_p),
+                                                                  P, C.c_void_p(stream.cuda_stream)), self._h)
                 self.last_lengths = lens
                 stream.synchronize()
         return (out, lens, logp, logit) if score else (out, lens)
@@ -758,20 +814,28 @@ class B200T5ForConditionalGeneration:
         """numpy in / numpy out through b200t5_generate_host_scored (the foreign-host entry point):
         H2D copy, generation, D2H copy and synchronisation all happen inside the library. Takes the logits
         processor kwargs `generate` takes. With output_scores=True it returns (ids, lengths, token_logprobs,
-        token_logits), the last two fp32 [B, T']."""
-        gp = self._gen_params(**kw)
+        token_logits), the last two fp32 [B, T']. decoder_input_ids as generate: ids [B, P+T'] start with the decoder
+        prompt (b200t5_generate_host_prefixed)."""
+        if kw.get("decoder_attention_mask") is not None:
+            raise NotImplementedError("generate_host(decoder_attention_mask=...) is not supported by the CUDA path")
+        ids = np.ascontiguousarray(input_ids, dtype=np.int64)
+        B, S = ids.shape
+        dec = kw.get("decoder_input_ids")
+        prompt = None if dec is None else self._decoder_prompt(dec, B, kw.get("decoder_start_token_id"))
+        gp = self._gen_params(**kw, _prompt_len=None if prompt is None else prompt.shape[1])
         if kw.get("do_sample") and kw.get("num_beams") not in (None, 1):
             raise NotImplementedError("beam sampling (do_sample=True, num_beams > 1) is not implemented")
         bp = beam_params(kw.get("num_beams"), kw, _eos_ids(kw.get("eos_token_id")), self.generation_config.eos_token_id,
                          self.config.vocab_size)
+        if prompt is not None and bp is not None:
+            raise NotImplementedError("generate_host(decoder_input_ids=...) with num_beams > 1 is not supported by the CUDA path")
         lp = self._logits_args(kw, kw.get("eos_token_id"))
-        ids = np.ascontiguousarray(input_ids, dtype=np.int64)
-        B, S = ids.shape
         mask = self._infer_mask_np(ids, gp, lp) if attention_mask is None else np.ascontiguousarray(attention_mask, dtype=np.int64)
         if bp is not None:
             self._check_inputs(ids, mask)
             return self._generate_beam(ids, mask, gp, bp, self._generate_host_beam_chunk)
-        out = np.empty((B, gp.max_new_tokens + 1), dtype=np.int64)
+        P = 1 if prompt is None else prompt.shape[1]
+        out = np.empty((B, gp.max_new_tokens + P), dtype=np.int64)
         lens = np.empty((B,), dtype=np.int32)
         want_scores = generate_output_flags(kw)[1]
         with self._gpu_lock:
@@ -781,14 +845,16 @@ class B200T5ForConditionalGeneration:
                 logp = np.empty((B, gp.max_new_tokens), dtype=np.float32)
                 logit = np.empty((B, gp.max_new_tokens), dtype=np.float32)
                 io, _keep = self._score_io(logp, logit, None)
-            _chk(self, self._lib.b200t5_generate_host_scored(self._h, ids.ctypes.data_as(C.c_void_p), mp, B, S, C.byref(gp),
-                                                             None if lp is None else lp.ref(), out.ctypes.data_as(C.c_void_p),
-                                                             lens.ctypes.data_as(C.c_void_p), None if io is None else C.byref(io)),
-                 self._h)
+            args = (self._h, ids.ctypes.data_as(C.c_void_p), mp, B, S, C.byref(gp), None if lp is None else lp.ref(),
+                    out.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p), None if io is None else C.byref(io))
+            if prompt is None:
+                _chk(self, self._lib.b200t5_generate_host_scored(*args), self._h)
+            else:
+                _chk(self, self._lib.b200t5_generate_host_prefixed(*args, prompt.ctypes.data_as(C.c_void_p), P), self._h)
         steps = int(lens.max())
         if want_scores:
-            return out[:, : steps + 1], lens, logp[:, :steps], logit[:, :steps]
-        return out[:, : steps + 1], lens
+            return out[:, : steps + P], lens, logp[:, :steps], logit[:, :steps]
+        return out[:, : steps + P], lens
 
     def _generate_host_beam_chunk(self, ids: np.ndarray, mask: Optional[np.ndarray], gp, bp):
         ids = np.ascontiguousarray(ids)
@@ -825,6 +891,8 @@ class B200T5ForConditionalGeneration:
         lp = _logits if _gen_params is not None else self._logits_args(kw, kw.get("eos_token_id"))
         if kw.get("num_beams") not in (None, 1):
             raise NotImplementedError("generate_stream(num_beams > 1): beam search runs as static batches (generate)")
+        if kw.get("decoder_input_ids") is not None:
+            raise NotImplementedError("generate_stream(decoder_input_ids=...): a decoder prompt runs as static batches (generate)")
         ids = np.ascontiguousarray(input_ids, dtype=np.int64)
         if ids.ndim != 2:
             raise ValueError(f"input_ids must be [batch, seq], got {ids.shape}")

@@ -204,6 +204,32 @@ int b200t5_generate_stream_scored(b200t5_handle h, const int64_t* input_ids, con
                                   int admit_min, int64_t* out_ids, int32_t* out_len, const b200t5_score_io* score);
 int b200t5_get_stats(b200t5_handle h, b200t5_stats* out);
 
+/* A decoder prompt (transformers' generate(decoder_input_ids=...)): b200t5_generate_scored whose rows start from the
+ * decoder ids d = decoder_input_ids int64 [B, P] instead of the start token. The library takes d as given: d[b][0] is
+ * the row's first decoder input, so a caller that follows transformers prepends the decoder start token itself (when
+ * every row's first id differs from it). Every row starts unfinished whatever d holds; every prompt position is
+ * attended to. The prompt's positions 0 .. P-2 run as one forward pass over B*(P-1) rows that fills the self-attention
+ * cache; then max_new_tokens decode steps run from position P-1.
+ *   out_ids: int64 [B, P + max_new_tokens] = d, then the generated tokens, then pad_token_id;
+ *   out_len: int32 [B] = NEW tokens per row (EOS included), not counting the prompt;
+ *   score (may be NULL): token_logprobs / token_logits fp32 [B, max_new_tokens], one column per new token.
+ * min_new_tokens counts new tokens; begin_suppress_tokens apply at position P-1, the first generated one; the
+ * repetition penalty and the n-gram bans see d. P == 1 with d[b][0] equal in every row is exactly
+ * b200t5_generate_scored with that decoder start token: same kernels, same launch count, same bits.
+ * B200T5_EINVAL for P < 1, decoder ids outside [0, vocab_size), P-1 + max_new_tokens > 4096 or score->forced_ids, and
+ * for P >= 2 when B200T5_SK sets the feed-forward wi tile to other than 128 rows (the prefill is b200t5_forward's
+ * decoder pass, which needs that tile), all before anything is enqueued.
+ * decoder_input_ids is a HOST pointer in both entry points: the prompt is checked and staged on the host. The other
+ * pointers are device pointers, and the call is enqueued on `stream` like b200t5_generate_scored. */
+int b200t5_generate_prefixed(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                             const b200t5_gen_params* params, const b200t5_logits_params* logits, int64_t* out_ids,
+                             int32_t* out_len, const b200t5_score_io* score, const int64_t* decoder_input_ids, int P,
+                             void* stream);
+/* The same with host buffers (as b200t5_generate_host_scored) for every pointer: synchronous. */
+int b200t5_generate_host_prefixed(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                                  const b200t5_gen_params* params, const b200t5_logits_params* logits, int64_t* out_ids,
+                                  int32_t* out_len, const b200t5_score_io* score, const int64_t* decoder_input_ids, int P);
+
 /* Beam search (transformers' GenerationMixin._beam_search with do_sample=False and one EOS id): each prompt decodes as
  * num_beams rows. Length penalty: a finished hypothesis of l generated tokens scores sum(log-probs) * fp32(1 / l**p),
  * the reciprocal taken in double. Ties: value descending, then token (beam * vocab + token across a prompt) ascending. */
@@ -343,6 +369,10 @@ int b200t5_encode(b200t5_handle h, const int64_t* input_ids, const int64_t* atte
  * (device); logits are the bf16 lm_head outputs widened to fp32, as HF's `.float()` does. */
 int b200t5_decode_logits(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
                          const int64_t* decoder_input_ids, int T, float* logits, void* stream);
+/* After a b200t5_generate_prefixed call with P >= 2 (and before any other call): decoder layer `layer`'s self-attention
+ * cache at the prompt positions 0 .. P-2, as the prefill wrote it: kv_out [2][B][H][P-1][64] in the build's 2-byte
+ * type (device), K then V. */
+int b200t5_test_prefill_cache(b200t5_handle h, int layer, void* kv_out, void* stream);
 /* T5Attention._relative_position_bucket for one offset (host-only, no GPU needed). */
 int b200t5_relative_bucket(int relative_position, int bidirectional, int num_buckets, int max_distance);
 
