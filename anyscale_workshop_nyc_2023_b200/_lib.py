@@ -168,6 +168,7 @@ SIGNATURES = {
     "b200t5_decode_logits": (_i, [_vp, _i64p, _i64p, _i, _i, _i64p, _i, _vp, _vp]),
     "b200t5_test_prefill_cache": (_i, [_vp, _i, _vp, _vp]),
     "b200t5_forward": (_i, [_vp, _i64p, _i64p, _i, _i, _i64p, _i64p, _i, C.POINTER(ForwardIO), _vp]),
+    "b200t5_forward_choices": (_i, [_vp, _i64p, _i64p, _i, _i, _vp, _i64p, _i, C.POINTER(ForwardIO), _vp]),
     "b200t5_relative_bucket": (_i, [_i, _i, _i, _i]),
     "b200t5_test_gemm": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "b200t5_test_enc_gemm": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp]),
@@ -178,6 +179,7 @@ SIGNATURES = {
     "b200t5_test_encoder_attn": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b200t5_test_decoder_self_attn": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "b200t5_test_decoder_cross_attn": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "b200t5_test_decoder_cross_attn_packed": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "b200t5_test_geglu": (_i, [_i, _vp, _vp, _vp, C.c_int64, _i, _vp]),
     "b200t5_version": (C.c_char_p, []),
 }

@@ -224,4 +224,29 @@ decoder_attn_kernel(const act_t* __restrict__ qkv, const act_t* __restrict__ kv,
   }
 }
 
+// The cross-attention of the multiple-choice forward pass (b200t5_forward_choices): the queries of all of prompt b's
+// candidates are the contiguous rows qoff[b] .. qoff[b+1]-1 of q [*, I], tiled 64 at a time as one query sequence
+// against prompt b's K/V in the cross-K/V arena kv = [2][B][H][S][64], keys masked by key_ok [B][S] / extent [B] as in
+// kAttnCross. Cross-attention has no causal mask and no position bias, and every query row keeps its own softmax, so
+// a row's result does not depend on which rows share its tile: each row gets the bits decoder_attn_kernel<kAttnCross>
+// gives it against a private copy of the prompt's K/V, which is loaded here once per tile instead of once per candidate.
+// ctx rows as q. Grid (tiles of the longest prompt's queries, B * H); CTAs past a prompt's queries exit.
+__global__ void __launch_bounds__(kEncThreads)
+decoder_cross_packed_kernel(const act_t* __restrict__ q, const act_t* __restrict__ kv, act_t* __restrict__ ctx,
+                            const unsigned char* __restrict__ key_ok, const int* __restrict__ extent,
+                            const int* __restrict__ qoff, int B, int S, int H) {
+  extern __shared__ __align__(128) uint8_t dec_smem[];
+  const int I = H * 64;
+  const int bh = blockIdx.y;
+  const int b = bh / H, h = bh - b * H;
+  const int i0 = blockIdx.x * kEncQ;
+  const int q0 = qoff[b], rows = qoff[b + 1] - q0;
+  if (i0 >= rows) return;
+  const size_t plane = static_cast<size_t>(B) * I * S;
+  const act_t* kg = kv + (static_cast<size_t>(b) * H + h) * S * 64;
+  attn_tile_2pass<kAttnCross>(dec_smem, q + static_cast<size_t>(q0) * I + h * 64, I, kg, kg + plane, 64,
+                              ctx + static_cast<size_t>(q0) * I + h * 64, I, nullptr, key_ok + static_cast<size_t>(b) * S,
+                              extent[b], rows, i0, S, h);
+}
+
 }  // namespace b200

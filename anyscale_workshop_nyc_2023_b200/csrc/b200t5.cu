@@ -599,6 +599,8 @@ static cudaError_t init_kernel_attrs() {
     return e;
   if ((e = cudaFuncSetAttribute(decoder_attn_kernel<kAttnCross>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024)) != cudaSuccess)
     return e;
+  if ((e = cudaFuncSetAttribute(decoder_cross_packed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024)) != cudaSuccess)
+    return e;
   if ((e = cudaFuncSetAttribute(attn_cross_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 static_cast<int>(XsSmem::bytes(kXsMaxStages, 4096)))) != cudaSuccess)
     return e;
@@ -2432,15 +2434,21 @@ static cudaError_t run_geglu_fwd(b200t5_ctx* h, const CUtensorMap& tmA, const De
 // layer's 128-row-box tensor maps, except GeGLU (run_geglu_fwd).
 // `prefill` (a decoder prompt's positions 0 .. T-1): each layer's K/V also go to cache positions 0 .. T-1
 // (prefill_cache_kernel), and the pass ends at the last layer's K/V: nothing reads the prompt positions' outputs.
-static int run_decoder_forward(b200t5_ctx* h, int T, cudaStream_t s, bool prefill = false) {
+// `qoff` (b200t5_forward_choices): the decoder runs R rows of T positions for the plan's B prompts, prompt b's rows
+// holding the query rows qoff[b] .. qoff[b+1]-1 (device int [B+1]), whose cross-attention is decoder_cross_packed_kernel
+// over q_tiles tiles of 64 queries. Without it row b is prompt b (R = B).
+static int run_decoder_forward(b200t5_ctx* h, int T, cudaStream_t s, bool prefill = false, int R = 0, const int* qoff = nullptr,
+                               int q_tiles = 0) {
   const Cfg& c = h->c;
   Plan& p = *h->plan;
-  const int B = p.B, S = p.S, d = c.d, I = c.I, F = c.F, H = c.H, M = B * T;
+  const int B = p.B, S = p.S, d = c.d, I = c.I, F = c.F, H = c.H;
+  if (!qoff) R = B;
+  const int M = R * T;
   res_t* x = p.x.as<res_t>();
   act_t* xn = p.xn.as<act_t>();
   act_t* qkv = p.qkv.as<act_t>();
   act_t* ctx = p.ctx.as<act_t>();
-  const dim3 agrid((T + kEncQ - 1) / kEncQ, B * H);
+  const dim3 agrid((T + kEncQ - 1) / kEncQ, R * H);
   for (int l = 0; l < c.Ld; ++l) {
     DecLayerW& w = h->dec[l];
     CU_OK(h, run_rmsnorm(h, x, w.ln0.as<act_t>(), xn, M, d, c.eps, s));
@@ -2452,7 +2460,7 @@ static int run_decoder_forward(b200t5_ctx* h, int T, cudaStream_t s, bool prefil
       if (l == c.Ld - 1) return B200T5_OK;
     }
     decoder_attn_kernel<kAttnCausal><<<agrid, kEncThreads, encoder_attn_smem_bytes(T), s>>>(
-        qkv, nullptr, ctx, p.fwd_bias.as<float>(), nullptr, nullptr, B, T, T, H);
+        qkv, nullptr, ctx, p.fwd_bias.as<float>(), nullptr, nullptr, R, T, T, H);
     h->launches++;
     CU_OK(h, cudaGetLastError());
     {
@@ -2462,9 +2470,13 @@ static int run_decoder_forward(b200t5_ctx* h, int T, cudaStream_t s, bool prefil
     }
     CU_OK(h, run_rmsnorm(h, x, w.ln1.as<act_t>(), xn, M, d, c.eps, s));
     CU_OK(h, run_gemm_2cta<EpiStore>(h, p.tm_xn, w.tm2_cq, M, I, d, EpiStore::Params{qkv, I}, s));
-    decoder_attn_kernel<kAttnCross><<<agrid, kEncThreads, encoder_attn_smem_bytes(S), s>>>(
-        qkv, p.cross_kv.as<act_t>() + static_cast<size_t>(l) * 2 * B * I * S, ctx, nullptr, p.key_ok.as<unsigned char>(),
-        p.extent.as<int>(), B, T, S, H);
+    const act_t* kv = p.cross_kv.as<act_t>() + static_cast<size_t>(l) * 2 * B * I * S;
+    if (qoff)
+      decoder_cross_packed_kernel<<<dim3(q_tiles, B * H), kEncThreads, encoder_attn_smem_bytes(S), s>>>(
+          qkv, kv, ctx, p.key_ok.as<unsigned char>(), p.extent.as<int>(), qoff, B, S, H);
+    else
+      decoder_attn_kernel<kAttnCross><<<agrid, kEncThreads, encoder_attn_smem_bytes(S), s>>>(
+          qkv, kv, ctx, nullptr, p.key_ok.as<unsigned char>(), p.extent.as<int>(), B, T, S, H);
     h->launches++;
     CU_OK(h, cudaGetLastError());
     {
@@ -2511,21 +2523,19 @@ static int ensure_fwd_bias(b200t5_ctx* h, int T) {
   return B200T5_OK;
 }
 
-extern "C" int b200t5_forward(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
-                              const int64_t* decoder_input_ids, const int64_t* labels, int T, const b200t5_forward_io* io,
-                              void* stream) {
-  TRY(validate(h, B, S, nullptr));
-  if (!input_ids || !io) return fail(h, B200T5_EINVAL, "forward: null argument");
-  if (!decoder_input_ids && !labels) return fail(h, B200T5_EINVAL, "forward: decoder_input_ids or labels is required");
-  if (!io->logits && !io->token_logprobs) return fail(h, B200T5_EINVAL, "forward: neither logits nor token_logprobs requested");
-  if (io->token_logprobs && !labels) return fail(h, B200T5_EINVAL, "forward: token_logprobs needs labels");
-  if (T < 1 || T > 4096) return fail(h, B200T5_EINVAL, "forward: T=%d outside [1, 4096]", T);
-  TRY(check_forward_wi(h, "forward"));
+// The teacher-forced pass of b200t5_forward and b200t5_forward_choices: the encoder and the cross-K/V projection over
+// B prompts, then the decoder over R rows of T positions and the lm_head. `offs` (host int [B+1], b200t5_forward_choices)
+// puts rows offs[b] .. offs[b+1]-1 on prompt b; NULL (b200t5_forward) puts row b on prompt b, R = B. `who` names the
+// entry point in error messages.
+static int forward_impl(b200t5_ctx* h, const char* who, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                        const int32_t* offs, const int64_t* decoder_input_ids, const int64_t* labels, int T,
+                        const b200t5_forward_io* io, void* stream) {
   CU_OK(h, cudaSetDevice(h->device));
   const Cfg& c = h->c;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const size_t M = static_cast<size_t>(B) * T;
-  if (M > static_cast<size_t>(INT32_MAX) / 8) return fail(h, B200T5_EINVAL, "forward: B*T too large");
+  const int R = offs ? offs[B] : B;
+  const size_t M = static_cast<size_t>(R) * T;
+  if (M > static_cast<size_t>(INT32_MAX) / 8) return fail(h, B200T5_EINVAL, "%s: %s*T too large", who, offs ? "R" : "B");
   // labels and decoder ids are read back and checked; without decoder ids they are transformers' _shift_right(labels)
   std::vector<long long> lab, dec(M);
   CU_OK(h, cudaStreamSynchronize(s));
@@ -2533,24 +2543,24 @@ extern "C" int b200t5_forward(b200t5_handle h, const int64_t* input_ids, const i
     lab.resize(M);
     CU_OK(h, cudaMemcpy(lab.data(), labels, M * 8, cudaMemcpyDeviceToHost));
     for (long long v : lab)
-      if (v != -100 && (v < 0 || v >= c.V)) return fail(h, B200T5_EINVAL, "forward: label %lld outside [0, %d) and not -100", v, c.V);
+      if (v != -100 && (v < 0 || v >= c.V)) return fail(h, B200T5_EINVAL, "%s: label %lld outside [0, %d) and not -100", who, v, c.V);
   }
   if (decoder_input_ids) {
     CU_OK(h, cudaMemcpy(dec.data(), decoder_input_ids, M * 8, cudaMemcpyDeviceToHost));
     for (long long v : dec)
-      if (v < 0 || v >= c.V) return fail(h, B200T5_EINVAL, "forward: decoder id %lld outside [0, %d)", v, c.V);
+      if (v < 0 || v >= c.V) return fail(h, B200T5_EINVAL, "%s: decoder id %lld outside [0, %d)", who, v, c.V);
   } else {
-    if (c.start < 0 || c.start >= c.V || c.pad < 0 || c.pad >= c.V) return fail(h, B200T5_EINVAL, "forward: special token id out of range");
-    for (size_t b = 0; b < static_cast<size_t>(B); ++b)
+    if (c.start < 0 || c.start >= c.V || c.pad < 0 || c.pad >= c.V) return fail(h, B200T5_EINVAL, "%s: special token id out of range", who);
+    for (size_t b = 0; b < static_cast<size_t>(R); ++b)
       for (int t = 0; t < T; ++t) {
         const long long v = t == 0 ? c.start : lab[b * T + t - 1];
         dec[b * T + t] = v == -100 ? c.pad : v;
       }
   }
-  // the plan of (B, S): reused whatever its Tmax when its workspace holds B*T rows, else rebuilt with the same Tmax
-  // (1 for a new shape: the forward pass has no self-attention cache)
+  // the plan of (B, S): reused whatever its Tmax when its workspace holds the R*T decoder rows, else rebuilt with the
+  // same Tmax (1 for a new shape: the forward pass has no self-attention cache)
   {
-    const int ws = std::max(S, T);
+    const int ws = static_cast<int>(std::max<size_t>(S, (M + B - 1) / B));
     const bool same = h->plan && h->plan->B == B && h->plan->S == S && h->plan->group == 1;
     if (!same || h->plan->ws_S < ws) {
       const int Tm = same ? h->plan->Tmax : 1;
@@ -2561,16 +2571,26 @@ extern "C" int b200t5_forward(b200t5_handle h, const int64_t* input_ids, const i
   }
   Plan& p = *h->plan;
   const int nt = p.n_vtiles;
-  // ids [M] int64, label columns [M] int32, one zero int (the lm_head's step: min_new is 0)
-  const size_t ids_bytes = M * 8 + M * 4 + 16;
+  // ids [M] int64, label columns [M] int32, one zero int (the lm_head's step: min_new is 0), then (choices) the query-row
+  // offsets int [B+1]
+  const size_t ids_bytes = M * 8 + M * 4 + 16 + (offs ? static_cast<size_t>(B + 1) * 4 : 0);
   if (p.fwd_ids.bytes < ids_bytes) CU_OK(h, p.fwd_ids.alloc(ids_bytes));
   long long* ids_dev = p.fwd_ids.as<long long>();
   int* ftok_dev = reinterpret_cast<int*>(ids_dev + M);
   int* zero_dev = ftok_dev + M;
+  int* qoff_dev = zero_dev + 4;
   std::vector<int> ftok(M + 4, 0);
   for (size_t m = 0; m < M && labels; ++m) ftok[m] = lab[m] == -100 ? -1 : static_cast<int>(lab[m]);
   CU_OK(h, cudaMemcpyAsync(ids_dev, dec.data(), M * 8, cudaMemcpyHostToDevice, s));
   CU_OK(h, cudaMemcpyAsync(ftok_dev, ftok.data(), (M + 4) * 4, cudaMemcpyHostToDevice, s));
+  int q_tiles = 0;
+  std::vector<int> qoff;
+  if (offs) {
+    qoff.resize(B + 1);
+    for (int b = 0; b <= B; ++b) qoff[b] = offs[b] * T;
+    for (int b = 0; b < B; ++b) q_tiles = std::max(q_tiles, (qoff[b + 1] - qoff[b] + kEncQ - 1) / kEncQ);
+    CU_OK(h, cudaMemcpyAsync(qoff_dev, qoff.data(), qoff.size() * 4, cudaMemcpyHostToDevice, s));
+  }
   TRY(ensure_fwd_bias(h, T));
   // lm_head partials [M][n_tiles] x 3 + fval [M]: in hff (free after the last feed-forward block) when they fit
   const bool lp_on = io->token_logprobs != nullptr;
@@ -2587,7 +2607,7 @@ extern "C" int b200t5_forward(b200t5_handle h, const int64_t* input_ids, const i
   CU_OK(h, cudaEventRecord(h->ev[1], s));
   embed_rows_kernel<<<static_cast<unsigned>((M + 7) / 8), 256, 0, s>>>(ids_dev, h->shared.as<act_t>(), p.x.as<res_t>(), static_cast<int>(M), c.d, c.V);
   h->launches++;
-  TRY(run_decoder_forward(h, T, s));
+  TRY(run_decoder_forward(h, T, s, false, R, offs ? qoff_dev : nullptr, q_tiles));
   LmHeadParams ep{};
   ep.pval = part;
   ep.pidx = reinterpret_cast<int*>(part + M * nt);
@@ -2617,6 +2637,38 @@ extern "C" int b200t5_forward(b200t5_handle h, const int64_t* input_ids, const i
   h->last_steps = 0;
   h->ev_valid = true;
   return B200T5_OK;
+}
+
+extern "C" int b200t5_forward(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                              const int64_t* decoder_input_ids, const int64_t* labels, int T, const b200t5_forward_io* io,
+                              void* stream) {
+  TRY(validate(h, B, S, nullptr));
+  if (!input_ids || !io) return fail(h, B200T5_EINVAL, "forward: null argument");
+  if (!decoder_input_ids && !labels) return fail(h, B200T5_EINVAL, "forward: decoder_input_ids or labels is required");
+  if (!io->logits && !io->token_logprobs) return fail(h, B200T5_EINVAL, "forward: neither logits nor token_logprobs requested");
+  if (io->token_logprobs && !labels) return fail(h, B200T5_EINVAL, "forward: token_logprobs needs labels");
+  if (T < 1 || T > 4096) return fail(h, B200T5_EINVAL, "forward: T=%d outside [1, 4096]", T);
+  TRY(check_forward_wi(h, "forward"));
+  return forward_impl(h, "forward", input_ids, attention_mask, B, S, nullptr, decoder_input_ids, labels, T, io, stream);
+}
+
+extern "C" int b200t5_forward_choices(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                                      const int32_t* row_offsets, const int64_t* labels, int T, const b200t5_forward_io* io,
+                                      void* stream) {
+  TRY(validate(h, B, S, nullptr));
+  if (!input_ids || !io || !row_offsets || !labels) return fail(h, B200T5_EINVAL, "forward_choices: null argument");
+  if (!io->logits && !io->token_logprobs) return fail(h, B200T5_EINVAL, "forward_choices: neither logits nor token_logprobs requested");
+  if (T < 1 || T > 4096) return fail(h, B200T5_EINVAL, "forward_choices: T=%d outside [1, 4096]", T);
+  if (row_offsets[0] != 0) return fail(h, B200T5_EINVAL, "forward_choices: row_offsets[0] = %d, not 0", row_offsets[0]);
+  for (int b = 0; b < B; ++b)
+    if (row_offsets[b + 1] <= row_offsets[b])
+      return fail(h, B200T5_EINVAL, "forward_choices: row_offsets not strictly increasing at prompt %d (%d, %d)", b, row_offsets[b],
+                  row_offsets[b + 1]);
+  if (static_cast<long long>(row_offsets[B]) * h->c.H > 65535)
+    return fail(h, B200T5_EINVAL, "forward_choices: R*H = %lld exceeds 65535 (the causal self-attention's grid)",
+                static_cast<long long>(row_offsets[B]) * h->c.H);
+  TRY(check_forward_wi(h, "forward_choices"));
+  return forward_impl(h, "forward_choices", input_ids, attention_mask, B, S, row_offsets, nullptr, labels, T, io, stream);
 }
 
 // ================================================================== decoder prompt
@@ -3273,6 +3325,32 @@ extern "C" int b200t5_test_decoder_cross_attn(int device, const void* q, const v
       static_cast<const act_t*>(q), static_cast<const act_t*>(kv), static_cast<act_t*>(ctx), nullptr, key_ok, extent, B, T, S, H);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "decoder_cross_attn: %s", cudaGetErrorString(e));
+  return B200T5_OK;
+}
+
+extern "C" int b200t5_test_decoder_cross_attn_packed(int device, const void* q, const void* kv, void* ctx, const uint8_t* key_ok,
+                                                     const int32_t* extent, const int32_t* qoff, int B, int S, int H, void* stream) {
+  const int sms = hook_device(device);
+  if (sms < 0) return sms;
+  if (!q || !kv || !ctx || !key_ok || !extent || !qoff || B < 1 || H < 1 || S < 1 || B * H > 65535 ||
+      encoder_attn_smem_bytes(S) > 96 * 1024)
+    return fail(nullptr, B200T5_EINVAL, "decoder_cross_attn_packed: bad argument");
+  // the grid spans the longest prompt's query tiles: the offsets are read back
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  std::vector<int> h_off(B + 1);
+  cudaError_t e = cudaMemcpyAsync(h_off.data(), qoff, (B + 1) * sizeof(int), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "decoder_cross_attn_packed: %s", cudaGetErrorString(e));
+  int tiles = 0;
+  for (int b = 0; b < B; ++b) {
+    if (h_off[b + 1] < h_off[b]) return fail(nullptr, B200T5_EINVAL, "decoder_cross_attn_packed: offsets decrease at %d", b);
+    tiles = std::max(tiles, (h_off[b + 1] - h_off[b] + kEncQ - 1) / kEncQ);
+  }
+  if (tiles == 0) return B200T5_OK;
+  decoder_cross_packed_kernel<<<dim3(tiles, B * H), kEncThreads, encoder_attn_smem_bytes(S), st>>>(
+      static_cast<const act_t*>(q), static_cast<const act_t*>(kv), static_cast<act_t*>(ctx), key_ok, extent, qoff, B, S, H);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "decoder_cross_attn_packed: %s", cudaGetErrorString(e));
   return B200T5_OK;
 }
 

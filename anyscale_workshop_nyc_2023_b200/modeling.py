@@ -260,6 +260,88 @@ def score_labels(labels, vocab_size: int) -> np.ndarray:
     return lab
 
 
+class ChoiceScores:
+    """`score_choices(...)`, also readable by key: `.token_logprobs` fp32 [B, Cmax, L] (log p(candidate token | prompt,
+    earlier tokens), 0 past a candidate's end and for absent candidates), `.lengths` int32 [B, Cmax] (0 when absent),
+    `.logprobs` fp32 [B, Cmax] (each candidate's log-likelihood, summed in double; -inf when absent) and `.best` int64 [B]
+    (the argmax of logprobs, or of logprobs / lengths with normalize=True; ties to the lowest index)."""
+
+    def __init__(self, token_logprobs, lengths, logprobs, best):
+        self.token_logprobs = token_logprobs
+        self.lengths = lengths
+        self.logprobs = logprobs
+        self.best = best
+
+    def __getitem__(self, key):
+        return getattr(self, key)
+
+
+def choice_targets(choices, batch: int, vocab_size: int):
+    """The candidates of score_choices as decoder targets: (labels int64 [R, L], -100 after a candidate's last token;
+    counts int64 [batch], candidates per prompt; R = counts.sum(), prompt b's candidates the rows after those of prompts
+    0 .. b-1). `choices` is [C, L] or a list of C token-id lists (the same candidates for every prompt), [batch, C, L], or
+    a list of `batch` lists of token-id lists (ragged: C_b >= 1 each). Array forms pad with -100; the rules of
+    score_labels apply (ValueError)."""
+    if isinstance(choices, torch.Tensor):
+        choices = choices.detach().cpu().numpy()
+    if isinstance(choices, np.ndarray):
+        lab = np.ascontiguousarray(choices)
+        if lab.ndim == 2:
+            counts = np.full(batch, lab.shape[0], np.int64)
+            lab = np.tile(lab, (batch, 1))
+        elif lab.ndim == 3:
+            if lab.shape[0] != batch:
+                raise ValueError(f"choices [B, C, L] must have B = {batch} prompts, got {lab.shape}")
+            counts = np.full(batch, lab.shape[1], np.int64)
+            lab = lab.reshape(-1, lab.shape[2])
+        else:
+            raise ValueError(f"choices must be [C, L] or [batch, C, L], got {lab.shape}")
+        if lab.shape[0] == 0:
+            raise ValueError("choices holds no candidate")
+        return score_labels(lab, vocab_size), counts
+    if not isinstance(choices, (list, tuple)) or len(choices) == 0:
+        raise ValueError("choices must be an array or a non-empty list")
+    ragged = isinstance(choices[0], (list, tuple)) and len(choices[0]) > 0 and isinstance(choices[0][0], (list, tuple, np.ndarray, torch.Tensor))
+    groups = choices if ragged else [choices] * batch
+    if ragged and len(groups) != batch:
+        raise ValueError(f"ragged choices need one list of candidates per prompt: {batch} prompts, {len(groups)} lists")
+    cands = []
+    for g in groups:
+        if not isinstance(g, (list, tuple)) or len(g) == 0:
+            raise ValueError("every prompt needs at least one candidate")
+        for c in g:
+            ids = c.tolist() if isinstance(c, (np.ndarray, torch.Tensor)) else c
+            if not isinstance(ids, (list, tuple)) or len(ids) == 0 or not all(isinstance(t, (int, np.integer)) for t in ids):
+                raise ValueError(f"a candidate must be a non-empty list of token ids, got {c!r}")
+            if any(t < 0 or t >= vocab_size for t in ids):
+                raise ValueError(f"candidate {list(ids)} contains ids outside [0, {vocab_size})")
+            cands.append(ids)
+    lab = np.full((len(cands), max(len(c) for c in cands)), -100, np.int64)
+    for r, c in enumerate(cands):
+        lab[r, :len(c)] = c
+    return lab, np.array([len(g) for g in groups], np.int64)
+
+
+def choice_scores(token_logprobs: torch.Tensor, labels: np.ndarray, counts: np.ndarray, normalize: bool = False) -> ChoiceScores:
+    """ChoiceScores from the rows of score_choices: token_logprobs fp32 [R, L] and labels [R, L] of the R candidate rows,
+    counts [B] candidates per prompt (choice_targets)."""
+    B, R, L = len(counts), labels.shape[0], labels.shape[1]
+    Cmax = int(counts.max())
+    dev = token_logprobs.device
+    off = np.concatenate([[0], np.cumsum(counts)])
+    b_of = np.repeat(np.arange(B), counts)
+    c_of = np.arange(R) - off[b_of]
+    bi, ci = torch.from_numpy(b_of).to(dev), torch.from_numpy(c_of).to(dev)
+    tlp = torch.zeros((B, Cmax, L), dtype=torch.float32, device=dev)
+    tlp[bi, ci] = token_logprobs
+    lengths = torch.zeros((B, Cmax), dtype=torch.int32, device=dev)
+    lengths[bi, ci] = torch.from_numpy((labels != -100).sum(1).astype(np.int32)).to(dev)
+    present = lengths > 0
+    lp = torch.where(present, tlp.double().sum(-1).float(), torch.full((B, Cmax), float("-inf"), device=dev))
+    key = torch.where(present, lp / lengths.clamp(min=1).float(), lp) if normalize else lp
+    return ChoiceScores(tlp, lengths, lp, torch.argmax(key, dim=1))
+
+
 def _chk(model, rc: int, handle=None) -> None:
     _lib.check(rc, handle, model._lib)
 
@@ -638,6 +720,48 @@ class B200T5ForConditionalGeneration:
         return ForwardOutput(loss=loss, logits=logits, token_logprobs=logp)
 
     __call__ = forward
+
+    @torch.no_grad()
+    def score_choices(self, input_ids, attention_mask=None, choices=None, normalize: bool = False) -> ChoiceScores:
+        """Rank classification: every prompt's candidate answers scored as targets from one encoder pass per prompt
+        (b200t5_forward_choices). `choices`: [C, L] or a list of C token-id lists (the same candidates for every
+        prompt), [B, C, L], or a list of B lists of token-id lists (prompt b has its own C_b >= 1 candidates); array
+        forms pad a candidate with -100 after its last token (choice_targets). Each candidate is a target exactly as
+        `labels` are in forward, so row for row `token_logprobs` equals forward's on the prompt repeated once per
+        candidate, bit for bit. Returns a ChoiceScores; `.best` ranks by log-likelihood, or by its mean per token with
+        normalize=True. Batches run in chunks of at most pool_size prompts and a bounded number of candidate rows (a
+        prompt's candidates may be split across chunks); results do not depend on the chunking."""
+        ids = torch.as_tensor(input_ids).to(self._device, torch.long).contiguous()
+        if ids.dim() != 2:
+            raise ValueError(f"input_ids must be [batch, seq], got {tuple(ids.shape)}")
+        mask = None if attention_mask is None else torch.as_tensor(attention_mask).to(self._device, torch.long).contiguous()
+        self._check_inputs(ids, mask)
+        if choices is None:
+            raise ValueError("choices is required")
+        B, S = ids.shape
+        lab, counts = choice_targets(choices, B, self.config.vocab_size)
+        R, L = lab.shape
+        off = np.concatenate([[0], np.cumsum(counts)])
+        b_of = np.repeat(np.arange(B), counts)
+        # decoder rows per call: no larger a workspace than forward's pool_size rows, and the causal self-attention's
+        # grid of rows * num_heads <= 65535
+        max_rows = max(1, min(self.pool_size * max(S, L) // L, 65535 // self.config.num_heads))
+        lab_dev = torch.from_numpy(lab).to(self._device)
+        logp = torch.empty((R, L), dtype=torch.float32, device=self._device)
+        with torch.cuda.device(self._index):
+            stream = torch.cuda.current_stream(self._device)
+            r0 = 0
+            while r0 < R:
+                b0 = int(b_of[r0])
+                r1 = min(R, r0 + max_rows, int(off[min(B, b0 + self.pool_size)]))
+                b1 = int(b_of[r1 - 1]) + 1
+                offs = np.ascontiguousarray(np.clip(off[b0:b1 + 1], r0, r1) - r0, dtype=np.int32)
+                io = _lib.ForwardIO(logits=None, token_logprobs=logp[r0:r1].data_ptr())
+                _chk(self, self._lib.b200t5_forward_choices(self._h, _ptr(ids[b0:b1]), _ptr(None if mask is None else mask[b0:b1]),
+                                                            b1 - b0, S, offs.ctypes.data_as(C.c_void_p), _ptr(lab_dev[r0:r1]), L,
+                                                            C.byref(io), C.c_void_p(stream.cuda_stream)), self._h)
+                r0 = r1
+        return choice_scores(logp, lab, counts, normalize)
 
     def _run_scored(self, host: torch.Tensor, attention_mask, gp, lp, labels: Optional[np.ndarray]):
         """generate's routing (static batch, slot pool, static chunks) for a scored call: (sequences [B, 1+T'],

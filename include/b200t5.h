@@ -281,6 +281,19 @@ typedef struct b200t5_forward_io {
 int b200t5_forward(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
                    const int64_t* decoder_input_ids, const int64_t* labels, int T, const b200t5_forward_io* io,
                    void* stream);
+/* Multiple-choice scoring (rank classification): b200t5_forward over R (prompt, candidate) rows whose prompts are shared.
+ * The encoder and the cross-attention K/V projection run over the B prompts only; the decoder runs R*T rows, the
+ * candidates of prompt b being rows row_offsets[b] .. row_offsets[b+1]-1, and each prompt's cross-attention runs all
+ * its candidates' queries as one sequence against its keys (csrc/attention_decoder.cuh: decoder_cross_packed_kernel).
+ * Every row gets the bits b200t5_forward gives it with that row's prompt repeated in its own row.
+ * row_offsets is a HOST int32 [B+1] array: 0 first, strictly increasing, R = row_offsets[B]. labels int64 [R,T] (device)
+ * as b200t5_forward's labels; the decoder input is transformers' _shift_right(labels). io: logits [R, T, vocab] and/or
+ * token_logprobs [R, T]. b200t5_get_stats' encoder_flops then counts the B prompts once each. NULL pointers, offsets
+ * that do not start at 0 or do not increase, R*num_heads > 65535, labels out of range or T outside [1, 4096] return
+ * B200T5_EINVAL before anything is enqueued. */
+int b200t5_forward_choices(b200t5_handle h, const int64_t* input_ids, const int64_t* attention_mask, int B, int S,
+                           const int32_t* row_offsets, const int64_t* labels, int T, const b200t5_forward_io* io,
+                           void* stream);
 
 /* ---- measurement hooks (bench.py) --------------------------------------------------- */
 /* Times the cross-attention decode kernel alone over the cross-KV arena of the last generate call, in launches of
@@ -426,6 +439,10 @@ int b200t5_test_decoder_self_attn(int device, const void* qkv, void* ctx, const 
                                   void* stream);
 int b200t5_test_decoder_cross_attn(int device, const void* q, const void* kv, void* ctx, const uint8_t* key_ok,
                                    const int32_t* extent, int B, int T, int S, int H, void* stream);
+/* The cross-attention of b200t5_forward_choices: q [qoff[B], H*64], prompt b's queries the rows qoff[b] .. qoff[b+1]-1
+ * (qoff: DEVICE int32 [B+1], non-decreasing; read back for the grid), kv / key_ok / extent as above, ctx rows as q. */
+int b200t5_test_decoder_cross_attn_packed(int device, const void* q, const void* kv, void* ctx, const uint8_t* key_ok,
+                                          const int32_t* extent, const int32_t* qoff, int B, int S, int H, void* stream);
 /* out[i] = act(gelu_new(gate[i]) * up[i]). mode 0: exactly the GeGLU epilogue's function (bf16 build: the exhaustive
  * gelu table; fp16 build: the op-by-op fp16 arithmetic with single-rounded pow); mode 2: the op-by-op arithmetic with
  * double-rounded pow (x*x*x in act_t); mode 1: same with single-rounded pow. */
