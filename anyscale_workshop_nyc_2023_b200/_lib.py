@@ -175,6 +175,7 @@ SIGNATURES = {
     "b200t5_test_gemm_splitk": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
     "b200t5_test_ffo": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "b200t5_test_rmsnorm": (_i, [_i, _vp, _vp, _vp, _i, _i, C.c_float, _vp]),
+    "b200t5_test_rmsnorm_scaled": (_i, [_i, _vp, _vp, _vp, _i, _i, C.c_float, C.c_float, _vp]),
     "b200t5_test_attn_decode": (_i, [_i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "b200t5_test_encoder_attn": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b200t5_test_decoder_self_attn": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _vp]),

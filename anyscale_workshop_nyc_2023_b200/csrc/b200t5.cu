@@ -154,6 +154,8 @@ struct Cfg {
   int V, d, F, H, I, Le, Ld, nb, maxdist;
   float eps;
   int pad, eos, start;
+  bool gated;       // feed-forward: gated-GELU (T5 v1.1 / FLAN-T5), else ReLU (T5 v1.0)
+  float out_scale;  // scale_decoder_outputs: fp32(d_model ** -0.5) after the final decoder norm; 0 = none
 };
 
 struct DevBuf {
@@ -559,11 +561,17 @@ static cudaError_t run_ffo_sk(b200t5_ctx* h, const b200t5_ctx::SkChoice& ch, con
   return launch_gemm_splitk<64, EpiResidual, tf>(tmA, tmB, M, N, h->ffo_k, split, ep, s, pdl, akb, h->sk_stages64);
 }
 
+// scale != 0: the rescaled final decoder norm of a T5 v1.0 checkpoint (rmsnorm_scaled_kernel), same launch shape
 static cudaError_t run_rmsnorm(b200t5_ctx* h, const res_t* x, const act_t* w, act_t* y, int M, int d, float eps,
-                               cudaStream_t s, bool pdl = false) {
+                               cudaStream_t s, bool pdl = false, float scale = 0.f) {
   if (h) h->launches++;
   const int wpb = 8;
   const int grid = (M + wpb - 1) / wpb;
+  if (scale != 0.f) {
+    if (d <= 1024) return launch_kernel(rmsnorm_scaled_kernel<4>, dim3(grid), dim3(wpb * 32), 0, s, pdl, x, w, y, M, d, eps, scale);
+    if (d <= 4096) return launch_kernel(rmsnorm_scaled_kernel<16>, dim3(grid), dim3(wpb * 32), 0, s, pdl, x, w, y, M, d, eps, scale);
+    return cudaErrorInvalidValue;
+  }
   if (d <= 1024) return launch_kernel(rmsnorm_kernel<4>, dim3(grid), dim3(wpb * 32), 0, s, pdl, x, w, y, M, d, eps);
   if (d <= 4096) return launch_kernel(rmsnorm_kernel<16>, dim3(grid), dim3(wpb * 32), 0, s, pdl, x, w, y, M, d, eps);
   return cudaErrorInvalidValue;
@@ -593,6 +601,12 @@ static cudaError_t init_kernel_attrs() {
   if ((e = prepare_gemm_splitk<128, EpiResidual, B200T5_F16 != 0>()) != cudaSuccess) return e;
   // the teacher-forced forward pass (b200t5_forward): the GeGLU product on the decode packing, the lm_head variants
   if ((e = prepare_gemm<128, EpiGegluNarrow>()) != cudaSuccess) return e;
+  // the ReLU feed-forward of T5 v1.0 checkpoints, in the encoder, the decode step and the forward pass
+  if ((e = prepare_gemm_2cta<EpiRelu>()) != cudaSuccess) return e;
+  if ((e = prepare_gemm_enc_ws<EpiRelu>()) != cudaSuccess) return e;
+  if ((e = prepare_gemm_splitk<64, EpiRelu>()) != cudaSuccess) return e;
+  if ((e = prepare_gemm_splitk<128, EpiRelu>()) != cudaSuccess) return e;
+  if ((e = prepare_gemm<128, EpiRelu>()) != cudaSuccess) return e;
   if ((e = prepare_gemm<128, EpiLmLogits<false>>()) != cudaSuccess) return e;
   if ((e = prepare_gemm<128, EpiLmLogits<true>>()) != cudaSuccess) return e;
   if ((e = cudaFuncSetAttribute(decoder_attn_kernel<kAttnCausal>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024)) != cudaSuccess)
@@ -666,8 +680,10 @@ extern "C" int b200t5_create(const b200t5_config* cfg, int device, b200t5_handle
   if (!cfg || !out) return fail(nullptr, B200T5_EINVAL, "null argument");
   *out = nullptr;
   if (cfg->d_kv != 64) return fail(nullptr, B200T5_EINVAL, "d_kv=%d unsupported (kernels are specialised for 64)", cfg->d_kv);
-  if (!cfg->is_gated_gelu) return fail(nullptr, B200T5_EINVAL, "only feed_forward_proj='gated-gelu' (T5 v1.1 / FLAN-T5) is supported");
-  if (cfg->scale_decoder_outputs) return fail(nullptr, B200T5_EINVAL, "scale_decoder_outputs (tied-embedding T5 v1.0) is not supported");
+  if (cfg->is_gated_gelu != 0 && cfg->is_gated_gelu != 1)
+    return fail(nullptr, B200T5_EINVAL, "is_gated_gelu=%d: 1 = feed_forward_proj 'gated-gelu', 0 = 'relu'", cfg->is_gated_gelu);
+  if (cfg->scale_decoder_outputs != 0 && cfg->scale_decoder_outputs != 1)
+    return fail(nullptr, B200T5_EINVAL, "scale_decoder_outputs=%d: must be 0 or 1", cfg->scale_decoder_outputs);
   if (cfg->d_model % 8 || cfg->d_ff % 32 || cfg->d_model > 4096 || cfg->vocab_size < 2 || cfg->num_heads < 1 ||
       cfg->num_layers < 1 || cfg->num_decoder_layers < 1)
     return fail(nullptr, B200T5_EINVAL, "unsupported shape: d_model=%d d_ff=%d vocab=%d", cfg->d_model, cfg->d_ff, cfg->vocab_size);
@@ -677,7 +693,10 @@ extern "C" int b200t5_create(const b200t5_config* cfg, int device, b200t5_handle
   if (!h) return fail(nullptr, B200T5_ENOMEM, "out of host memory");
   h->c = Cfg{cfg->vocab_size, cfg->d_model, cfg->d_ff, cfg->num_heads, cfg->num_heads * 64, cfg->num_layers,
              cfg->num_decoder_layers, cfg->relative_attention_num_buckets, cfg->relative_attention_max_distance,
-             cfg->layer_norm_epsilon, cfg->pad_token_id, cfg->eos_token_id, cfg->decoder_start_token_id};
+             cfg->layer_norm_epsilon, cfg->pad_token_id, cfg->eos_token_id, cfg->decoder_start_token_id,
+             cfg->is_gated_gelu == 1,
+             // transformers: sequence_output * (self.model_dim ** -0.5), a Python float taken as fp32 by the multiply
+             cfg->scale_decoder_outputs ? static_cast<float>(pow(static_cast<double>(cfg->d_model), -0.5)) : 0.f};
   h->device = device;
   h->num_sms = sms;
   h->enc.resize(h->c.Le);
@@ -872,6 +891,25 @@ static int clone_buf(b200t5_ctx* h, DevBuf& dst, const act_t* src, size_t n) {
   return B200T5_OK;
 }
 
+// The feed-forward input weight(s) of one layer (`prefix` = "<side>.block.<l>.layer.<k>.DenseReluDense.") as the GEMMs
+// with N-tiles of bn rows read them. Gated-GELU: wi_0 and wi_1 interleaved per tile (interleave_geglu), rows_out =
+// the padded row count. ReLU (T5 v1.0): wi [F, d] as is, which every tile width reads in place (the tensor map's
+// out-of-bounds rows load as zeros and no store reaches past F), rows_out = F.
+static int pack_wi(b200t5_ctx* h, const std::string& prefix, DevBuf& dst, int bn, int* rows_out) {
+  const int F = h->c.F, d = h->c.d;
+  int rc = B200T5_OK;
+  if (!h->c.gated) {
+    const act_t* wi = take(h, prefix + "wi.weight", F, d, &rc);
+    if (!wi) return rc;
+    *rows_out = F;
+    return clone_buf(h, dst, wi, static_cast<size_t>(F) * d);
+  }
+  const act_t* wi0 = take(h, prefix + "wi_0.weight", F, d, &rc);
+  const act_t* wi1 = wi0 ? take(h, prefix + "wi_1.weight", F, d, &rc) : nullptr;
+  if (!wi1) return rc;
+  return interleave_geglu(h, wi0, wi1, dst, F, d, bn, rows_out);
+}
+
 #define TRY(expr)            \
   do {                       \
     int _rc = (expr);        \
@@ -943,11 +981,8 @@ extern "C" int b200t5_finalize(b200t5_handle h) {
     CU_OK(h, cudaMemcpy(w.wqkv.as<act_t>() + 2 * blk, v, blk * 2, cudaMemcpyDeviceToDevice));
     if (!(p = take(h, key("layer.0.SelfAttention.o.weight"), d, I, &rc))) return rc;
     TRY(clone_buf(h, w.wo, p, static_cast<size_t>(d) * I));
-    const act_t* wi0 = take(h, key("layer.1.DenseReluDense.wi_0.weight"), F, d, &rc);
-    const act_t* wi1 = wi0 ? take(h, key("layer.1.DenseReluDense.wi_1.weight"), F, d, &rc) : nullptr;
-    if (!wi1) return rc;
     int wi_rows = 0;
-    TRY(interleave_geglu(h, wi0, wi1, w.wi, F, d, 256, &wi_rows));
+    TRY(pack_wi(h, key("layer.1.DenseReluDense."), w.wi, 256, &wi_rows));
     if (!(p = take(h, key("layer.1.DenseReluDense.wo.weight"), d, F, &rc))) return rc;
     TRY(build_ffo(h, w.wff_o, key("layer.1.DenseReluDense.wo.weight"), p, d, F, &h->ffo_k));
     TMAP(h, &w.tm_qkv, w.wqkv.p, 3 * I, d, k2ctaBox);
@@ -989,13 +1024,10 @@ extern "C" int b200t5_finalize(b200t5_handle h) {
     CU_OK(h, cudaMemcpy(h->wcrosskv.as<act_t>() + (static_cast<size_t>(l) * 2 + 1) * blk, cv, blk * 2, cudaMemcpyDeviceToDevice));
     if (!(p = take(h, key("layer.1.EncDecAttention.o.weight"), d, I, &rc))) return rc;
     TRY(clone_buf(h, w.wco, p, static_cast<size_t>(d) * I));
-    const act_t* wi0 = take(h, key("layer.2.DenseReluDense.wi_0.weight"), F, d, &rc);
-    const act_t* wi1 = wi0 ? take(h, key("layer.2.DenseReluDense.wi_1.weight"), F, d, &rc) : nullptr;
-    if (!wi1) return rc;
     int wi_rows = 0;
     // TMA box rows = the N-tile of the split-K kernel that will read the weight
     const int bn_qkv = h->sk_qkv.bn, bn_proj = h->sk_proj.bn, bn_wi = h->sk_wi.bn, bn_ffo = h->sk_ffo.bn;
-    TRY(interleave_geglu(h, wi0, wi1, w.wi, F, d, bn_wi, &wi_rows));
+    TRY(pack_wi(h, key("layer.2.DenseReluDense."), w.wi, bn_wi, &wi_rows));
     w.wi_rows = wi_rows;
     if (!(p = take(h, key("layer.2.DenseReluDense.wo.weight"), d, F, &rc))) return rc;
     TRY(build_ffo(h, w.wff_o, key("layer.2.DenseReluDense.wo.weight"), p, d, F, &h->ffo_k));
@@ -1186,9 +1218,11 @@ static int run_encoder(b200t5_ctx* h, const long long* ids, const long long* mas
       CU_OK(h, run_gemm_2cta<EpiResidual>(h, p.tm_ctx, w.tm_o, M, d, I, ep, s));
     }
     CU_OK(h, run_rmsnorm(h, p.x.as<res_t>(), w.ln1.as<act_t>(), p.xn.as<act_t>(), M, d, c.eps, s));
-    {
+    if (c.gated) {
       EpiGeglu::Params ep{p.hff.as<ffh_t>(), F, h->gelu_lut};
       CU_OK(h, run_gemm_2cta<EpiGeglu>(h, p.tm_xn, w.tm_wi, M, wi_tiles * 256, d, ep, s));
+    } else {
+      CU_OK(h, run_gemm_2cta<EpiRelu>(h, p.tm_xn, w.tm_wi, M, F, d, EpiRelu::Params{p.hff.as<ffh_t>(), F}, s));
     }
     {
       EpiResidual::Params ep{p.x.as<res_t>(), p.x.as<res_t>(), d};
@@ -1318,9 +1352,11 @@ static int chain_layer_post(b200t5_ctx* h, cudaStream_t s, const ChainView& v, i
     CU_OK(h, run_gemm_sk<EpiResidual>(h, h->sk_proj, v.ch->tm_dctx, w.tm_co, v.nb, d, I, ep, s, pdl));
   }
   CU_OK(h, run_rmsnorm(h, v.dx, w.ln2.as<act_t>(), v.dxn, v.nb, d, c.eps, s, pdl));
-  {
+  if (c.gated) {
     EpiGeglu::Params ep{v.dh, F, h->gelu_lut};
     CU_OK(h, run_gemm_sk<EpiGeglu>(h, h->sk_wi, v.ch->tm_dxn, w.tm_wi, v.nb, w.wi_rows, d, ep, s, pdl));
+  } else {
+    CU_OK(h, run_gemm_sk<EpiRelu>(h, h->sk_wi, v.ch->tm_dxn, w.tm_wi, v.nb, F, d, EpiRelu::Params{v.dh, F}, s, pdl));
   }
   {
     EpiResidual::Params ep{v.dx, v.dx, d};
@@ -1338,7 +1374,7 @@ static int chain_head(b200t5_ctx* h, cudaStream_t s, const ChainView& v, float* 
   const StepMode& m = p.mode;
   const int d = c.d, T = p.Tmax;
   const bool pdl = h->use_pdl;
-  CU_OK(h, run_rmsnorm(h, v.dx, h->dec_final_ln.as<act_t>(), v.dxn, v.nb, d, c.eps, s, pdl));
+  CU_OK(h, run_rmsnorm(h, v.dx, h->dec_final_ln.as<act_t>(), v.dxn, v.nb, d, c.eps, s, pdl, c.out_scale));
   if (logits_out) {
     EpiStoreF32::Params ep{logits_out + static_cast<size_t>(v.b0) * ldl, ldl};
     h->launches++;
@@ -1648,7 +1684,10 @@ static void fill_stats_model(b200t5_ctx* h, int steps) {
   const Plan& p = *h->plan;
   // SURVEY 8(d): weights once per step + cross-KV + self-KV read/write, bf16.
   // (element count; the fp16 build's `wo` weights are fp32: counted twice)
-  const double wstep = static_cast<double>(c.Ld) * (6.0 * c.d * c.I + (B200T5_F16 ? 4.0 : 3.0) * c.d * c.F) + static_cast<double>(c.V) * c.d;
+  // feed-forward F x d matrices per layer: wi_0, wi_1, wo (gated-GELU) or wi, wo (ReLU)
+  const double ff_mats = c.gated ? 3.0 : 2.0;
+  const double wstep = static_cast<double>(c.Ld) * (6.0 * c.d * c.I + (ff_mats + (B200T5_F16 ? 1.0 : 0.0)) * c.d * c.F) +
+                       static_cast<double>(c.V) * c.d;
   std::vector<int> ext(p.B, p.S);
   if (cudaMemcpy(ext.data(), p.extent.p, p.B * 4, cudaMemcpyDeviceToHost) != cudaSuccess)
     ext.assign(p.B, p.S);  // statistics only: fall back to the padded length
@@ -1663,7 +1702,7 @@ static void fill_stats_model(b200t5_ctx* h, int steps) {
   // prompts this is SURVEY 8(d)'s figure, for padded ones it is the work the packed encoder actually does
   double sum_s2 = 0;
   for (int v : ext) sum_s2 += static_cast<double>(v) * v;
-  h->last_enc_flops = 2.0 * c.Le * (4.0 * c.d * c.I + 3.0 * c.d * c.F) * sum_s + c.Le * 4.0 * sum_s2 * c.I +
+  h->last_enc_flops = 2.0 * c.Le * (4.0 * c.d * c.I + ff_mats * c.d * c.F) * sum_s + c.Le * 4.0 * sum_s2 * c.I +
                       2.0 * c.Ld * 2.0 * c.d * c.I * sum_s;
 }
 
@@ -2423,8 +2462,10 @@ extern "C" int b200t5_decode_logits(b200t5_handle h, const int64_t* input_ids, c
 // ================================================================== teacher-forced forward pass
 // The forward pass's GeGLU product: the decoder's wi is interleaved per 128-row tile for the split-K decode GEMM, so its
 // B*T-row product runs 128 x 128 tiles that read that packing (the encoder's 128 x 256 tiles would need a second copy).
+// A ReLU model's wi runs the same tiles through the same 128-row boxes with EpiRelu.
 static cudaError_t run_geglu_fwd(b200t5_ctx* h, const CUtensorMap& tmA, const DecLayerW& w, int M, const EpiGeglu::Params& ep, cudaStream_t s) {
   h->launches++;
+  if (!h->c.gated) return launch_gemm<128, EpiRelu>(tmA, w.tm_wi, M, h->c.F, h->c.d, 0, EpiRelu::Params{ep.out, ep.F}, h->num_sms, s);
   return launch_gemm<128, EpiGegluNarrow>(tmA, w.tm_wi, M, w.wi_rows, h->c.d, 0, ep, h->num_sms, s);
 }
 
@@ -2493,12 +2534,12 @@ static int run_decoder_forward(b200t5_ctx* h, int T, cudaStream_t s, bool prefil
       CU_OK(h, run_ffo_2cta(h, p.tm_hff, w.tm2_ffo, M, d, ep, s));
     }
   }
-  CU_OK(h, run_rmsnorm(h, x, h->dec_final_ln.as<act_t>(), xn, M, d, c.eps, s));
+  CU_OK(h, run_rmsnorm(h, x, h->dec_final_ln.as<act_t>(), xn, M, d, c.eps, s, false, c.out_scale));
   return B200T5_OK;
 }
 
 // run_decoder_forward's GeGLU product (run_geglu_fwd) reads wi in the decode step's packing through 128-row boxes: it
-// needs the default 128-row wi tile of the split-K decode GEMM. Checked before anything is launched.
+// needs the default 128-row wi tile of the split-K decode GEMM (the tensor map's box, for a ReLU model too). Checked before anything is launched.
 static int check_forward_wi(b200t5_ctx* h, const char* who) {
   if (h->sk_wi.bn != 128)
     return fail(h, B200T5_EINVAL, "%s: needs the feed-forward wi packed in 128-row tiles, but B200T5_SK set the wi tile to %d rows "
@@ -2852,10 +2893,10 @@ extern "C" int b200t5_test_gemm(int device, const void* A, const void* W, void* 
   if (sms < 0) return sms;
   if (K % 8) return fail(nullptr, B200T5_EINVAL, "K must be a multiple of 8");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  // bn 512: the encoder configuration (128 x 256 tiles, weight loaded in 128-row boxes, gemm_2cta.cuh), modes 0/1/2/5;
-  // bn 128: the fp32 logits of b200t5_decode_logits, mode 3
-  if (!((bn == 512 && (mode == 0 || mode == 1 || mode == 2 || mode == 5)) || (bn == 128 && mode == 3)))
-    return fail(nullptr, B200T5_EINVAL, "test_gemm: bn=512 with mode 0/1/2/5, or bn=128 with mode 3");
+  // bn 512: the encoder configuration (128 x 256 tiles, weight loaded in 128-row boxes, gemm_2cta.cuh), modes 0/1/2/5/6;
+  // bn 128: the fp32 logits of b200t5_decode_logits, mode 3, or the forward pass's ReLU product (128 x 128 tiles), mode 6
+  if (!((bn == 512 && (mode == 0 || mode == 1 || mode == 2 || mode == 5 || mode == 6)) || (bn == 128 && (mode == 3 || mode == 6))))
+    return fail(nullptr, B200T5_EINVAL, "test_gemm: bn=512 with mode 0/1/2/5/6, or bn=128 with mode 3/6");
   CUtensorMap ta, tb;
   if (!make_tmap(&ta, A, M, K, 128) || !make_tmap(&tb, W, N, K, 128)) return fail(nullptr, B200T5_ECUDA, "%s", g_err);
   b200t5_ctx dummy;
@@ -2873,6 +2914,9 @@ extern "C" int b200t5_test_gemm(int device, const void* A, const void* W, void* 
     if (lrc != B200T5_OK) return lrc;
     EpiGeglu::Params ep{static_cast<ffh_t*>(C), N / 2, lut};
     e = run_gemm_2cta<EpiGeglu>(&dummy, ta, tb, M, N, K, ep, s);
+  } else if (mode == 6) {
+    const EpiRelu::Params ep{static_cast<ffh_t*>(C), N};
+    e = bn == 512 ? run_gemm_2cta<EpiRelu>(&dummy, ta, tb, M, N, K, ep, s) : launch_gemm<128, EpiRelu>(ta, tb, M, N, K, 0, ep, sms, s);
   } else {
     EpiStoreF32::Params ep{static_cast<float*>(C), N};
     e = launch_gemm<128, EpiStoreF32>(ta, tb, M, N, K, 1, ep, sms, s);
@@ -2913,6 +2957,8 @@ extern "C" int b200t5_test_enc_gemm(int device, const void* A, const void* W, vo
   } else if (mode == 3) {
     EpiCrossKV::Params ep{Cb, B, H, S, row_b, row_s};
     e = run_gemm_2cta<EpiCrossKV>(&dummy, ta, tb, M, N, K, ep, s);
+  } else if (mode == 6) {
+    e = run_gemm_2cta<EpiRelu>(&dummy, ta, tb, M, N, K, EpiRelu::Params{static_cast<ffh_t*>(C), N}, s);
   }
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_enc_gemm(kernel=%d, mode=%d): %s", kernel, mode, cudaGetErrorString(e));
   return B200T5_OK;
@@ -3066,6 +3112,8 @@ extern "C" int b200t5_test_gemm_splitk(int device, const void* A, const void* W,
     EpiQkvDecode::Params ep{Cb, static_cast<act_t*>(aux), &st.as<DecodeState>()->step, M, N / 192, Tmax};
     e = run_gemm_sk<EpiQkvDecode>(&dummy, ch, ta, tb, M, N, K, ep, s, false);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  } else if (mode == 6) {
+    e = run_gemm_sk<EpiRelu>(&dummy, ch, ta, tb, M, N, K, EpiRelu::Params{static_cast<ffh_t*>(C), N}, s, false);
   }
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "test_gemm_splitk(bn=%d, split=%d, mode=%d): %s", bn, split, mode, cudaGetErrorString(e));
   return B200T5_OK;
@@ -3239,6 +3287,17 @@ extern "C" int b200t5_test_rmsnorm(int device, const void* x, const void* w, voi
   if (sms < 0) return sms;
   cudaError_t e = run_rmsnorm(nullptr, static_cast<const res_t*>(x), static_cast<const act_t*>(w), static_cast<act_t*>(y), M, d, eps, static_cast<cudaStream_t>(stream));
   if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "rmsnorm: %s", cudaGetErrorString(e));
+  return B200T5_OK;
+}
+
+extern "C" int b200t5_test_rmsnorm_scaled(int device, const void* x, const void* w, void* y, int M, int d, float eps, float scale,
+                                          void* stream) {
+  const int sms = hook_device(device);
+  if (sms < 0) return sms;
+  if (!(scale != 0.f)) return fail(nullptr, B200T5_EINVAL, "test_rmsnorm_scaled: scale must be nonzero");
+  cudaError_t e = run_rmsnorm(nullptr, static_cast<const res_t*>(x), static_cast<const act_t*>(w), static_cast<act_t*>(y), M, d, eps,
+                              static_cast<cudaStream_t>(stream), false, scale);
+  if (e != cudaSuccess) return fail(nullptr, B200T5_ECUDA, "rmsnorm_scaled: %s", cudaGetErrorString(e));
   return B200T5_OK;
 }
 

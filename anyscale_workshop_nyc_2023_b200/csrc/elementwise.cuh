@@ -121,9 +121,12 @@ __global__ void unpack_rows_kernel(const act_t* __restrict__ xp, const int* __re
 //   y1  = bf16( float(x) * rsqrt(var + eps) )   first rounding
 //   y   = bf16( float(w) * float(y1) )          second rounding
 // One warp per row; the row stays in registers between the two passes.
-template <int kMaxVec>  // 8-element vectors per lane: d <= kMaxVec * 256
-__global__ void rmsnorm_kernel(const res_t* __restrict__ x, const act_t* __restrict__ w,
-                               act_t* __restrict__ y, int M, int d, float eps) {
+// kScaled: the final decoder norm of a T5 v1.0 checkpoint (scale_decoder_outputs, modeling_t5.py:1107-1108), whose
+// output is multiplied by scale = fp32(d_model ** -0.5) in fp32 and rounded once more:
+//   y   = act( float(act(w * y1)) * scale )
+template <int kMaxVec, bool kScaled>  // 8-element vectors per lane: d <= kMaxVec * 256
+DEVINL void rmsnorm_rows(const res_t* __restrict__ x, const act_t* __restrict__ w, act_t* __restrict__ y, int M, int d,
+                         float eps, float scale) {
   pdl_launch_dependents();
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = lane_id();
@@ -164,11 +167,24 @@ __global__ void rmsnorm_kernel(const res_t* __restrict__ x, const act_t* __restr
       for (int j = 0; j < 4; ++j) {
         const float a = act_round(v[i][2 * j] * inv);
         const float b = act_round(v[i][2 * j + 1] * inv);
-        o[j] = pack_act2(act_lo(ws[j]) * a, act_hi(ws[j]) * b);
+        if constexpr (kScaled)
+          o[j] = pack_act2(act_round(act_lo(ws[j]) * a) * scale, act_round(act_hi(ws[j]) * b) * scale);
+        else
+          o[j] = pack_act2(act_lo(ws[j]) * a, act_hi(ws[j]) * b);
       }
       yr[idx] = make_uint4(o[0], o[1], o[2], o[3]);
     }
   }
+}
+template <int kMaxVec>
+__global__ void rmsnorm_kernel(const res_t* __restrict__ x, const act_t* __restrict__ w, act_t* __restrict__ y, int M,
+                               int d, float eps) {
+  rmsnorm_rows<kMaxVec, false>(x, w, y, M, d, eps, 1.f);
+}
+template <int kMaxVec>
+__global__ void rmsnorm_scaled_kernel(const res_t* __restrict__ x, const act_t* __restrict__ w, act_t* __restrict__ y,
+                                      int M, int d, float eps, float scale) {
+  rmsnorm_rows<kMaxVec, true>(x, w, y, M, d, eps, scale);
 }
 
 // ---------------------------------------------------------------- attention-mask preparation

@@ -587,6 +587,42 @@ struct EpiGegluNarrow {
   }
 };
 
+// ---- ReLU feed-forward of T5 v1.0 (T5DenseActDense, modeling_t5.py:84-100): out = relu(act(acc)), the A operand of
+// `wo` in ffh_t (fp16 build: fp32 holding fp16 values, the cast up of transformers' forward). relu(act(x)) ==
+// act(relu(x)), so the one rounding point is transformers': the output of `wi`. `wi` is stored as is ([F, d], no
+// interleave), so N = F and the stores clip to it.
+struct EpiRelu {
+  struct Params {
+    ffh_t* out;  // [M, ld]
+    int ld;
+  };
+  static constexpr bool kPaired = false;
+  typedef NoPre ChunkPre;
+  static DEVINL void prologue(const Params&, uint8_t*, int, int = 128) {}
+  static DEVINL void chunk_pre(const Params&, int, int, int, ChunkPre&) {}
+  static DEVINL float relu(float x) { return x < 0.f ? 0.f : x; }  // NaN propagates, as torch.relu
+  static DEVINL void chunk(const Params& p, const uint32_t (&acc)[32], int m, int n0, int N, const uint8_t*,
+                           const ChunkPre&) {
+#if B200T5_F16
+    float o[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = relu(act_round(__uint_as_float(acc[i])));
+    store_row_chunk_f32(p.out + static_cast<size_t>(m) * p.ld + n0, o, n0, N);
+#else
+    uint32_t o[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+      o[i] = pack_act2(relu(act_round(__uint_as_float(acc[2 * i]))), relu(act_round(__uint_as_float(acc[2 * i + 1]))));
+    store_row_chunk(p.out + static_cast<size_t>(m) * p.ld + n0, o, n0, N);
+#endif
+  }
+  template <int BN>
+  static DEVINL void run(const Params& p, uint32_t taddr, int m, bool m_ok, int n_tile, int N, const uint8_t* es,
+                         int part, int parts) {
+    run_chunks<BN, EpiRelu>(p, taddr, m, m_ok, n_tile, N, es, part, parts);
+  }
+};
+
 // ---- cross-attention K/V projection for all decoder layers at once (X1):
 // row m = (b, s) of the encoder output; column n = ((layer*2 + kv)*H + h)*64 + d.
 // Written straight into the decode arena  [layer][kv][B][H][S][64].

@@ -350,13 +350,31 @@ def _ptr(t: Optional[torch.Tensor]):
     return C.c_void_p(t.data_ptr()) if t is not None else None
 
 
+def _is_gated_gelu(config: Dict[str, Any]) -> int:
+    """b200t5_config.is_gated_gelu for a config.json: 1 for feed_forward_proj "gated-gelu" (T5 v1.1 / FLAN-T5), 0 for
+    "relu" (T5 v1.0; transformers' default when the key is absent, as in the original t5-small / t5-base configs)."""
+    ffp = config.get("feed_forward_proj", "relu")
+    if ffp == "gated-gelu":
+        return 1
+    if ffp == "relu":
+        return 0
+    raise ValueError(f"feed_forward_proj={ffp!r} is not supported: the CUDA path runs 'gated-gelu' (T5 v1.1 / FLAN-T5) "
+                     "and 'relu' (T5 v1.0)")
+
+
 class B200T5ForConditionalGeneration:
-    """FLAN-T5 greedy generation on one H100. API subset of transformers.T5ForConditionalGeneration
-    that the workshop's predictor and notebook cells touch."""
+    """T5 generation, scoring and teacher-forced forward passes on one H100. API subset of
+    transformers.T5ForConditionalGeneration that the workshop's predictor and notebook cells touch.
+
+    Two T5 architectures load (d_kv 64): T5 v1.1 / FLAN-T5 (feed_forward_proj "gated-gelu", separate lm_head) and the
+    original T5 v1.0 - t5-small, t5-base, t5-large and their fine-tunes (feed_forward_proj "relu"; the lm_head is the
+    shared embedding when the checkpoint has none, and the decoder output is scaled by d_model ** -0.5 unless the
+    config says tie_word_embeddings: false, as in transformers). Any other feed_forward_proj raises ValueError."""
 
     main_input_name = "input_ids"
 
     def __init__(self, config: Dict[str, Any], device: torch.device, compute_dtype: torch.dtype = torch.bfloat16):
+        is_gated_gelu = _is_gated_gelu(config)  # before anything touches the device or the library
         if device.type != "cuda":
             raise RuntimeError("B200T5ForConditionalGeneration runs on an H100 only; there is no CPU fallback")
         if compute_dtype not in (torch.bfloat16, torch.float16):
@@ -373,7 +391,6 @@ class B200T5ForConditionalGeneration:
             pad_token_id=config.get("pad_token_id", 0),
             decoder_start_token_id=config.get("decoder_start_token_id", config.get("pad_token_id", 0)),
         )
-        ffp = config.get("feed_forward_proj", "gated-gelu")
         cfg = _lib.Config(
             vocab_size=config["vocab_size"], d_model=config["d_model"], d_kv=config["d_kv"], d_ff=config["d_ff"],
             num_heads=config["num_heads"], num_layers=config["num_layers"],
@@ -384,7 +401,7 @@ class B200T5ForConditionalGeneration:
             pad_token_id=self.generation_config.pad_token_id,
             eos_token_id=self.generation_config.eos_token_id,
             decoder_start_token_id=self.generation_config.decoder_start_token_id,
-            is_gated_gelu=1 if ffp == "gated-gelu" else 0,
+            is_gated_gelu=is_gated_gelu,
             # HF decides "scale decoder outputs" from tie_word_embeddings (configuration_t5.py:82)
             scale_decoder_outputs=0 if config.get("tie_word_embeddings", True) is False else 1,
         )
@@ -418,6 +435,8 @@ class B200T5ForConditionalGeneration:
         if not (path / "config.json").exists():
             raise FileNotFoundError(f"{path} is not a Hugging Face checkpoint directory (no config.json); "
                                     "hub downloads are not available offline")
+        config = json.loads((path / "config.json").read_text())
+        _is_gated_gelu(config)  # an unsupported architecture fails before the device is looked at
         want = dtype if dtype is not None else torch_dtype
         compute = torch.float16 if want in (torch.float16, "float16", "half") else torch.bfloat16
         if want not in (None, torch.bfloat16, "bfloat16", "auto", torch.float16, "float16", "half"):
@@ -435,7 +454,6 @@ class B200T5ForConditionalGeneration:
         if torch.device(device).type == "cuda" and torch.device(device).index is None:
             device = torch.device("cuda", torch.cuda.current_device())
         device = torch.device(device)
-        config = json.loads((path / "config.json").read_text())
         model = cls(config, device, compute)
         model._load_weights(path)
         return model

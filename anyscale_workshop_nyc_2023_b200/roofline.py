@@ -25,11 +25,16 @@ def peaks(root: Path) -> Tuple[float, float, str]:
     return H100_HBM_GBS, H100_BF16_TFLOPS, "H100 SXM data sheet (HBM3 3.35 TB/s, dense BF16 989 TFLOP/s at 700 W)"
 
 
+def ff_matrices(spec) -> int:
+    """d_ff x d_model matrices of one feed-forward block: wi_0, wi_1, wo (gated-GELU, FLAN-T5) or wi, wo (ReLU, T5 v1.0)."""
+    return 3 if getattr(spec, "feed_forward_proj", "gated-gelu") == "gated-gelu" else 2
+
+
 def step_weight_elements(spec) -> int:
-    """W_step: decoder weights read once per decode step (self q,k,v,o + cross q,o + wi_0,wi_1,wo per layer, + lm_head);
-    the cross k,v projections are prefill-only."""
+    """W_step: decoder weights read once per decode step (self q,k,v,o + cross q,o + the feed-forward matrices per layer,
+    + lm_head); the cross k,v projections are prefill-only."""
     d, inner, f = spec.d_model, spec.inner_dim, spec.d_ff
-    return spec.num_decoder_layers * (4 * d * inner + 2 * d * inner + 3 * d * f) + spec.vocab_size * d
+    return spec.num_decoder_layers * (4 * d * inner + 2 * d * inner + ff_matrices(spec) * d * f) + spec.vocab_size * d
 
 
 def decode_bytes(spec, batch: int, steps: int, extents: Optional[Iterable[int]] = None, seq: Optional[int] = None,
@@ -52,19 +57,20 @@ def encoder_flops(spec, batch: int, extents: Optional[Iterable[int]] = None, seq
     sum_s = float(sum(ext))
     sum_s2 = float(sum(e * e for e in ext))
     d, inner, f = spec.d_model, spec.inner_dim, spec.d_ff
-    return (2.0 * spec.num_layers * (4 * d * inner + 3 * d * f) * sum_s + spec.num_layers * 4.0 * sum_s2 * inner
+    return (2.0 * spec.num_layers * (4 * d * inner + ff_matrices(spec) * d * f) * sum_s + spec.num_layers * 4.0 * sum_s2 * inner
             + 2.0 * spec.num_decoder_layers * 2.0 * d * inner * sum_s)
 
 
 def decoder_forward_flops(spec, batch: int, T: int, extents: Optional[Iterable[int]] = None, seq: Optional[int] = None) -> float:
     """The teacher-forced forward pass's decoder + lm_head FLOPs (b200t5_forward), T label positions per row: per layer
-    and position the QKV, output, cross-query, cross-output and GeGLU products (2 (6 d I + 3 d F)); causal self-attention
+    and position the QKV, output, cross-query, cross-output and feed-forward products (2 (6 d I + 3 d F) with GeGLU,
+    2 (6 d I + 2 d F) with ReLU); causal self-attention
     Q.K and P.V over the keys j <= i (4 I (i + 1)); cross-attention over the row's extent (4 I S_b); the lm_head
     (2 d V per position). The encoder and the cross-K/V projection are encoder_flops."""
     ext = list(extents) if extents is not None else [seq] * batch
     d, inner, f, ld = spec.d_model, spec.inner_dim, spec.d_ff, spec.num_decoder_layers
     rows = float(batch) * T
-    gemm = rows * (ld * 2.0 * (6 * d * inner + 3 * d * f) + 2.0 * d * spec.vocab_size)
+    gemm = rows * (ld * 2.0 * (6 * d * inner + ff_matrices(spec) * d * f) + 2.0 * d * spec.vocab_size)
     attn = ld * (batch * 2.0 * inner * T * (T + 1) + 4.0 * inner * T * float(sum(ext)))
     return gemm + attn
 

@@ -1,4 +1,4 @@
-"""Seeded synthetic assets: FLAN-T5-shaped checkpoints, Alpaca-schema prompts, token batches.
+"""Seeded synthetic assets: FLAN-T5- and T5 v1.0-shaped checkpoints, Alpaca-schema prompts, token batches.
 
 No FLAN-T5 weights, tokenizer model or Alpaca data exist offline (SURVEY section 0), so every
 parity and benchmark input is generated here from numpy seeds. Checkpoints are written in the
@@ -66,10 +66,19 @@ class T5Spec:
     # numerically chaotic - stock transformers bf16 on GPU and on CPU rarely agree on an arg-max - so no
     # implementation can be compared with another one on it.
     q_init_gain: float = 1.0
+    # the architecture: FLAN-T5 / T5 v1.1 ("gated-gelu", untied lm_head) by default; the original T5 v1.0 family is
+    # "relu" with tie_word_embeddings True: no lm_head.weight, and transformers scales the decoder output by
+    # d_model ** -0.5 before the shared embedding is applied as the head (configuration_t5.py:82)
+    feed_forward_proj: str = "gated-gelu"
+    tie_word_embeddings: bool = False
 
     @property
     def inner_dim(self) -> int:
         return self.num_heads * self.d_kv
+
+    @property
+    def gated(self) -> bool:
+        return self.feed_forward_proj == "gated-gelu"
 
     def hf_config(self) -> dict:
         return {
@@ -87,12 +96,12 @@ class T5Spec:
             "layer_norm_epsilon": self.layer_norm_epsilon,
             "dropout_rate": 0.1,
             "initializer_factor": 1.0,
-            "feed_forward_proj": "gated-gelu",
-            "dense_act_fn": "gelu_new",
-            "is_gated_act": True,
+            "feed_forward_proj": self.feed_forward_proj,
+            "dense_act_fn": "gelu_new" if self.gated else "relu",
+            "is_gated_act": self.gated,
             "is_encoder_decoder": True,
             "use_cache": True,
-            "tie_word_embeddings": False,
+            "tie_word_embeddings": self.tie_word_embeddings,
             "pad_token_id": self.pad_token_id,
             "eos_token_id": self.eos_token_id,
             "decoder_start_token_id": self.decoder_start_token_id,
@@ -108,6 +117,19 @@ SPECS: Dict[str, T5Spec] = {
     "flan-t5-small": T5Spec("flan-t5-small", d_model=512, d_ff=1024, num_heads=6, num_layers=8, num_decoder_layers=8),
     "flan-t5-base": T5Spec("flan-t5-base", d_model=768, d_ff=2048, num_heads=12, num_layers=12, num_decoder_layers=12),
     "flan-t5-large": T5Spec("flan-t5-large", d_model=1024, d_ff=2816, num_heads=16, num_layers=24, num_decoder_layers=24),
+    # the original T5 (v1.0): ReLU feed-forward, tied and rescaled head. Test sizes of the tiny / mini shapes (with an
+    # untied variant: a v1.0 config saying tie_word_embeddings: false keeps its lm_head and is not rescaled), then the
+    # t5-small and t5-base shapes (60.5 M / 222.9 M parameters)
+    "t5-tiny": T5Spec("t5-tiny", vocab_size=384, d_model=128, d_ff=256, num_heads=2, num_layers=2, num_decoder_layers=2,
+                      feed_forward_proj="relu", tie_word_embeddings=True),
+    "t5-tiny-untied": T5Spec("t5-tiny-untied", vocab_size=384, d_model=128, d_ff=256, num_heads=2, num_layers=2,
+                             num_decoder_layers=2, feed_forward_proj="relu"),
+    "t5-mini": T5Spec("t5-mini", vocab_size=1000, d_model=256, d_ff=512, num_heads=3, num_layers=3, num_decoder_layers=2,
+                      feed_forward_proj="relu", tie_word_embeddings=True),
+    "t5-small": T5Spec("t5-small", d_model=512, d_ff=2048, num_heads=8, num_layers=6, num_decoder_layers=6,
+                       feed_forward_proj="relu", tie_word_embeddings=True),
+    "t5-base": T5Spec("t5-base", d_model=768, d_ff=3072, num_heads=12, num_layers=12, num_decoder_layers=12,
+                      feed_forward_proj="relu", tie_word_embeddings=True),
 }
 
 
@@ -115,7 +137,9 @@ def param_names(spec: T5Spec) -> Dict[str, Tuple[int, ...]]:
     """HF state-dict keys and shapes (SURVEY Appendix G); nn.Linear layout [out, in]."""
     d, I, F, V, H = spec.d_model, spec.inner_dim, spec.d_ff, spec.vocab_size, spec.num_heads
     nb = spec.relative_attention_num_buckets
-    out: Dict[str, Tuple[int, ...]] = {"shared.weight": (V, d), "lm_head.weight": (V, d)}
+    out: Dict[str, Tuple[int, ...]] = {"shared.weight": (V, d)}
+    if not spec.tie_word_embeddings:
+        out["lm_head.weight"] = (V, d)
     for side, n_layers in (("encoder", spec.num_layers), ("decoder", spec.num_decoder_layers)):
         for i in range(n_layers):
             p = f"{side}.block.{i}.layer"
@@ -132,8 +156,11 @@ def param_names(spec: T5Spec) -> Dict[str, Tuple[int, ...]]:
                 out[f"{p}.1.EncDecAttention.o.weight"] = (d, I)
                 out[f"{p}.1.layer_norm.weight"] = (d,)
                 ff = 2
-            out[f"{p}.{ff}.DenseReluDense.wi_0.weight"] = (F, d)
-            out[f"{p}.{ff}.DenseReluDense.wi_1.weight"] = (F, d)
+            if spec.gated:
+                out[f"{p}.{ff}.DenseReluDense.wi_0.weight"] = (F, d)
+                out[f"{p}.{ff}.DenseReluDense.wi_1.weight"] = (F, d)
+            else:
+                out[f"{p}.{ff}.DenseReluDense.wi.weight"] = (F, d)
             out[f"{p}.{ff}.DenseReluDense.wo.weight"] = (d, F)
             out[f"{p}.{ff}.layer_norm.weight"] = (d,)
         out[f"{side}.final_layer_norm.weight"] = (d,)
@@ -146,15 +173,28 @@ def make_state_dict(spec: T5Spec, seed: int = 0, eos_boost: float = 2.5) -> Dict
     Scales follow T5's own initialisation (modeling_t5.py:_init_weights; query projections times
     spec.q_init_gain) except that the untied lm_head is N(0, d^-1/2) with the EOS row boosted, which
     gives varied output lengths instead of the degenerate all-pad generations of the default init (SURVEY 8c).
+
+    A tied checkpoint (T5 v1.0) has no lm_head: its logits are the final norm's output (unit RMS) times d^-1/2, against
+    the rows of the N(0, 1) shared embedding, so they have the same unit scale as the untied head's, and the EOS row
+    of the shared embedding takes the boost instead. Greedy decoding then sees the same logit statistics - top-1 /
+    top-2 gaps, EOS rate - as on the FLAN-T5 specs. (N(0, 1) logits without the rescale would be d^1/2 times wider.)
+    One more change makes that hold: the residual stream carries the embedding of the token just read, so with the
+    usual final-norm weights near 1 that token's own logit would be about d^1/2 times the others' spread and greedy
+    decoding would repeat its input forever. The tied specs draw the final decoder norm's weights N(0, 1) instead:
+    zero-mean, the token's own logit is no longer biased upwards (its spread is about 3^1/2 times the others').
     """
     rng = np.random.default_rng(seed)
     d, I, F = spec.d_model, spec.inner_dim, spec.d_ff
     sd: Dict[str, np.ndarray] = {}
     for name, shape in param_names(spec).items():
-        if name.endswith("layer_norm.weight"):
+        if name == "decoder.final_layer_norm.weight" and spec.tie_word_embeddings:
+            w = rng.standard_normal(shape)
+        elif name.endswith("layer_norm.weight"):
             w = 1.0 + 0.1 * rng.standard_normal(shape)
         elif name == "shared.weight":
             w = rng.standard_normal(shape)
+            if spec.tie_word_embeddings:
+                w[spec.eos_token_id] *= eos_boost
         elif name == "lm_head.weight":
             w = rng.standard_normal(shape) * d ** -0.5
             w[spec.eos_token_id] *= eos_boost
@@ -162,7 +202,7 @@ def make_state_dict(spec: T5Spec, seed: int = 0, eos_boost: float = 2.5) -> Dict
             w = rng.standard_normal(shape) * 0.5
         elif ".q.weight" in name:
             w = rng.standard_normal(shape) * (d * spec.d_kv) ** -0.5 * spec.q_init_gain
-        elif ".k.weight" in name or ".v.weight" in name or "wi_" in name:
+        elif ".k.weight" in name or ".v.weight" in name or "wi_" in name or ".wi.weight" in name:
             w = rng.standard_normal(shape) * d ** -0.5
         elif ".o.weight" in name:
             w = rng.standard_normal(shape) * I ** -0.5
@@ -258,6 +298,8 @@ def spec_from_config(cfg: dict, name: str = "from-config") -> T5Spec:
         layer_norm_epsilon=cfg.get("layer_norm_epsilon", 1e-6),
         pad_token_id=cfg.get("pad_token_id", 0), eos_token_id=cfg.get("eos_token_id", 1),
         decoder_start_token_id=cfg.get("decoder_start_token_id", cfg.get("pad_token_id", 0)),
+        feed_forward_proj=cfg.get("feed_forward_proj", "relu"),
+        tie_word_embeddings=cfg.get("tie_word_embeddings", True) is not False,
     )
 
 

@@ -1,6 +1,8 @@
 /*
- * b200t5.h - C ABI of libb200t5.so: FLAN-T5 (T5 v1.1, gated-GELU) greedy generation on one
- * NVIDIA H100 (sm_90a), the hot path of the workshop's batch-inference loop.
+ * b200t5.h - C ABI of libb200t5.so: T5 greedy generation on one NVIDIA H100 (sm_90a), the hot path of the
+ * workshop's batch-inference loop. Two T5 architectures load: FLAN-T5 / T5 v1.1 (gated-GELU feed-forward, untied
+ * lm_head) and the original T5 v1.0 (t5-small / t5-base / t5-large and their fine-tunes: ReLU feed-forward, lm_head
+ * tied to the shared embedding, decoder output scaled by d_model ** -0.5). d_kv must be 64 (not t5-3b / t5-11b).
  *
  * What this boundary replaces in the reference (ray-project/anyscale-workshop-nyc-2023):
  * the reference has no FFI of its own; its plug-in seam is the Python attribute
@@ -70,8 +72,11 @@ typedef struct b200t5_config {
   int32_t pad_token_id;                     /* 0 */
   int32_t eos_token_id;                     /* 1 */
   int32_t decoder_start_token_id;           /* 0 */
-  int32_t is_gated_gelu;          /* must be 1 (feed_forward_proj == "gated-gelu") */
-  int32_t scale_decoder_outputs;  /* must be 0 (tie_word_embeddings == false checkpoints) */
+  int32_t is_gated_gelu;          /* 1: feed_forward_proj "gated-gelu" (T5 v1.1 / FLAN-T5: wi_0, wi_1, wo);
+                                   * 0: "relu" (T5 v1.0: wi, wo). Any other value: B200T5_EINVAL */
+  int32_t scale_decoder_outputs;  /* 1: the final decoder norm's output is multiplied by fp32(d_model ** -0.5) and
+                                   * rounded once more before the lm_head (transformers: unless the checkpoint's config
+                                   * says tie_word_embeddings: false); 0: not. Any other value: B200T5_EINVAL */
 } b200t5_config;
 
 /* Greedy-generation controls: the subset of GenerationConfig the reference path uses
@@ -147,7 +152,9 @@ int b200t5_create(const b200t5_config* cfg, int device, b200t5_handle* out);
  * Unknown names that HF also ignores are accepted and dropped. */
 int b200t5_set_weight(b200t5_handle h, const char* name, const void* dev_ptr, int dtype, const int64_t* shape,
                       int ndim);
-/* Checks that every required tensor arrived, repacks (QKV concat, GeGLU interleave, cross-KV concat). */
+/* Checks that every required tensor arrived, repacks (QKV concat, GeGLU interleave, cross-KV concat). A ReLU model
+ * (is_gated_gelu 0) takes {encoder,decoder}.block.*.layer.*.DenseReluDense.wi.weight [d_ff, d_model] in place of
+ * wi_0 / wi_1. Without lm_head.weight the lm_head is shared.weight (tied). */
 int b200t5_finalize(b200t5_handle h);
 int b200t5_destroy(b200t5_handle h);
 const char* b200t5_last_error(b200t5_handle h);
@@ -395,21 +402,24 @@ int b200t5_relative_bucket(int relative_position, int bidirectional, int num_buc
 /* C[M,N] = act(A[M,K] W[N,K]^T) via the wgmma GEMM in one of the configurations the library launches:
  * bn = 512, the encoder configuration (128 x 256 tiles, weight in 128-row boxes) with mode 0 plain, 1 += residual R
  * (in C), 5 += residual as in decoder / encoder layer 0 (fp16 build: C = fp16(R + fp16(acc)), where mode 1 is
- * C = R + fp16(acc); bf16 build: same as 1), 2 GeGLU (W rows interleaved per 128, C is [M,N/2]); or bn = 128 with
- * mode 3, the fp32 logits of b200t5_decode_logits (C is float*). Anything else returns B200T5_EINVAL. pow_mode: the
- * gelu table's (bf16 build; the fp16 build's epilogue has no table). */
+ * C = R + fp16(acc); bf16 build: same as 1), 2 GeGLU (W rows interleaved per 128, C is [M,N/2]), 6 ReLU
+ * (C = relu(act(acc)) in the GeGLU output's type: the T5 v1.0 feed-forward input); or bn = 128 with mode 3, the fp32
+ * logits of b200t5_decode_logits (C is float*), or mode 6, the ReLU product as the forward pass runs it (128 x 128
+ * tiles). Anything else returns B200T5_EINVAL. pow_mode: the gelu table's (bf16 build; the fp16 build's epilogue has
+ * no table). */
 int b200t5_test_gemm(int device, const void* A, const void* W, void* C, int M, int N, int K, int bn, int mode,
                      int pow_mode, void* stream);
 /* The 128 x 256 encoder GEMM as the encoder launches it; kernel 0 = the kernel whose epilogue follows each main loop,
  * 1 = the epilogue-overlapped kernel (option "enc_gemm"). mode 0 plain, 1 and 5 += residual R (in C), 2 GeGLU (W rows
- * interleaved per 128, C is [M,N/2]), 3 cross-attention K/V scatter: C is the arena [N/(H*64)][B][H][S][64] and row m
+ * interleaved per 128, C is [M,N/2]), 6 ReLU (as b200t5_test_gemm), 3 cross-attention K/V scatter: C is the arena [N/(H*64)][B][H][S][64] and row m
  * is position row_s[m] of prompt row_b[m] (both NULL: m = b*S + s, M = B*S). B, H, S are read in mode 3 only. */
 int b200t5_test_enc_gemm(int device, const void* A, const void* W, void* C, int M, int N, int K, int kernel, int mode,
                          int pow_mode, const int* row_b, const int* row_s, int B, int H, int S, void* stream);
 /* Same contract through the cluster split-K kernel the decode step uses (csrc/gemm_splitk.cuh):
  * bn in {64,128}; split in {1,2,4,8} CTAs per cluster along K (reduced automatically when K has
- * fewer 64-wide k-blocks); mode 0 plain, 1 and 5 += residual (in C), 2 GeGLU, 4 decoder QKV: C is the q
- * buffer [M, N/3] and `aux` the self-KV cache [2][M][H][Tmax][64] whose row `step` is written. */
+ * fewer 64-wide k-blocks); mode 0 plain, 1 and 5 += residual (in C), 2 GeGLU, 6 ReLU (as b200t5_test_gemm),
+ * 4 decoder QKV: C is the q buffer [M, N/3] and `aux` the self-KV cache [2][M][H][Tmax][64] whose row `step` is
+ * written. */
 int b200t5_test_gemm_splitk(int device, const void* A, const void* W, void* C, int M, int N, int K, int bn, int split,
                             int mode, int pow_mode, void* aux, int Tmax, int step, void* stream);
 /* fp16 build (libb200t5_f16.so) only: the fp32-weight feed-forward output projection (transformers keeps T5's `wo`
@@ -419,6 +429,10 @@ int b200t5_test_gemm_splitk(int device, const void* A, const void* W, void* C, i
 int b200t5_test_ffo(int device, const void* A, const void* W, void* R, int M, int N, int F, int kernel, int bn, int split,
                     void* stream);
 int b200t5_test_rmsnorm(int device, const void* x, const void* w, void* y, int M, int d, float eps, void* stream);
+/* The final decoder norm of a scale_decoder_outputs model: y = act(float(act(w * act(x * rsqrt(var + eps)))) * scale),
+ * the last product in fp32 (scale = fp32(d_model ** -0.5) in the model). scale == 0 returns B200T5_EINVAL. */
+int b200t5_test_rmsnorm_scaled(int device, const void* x, const void* w, void* y, int M, int d, float eps, float scale,
+                               void* stream);
 /* Decoder self-attention: self == 3 the 4-warp-per-(row, head) kernel the decode step runs; keys = t+1 with t = step, or, when extent is not NULL, t = extent[b] (int32 [B]: the
  * slot pool's per-row positions); dist_bias float [H][Tk]. Cross-attention: self == 0: extent int32 [B], key_ok uint8 [B][Tk];
  * self == 2: as 0 through the TMA stream kernel (csrc/attention_cross_stream.cuh), `step` = ring stages (0: 5);
